@@ -772,8 +772,8 @@ def test_conv2d_im2col_gemm_engine(nk, dev, O, xs, cout, k, stride, dil):
         O.conv_backward_kernel(ww, g, x, stride, dil)
         wx = wx + gx
         sx = float(np.sqrt((gx.astype(np.float64) ** 2).mean())) + 1e-9
-        # dX: the column gradients are rounded to bf16 before col2im sums up to kh*kw of them
-        assert np.all(np.abs(dx.as_ndarray() - wx) <= 1.5e-2 * sx + 2.0 ** -7 * np.abs(wx)), beta
+        # dX: the column gradients stay in f32 through col2im, so each element is rounded to bf16 once
+        assert np.all(np.abs(dx.as_ndarray() - wx) <= 2e-3 * sx + (2.0 ** -7 if beta else 2.0 ** -8) * np.abs(wx) + 1e-6), beta
         sw_ = float(np.sqrt(((ww - (dw0 if beta else 0)) ** 2).mean())) + 1e-9
         assert np.all(np.abs(dw.as_ndarray() - ww) <= 2e-3 * sw_ + 1e-5 * np.abs(ww)), beta
         assert np.allclose(db.as_ndarray().ravel(), g.astype(np.float64).sum((0, 2, 3)), rtol=1e-4, atol=1e-3)
