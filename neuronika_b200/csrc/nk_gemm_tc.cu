@@ -11,9 +11,17 @@
 // Structure (persistent over 128 x BLOCK_N output tiles, one CTA per SM, three warpgroups):
 //   warpgroup 0    : TMA producer (one thread) -- cp.async.bulk.tensor 128B-swizzled boxes into a kStages smem ring
 //   warpgroups 1-2 : consumers -- each runs wgmma m64nBLOCK_Nk16 on its 64 rows of the tile with the accumulator in
-//                    registers, then drains it through a swizzled shared-memory stage: alpha/bias/ReLU, mask, beta,
-//                    column sums, reduce-scatter over NVLink and batched outputs as 16-byte global stores per row
-// Pipeline: smem full/empty mbarriers (TMA <-> the two consumer warpgroups).
+//                    registers, keeping one k-block's wgmma group in flight: it issues k-block k, waits for k-1's group
+//                    (wgmma.wait_group 1) and only then releases k-1's ring slot, so the tensor pipe never drains
+//                    between k-blocks (the consumer holds two slots; the producer prefetches kStages - 2 ahead).
+//                    Then the epilogue, one of two:
+//                    - TMA store (column bias, alpha, ReLU, beta == 0, no mask / column sums / reduce-scatter, C
+//                      TMA-addressable): the fragments are converted to C's type straight into one of two 128B-swizzled
+//                      64-row x 128-byte staging buffers per warpgroup and written by cp.async.bulk.tensor stores that
+//                      drain while the warpgroup already runs the next tile's main loop;
+//                    - the drain: through a swizzled shared-memory stage, alpha/bias/ReLU, mask, beta, column sums,
+//                      reduce-scatter over NVLink and batched outputs as 16-byte global stores per row.
+// Pipeline: smem full/empty mbarriers (TMA <-> the two consumer warpgroups); bulk async-groups for the output stores.
 #include "nk_internal.cuh"
 #include "nk_ptx.cuh"
 
@@ -56,6 +64,7 @@ struct GemmParams {
   // `splits` CTAs per tile, which add their partial sums into C with f32 atomics (C zeroed / scaled by the host).
   int batch, a_batched, b_batched, batch_reduce, splits;
   int64_t c_batch_stride;
+  int tma_store;   // the epilogue writes C through the C tensor map (see the header); the host checks the conditions
 };
 
 __device__ __forceinline__ int tile_m_block(const GemmParams& p, int tile) {
@@ -96,11 +105,13 @@ struct Cfg {
   static constexpr uint32_t SMEM_BYTES = kStages * STAGE_BYTES + 2048 + kEpiStageBytes;  // + alignment slack + barriers
 };
 
-// v[j] = alpha * acc[j] + bias (row- or column-indexed) for one 32-column chunk of one output row
+// v[j] = alpha * acc[j] + bias (row- or column-indexed) for one 32-column chunk of one output row.  The product is
+// rounded before the bias is added (__fmul_rn: never contracted into an FMA), in every epilogue, so that all of them
+// store the same bits
 __device__ __forceinline__ void scale_and_bias(const GemmParams& p, int64_t row, int64_t col0, const uint32_t* r, bool full,
                                                float* v) {
 #pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = p.alpha * __uint_as_float(r[j]);
+  for (int j = 0; j < 32; ++j) v[j] = __fmul_rn(p.alpha, __uint_as_float(r[j]));
   if (p.bias && p.bias_per_row) {
     const float b = p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[row]) : static_cast<const float*>(p.bias)[row];
 #pragma unroll
@@ -255,11 +266,30 @@ __device__ __forceinline__ int epi_index(int row, int col) {
   return row * kEpiCols + ((((col >> 2) ^ (row & 7))) << 2) + (col & 3);
 }
 
+// bias[col] of the column-indexed bias, 0 past the last column
+__device__ __forceinline__ float col_bias(const GemmParams& p, int64_t col) {
+  if (col >= p.N) return 0.f;
+  return p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[col]) : static_cast<const float*>(p.bias)[col];
+}
+
+// one output value of the TMA-store epilogue: the drain's alpha (rounded product), bias and ReLU
+__device__ __forceinline__ float epi_value(const GemmParams& p, float acc, float bias) {
+  float v = __fmul_rn(p.alpha, acc);
+  if (p.bias) v += bias;
+  return p.relu ? (v > 0.f ? v : 0.f) : v;
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+               const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
   using C_ = Cfg<BLOCK_N>;
   constexpr int kStages = C_::kStages;
+  // TMA-store epilogue: chunks of one 128-byte swizzle row (64 bf16 / 32 f32 columns) x 64 rows, two 8 KB staging
+  // buffers per consumer warpgroup in its half of the epilogue stage
+  constexpr int kStoreCols = 128 / int(sizeof(TC));
+  constexpr bool kTmaStore = !BATCH && BLOCK_N % kStoreCols == 0;
+  static_assert(2 * 2 * 64 * 128 <= kEpiStageBytes, "staging buffers");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms: 1024 B aligned
   const uint32_t smem_a0 = smem_base;
@@ -276,6 +306,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
+    if (kTmaStore && p.tma_store) ptx::prefetch_tmap(&tmap_c);
     for (int s = 0; s < kStages; ++s) {
       ptx::mbar_init(full_bar(s), 1);
       ptx::mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
@@ -366,6 +397,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   float acc[BLOCK_N / 2];
   int stage = 0;
   uint32_t phase = 0;
+  uint32_t store_buf = 0;   // TMA-store epilogue: the staging buffer the next chunk goes to
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int m_blk, n_blk;
     tile_coords(p, BATCH ? tile % tiles_mn : tile, m_blk, n_blk);
@@ -375,6 +407,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       batch_range(tile / tiles_mn, b0, b1);
       k_total *= (b1 - b0);
     }
+    int prev_stage = 0;
     for (int kb = 0; kb < k_total; ++kb) {
       ptx::mbar_wait_spin(full_bar(stage), phase);
       const uint64_t adesc = ptx::make_smem_desc_sw128(smem_a0 + stage * C_::A_BYTES + a_off, p.a_lbo, p.a_sbo);
@@ -386,12 +419,63 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         ptx::Wgmma<BLOCK_N>::template mma<int(A_MN), int(B_MN)>(acc, adesc + uint64_t((k * p.a_kstep) >> 4),
                                                                  bdesc + uint64_t((k * p.b_kstep) >> 4), (kb | k) != 0 ? 1u : 0u);
       ptx::wgmma_commit();
-      ptx::wgmma_wait<0>();
+      ptx::wgmma_wait<1>();   // k-block kb - 1's group is done; kb's stays in flight
       ptx::fence_regs(acc);
-      if (t == 0) ptx::mbar_arrive(empty_bar(stage));  // this warpgroup is done reading the slot
+      if (kb > 0 && t == 0) ptx::mbar_arrive(empty_bar(prev_stage));  // this warpgroup is done reading kb - 1's slot
+      prev_stage = stage;
       if (++stage == kStages) {
         stage = 0;
         phase ^= 1u;
+      }
+    }
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(acc);
+    if (t == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+
+    if constexpr (kTmaStore) {
+      if (p.tma_store) {
+        // ---- TMA-store epilogue: chunk ch = columns [ch kStoreCols, +kStoreCols) of this warpgroup's 64 rows.  Thread
+        // (warp w, lane) holds rows fr, fr + 8 and columns 8 jj + 2 (lane & 3) + {0, 1} of each 8-column block jj; it
+        // writes them, converted, to the 128B-swizzled layout of the C tensor map's box (16-byte unit u of row r at
+        // unit u ^ (r & 7); conflict-free: the eight rows of a warp's store hit eight different units)
+        const int fr = warp * 16 + (lane >> 2);
+        const int q = lane & 3;
+        const int row0 = m_blk * BLOCK_M + cw * 64;
+        const uint32_t stg0 = epi_stage + uint32_t(cw) * (2 * 64 * 128);
+#pragma unroll
+        for (int ch = 0; ch < BLOCK_N / kStoreCols; ++ch) {
+          const uint32_t buf = stg0 + store_buf * (64 * 128);
+          if (t == 0) ptx::tma_store_wait_read<1>();   // the store that last read this buffer is done with it
+          ptx::named_barrier(1 + cw, 128);
+          const int64_t col0 = int64_t(n_blk) * BLOCK_N + ch * kStoreCols;
+#pragma unroll
+          for (int jj = 0; jj < kStoreCols / 8; ++jj) {
+            const int j = (ch * (kStoreCols / 8) + jj) * 4;   // acc[j..j+1]: row fr, acc[j+2..j+3]: row fr + 8
+            const int64_t col = col0 + jj * 8 + 2 * q;
+            float b0 = 0.f, b1 = 0.f;
+            if (p.bias) b0 = col_bias(p, col), b1 = col_bias(p, col + 1);
+            const float v0 = epi_value(p, acc[j], b0), v1 = epi_value(p, acc[j + 1], b1);
+            const float v2 = epi_value(p, acc[j + 2], b0), v3 = epi_value(p, acc[j + 3], b1);
+            if constexpr (sizeof(TC) == 2) {
+              const uint32_t off = fr * 128 + ((jj ^ (fr & 7)) << 4) + 4 * q;
+              const __nv_bfloat162 lo = __floats2bfloat162_rn(v0, v1), hi = __floats2bfloat162_rn(v2, v3);
+              ptx::st_shared_b32(buf + off, *reinterpret_cast<const uint32_t*>(&lo));
+              ptx::st_shared_b32(buf + off + 8 * 128, *reinterpret_cast<const uint32_t*>(&hi));
+            } else {
+              const uint32_t off = fr * 128 + (((2 * jj + (q >> 1)) ^ (fr & 7)) << 4) + (q & 1) * 8;
+              ptx::st_shared_v2_f32(buf + off, v0, v1);
+              ptx::st_shared_v2_f32(buf + off + 8 * 128, v2, v3);
+            }
+          }
+          ptx::fence_proxy_async();   // the staged chunk is visible to the TMA unit ...
+          ptx::named_barrier(1 + cw, 128);
+          if (t == 0) {               // ... which clips the box at M, N (the ldc - N gap is never written)
+            if (row0 < p.M && col0 < p.N) ptx::tma_store_2d(&tmap_c, buf, int(col0), row0);
+            ptx::tma_store_commit();   // (an empty group when nothing was issued: one group per chunk)
+          }
+          store_buf ^= 1u;
+        }
+        continue;   // the stores drain while the next tile's main loop runs
       }
     }
 
@@ -434,7 +518,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           for (int c = lane; c < chunk_cols; c += 32) {
             const int64_t col = col_base + c;
             if (col >= p.N) break;
-            float v = p.alpha * stg[epi_index(srow, c)];
+            float v = __fmul_rn(p.alpha, stg[epi_index(srow, c)]);
             TC* cp = static_cast<TC*>(p.C) + c_off + grow * p.ldc + col;
             if (atomic) {
               if constexpr (sizeof(TC) == 4) atomicAdd(reinterpret_cast<float*>(cp), v);
@@ -468,22 +552,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       }
     }
   }
+  if (kTmaStore && p.tma_store && t == 0) ptx::tma_store_wait<0>();   // the staging buffers outlive the last stores
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// 2-D bf16 tensor map: `rows` x `cols` row-major with leading dimension ld, box (box_cols=64, box_rows)
+// 2-D tensor map (bf16 or f32 elements): `rows` x `cols` row-major with leading dimension ld, box (box_cols, box_rows)
+// with box_cols elements = 128 bytes, 128B-swizzled
 int make_tmap_2d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t rows, int64_t cols, int64_t ld,
-                 uint32_t box_cols, uint32_t box_rows) {
+                 uint32_t box_cols, uint32_t box_rows, int dtype = NK_BF16) {
   if (!ctx->encode_tiled) return nk_set_error(ctx, NK_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * nk_dtype_size(dtype)};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = reinterpret_cast<EncodeTiledFn>(ctx->encode_tiled)(
-      tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+      tm, dtype == NK_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+      const_cast<void*>(base), dims, strides, box, estr,
       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
@@ -493,7 +580,7 @@ int make_tmap_2d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t rows, i
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false>
-int launch_cfg(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, GemmParams& p) {
+int launch_cfg(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, GemmParams& p) {
   using C_ = Cfg<BLOCK_N>;
   auto kern = gemm_tc_kernel<BLOCK_N, A_MN, B_MN, TC, BATCH>;
   static bool attr_done[64] = {};  // per template instantiation and device (the attribute is per device)
@@ -526,7 +613,7 @@ int launch_cfg(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, GemmPa
     if (BLOCK_N != 256 || sizeof(TC) != 4 || p.N % 4 != 0)
       return nk_set_error(ctx, NK_ERR_UNSUPPORTED, "wgmma gemm: reduce-scatter epilogue needs 128x256 tiles, f32, N %% 4 == 0");
   }
-  kern<<<grid, kNumThreads, smem, ctx->stream>>>(ta, tb, p);
+  kern<<<grid, kNumThreads, smem, ctx->stream>>>(ta, tb, tc, p);
   ctx->launches++;
   cudaError_t le = cudaGetLastError();
   if (le != cudaSuccess)
@@ -537,15 +624,15 @@ int launch_cfg(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, GemmPa
 }
 
 template <bool A_MN, bool B_MN, typename TC>
-int launch_bn(nk_ctx* ctx, int block_n, const CUtensorMap& ta, const CUtensorMap& tb, GemmParams& p) {
+int launch_bn(nk_ctx* ctx, int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, GemmParams& p) {
   switch (block_n) {
-    case 256: return launch_cfg<256, A_MN, B_MN, TC>(ctx, ta, tb, p);
-    case 128: return launch_cfg<128, A_MN, B_MN, TC>(ctx, ta, tb, p);
-    case 64: return launch_cfg<64, A_MN, B_MN, TC>(ctx, ta, tb, p);
+    case 256: return launch_cfg<256, A_MN, B_MN, TC>(ctx, ta, tb, tc, p);
+    case 128: return launch_cfg<128, A_MN, B_MN, TC>(ctx, ta, tb, tc, p);
+    case 64: return launch_cfg<64, A_MN, B_MN, TC>(ctx, ta, tb, tc, p);
     default:
       if (!B_MN) {
-        if (block_n == 32) return launch_cfg<32, A_MN, false, TC>(ctx, ta, tb, p);
-        if (block_n == 16) return launch_cfg<16, A_MN, false, TC>(ctx, ta, tb, p);
+        if (block_n == 32) return launch_cfg<32, A_MN, false, TC>(ctx, ta, tb, tc, p);
+        if (block_n == 16) return launch_cfg<16, A_MN, false, TC>(ctx, ta, tb, tc, p);
       }
       return nk_set_error(ctx, NK_ERR_UNSUPPORTED, "wgmma gemm: unsupported BLOCK_N %d", block_n);
   }
@@ -634,6 +721,19 @@ int nk_gemm_wgmma(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int
   else
     rc = make_tmap_2d(ctx, &tb, B, N, K, ldb, BLOCK_K, (uint32_t)block_n);
   if (rc) return rc;
+  // TMA-store epilogue: an output the epilogue only writes (beta 0; alpha, column bias and ReLU are applied on the way)
+  // and that TMA can address; box = one 64-row x 128-byte staging buffer, whole chunks per tile.  The rows must also end
+  // on a 16-byte boundary: a store box clips at the last row exactly but at the last column only to the 16-byte unit
+  // that holds it, which would write into the ldc - N gap
+  const int64_t c_size = int64_t(nk_dtype_size(c_dtype));
+  CUtensorMap tc;
+  memset(&tc, 0, sizeof(tc));
+  p.tma_store = beta == 0.f && !mask && !colsum && !p.rs_world && (block_n * c_size) % 128 == 0 &&
+                (reinterpret_cast<uintptr_t>(C) & 15) == 0 && (ldc * c_size) % 16 == 0 && (N * c_size) % 16 == 0;
+  if (p.tma_store) {
+    rc = make_tmap_2d(ctx, &tc, C, M, N, ldc, uint32_t(128 / c_size), 64, c_dtype);
+    if (rc) return rc;
+  }
 
   static const char* names[2][2][5] = {
       {{"wgmma_nt_128x256", "wgmma_nt_128x128", "wgmma_nt_128x64", "wgmma_nt_128x32", "wgmma_nt_128x16"},
@@ -644,8 +744,8 @@ int nk_gemm_wgmma(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int
   ctx->last_gemm_kernel = names[a_mn][b_mn][bi];
 
 #define NK_TC(AM, BM_)                                                              \
-  (c_dtype == NK_BF16 ? launch_bn<AM, BM_, __nv_bfloat16>(ctx, block_n, ta, tb, p) \
-                      : launch_bn<AM, BM_, float>(ctx, block_n, ta, tb, p))
+  (c_dtype == NK_BF16 ? launch_bn<AM, BM_, __nv_bfloat16>(ctx, block_n, ta, tb, tc, p) \
+                      : launch_bn<AM, BM_, float>(ctx, block_n, ta, tb, tc, p))
   if (!a_mn && !b_mn) return NK_TC(false, false);
   if (!a_mn && b_mn) return NK_TC(false, true);
   if (a_mn && !b_mn) return NK_TC(true, false);
@@ -695,6 +795,7 @@ int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_
   for (int i = 0; i < 8; ++i) p.rs_dst[i] = nullptr;
   p.batch = int(batch), p.a_batched = strideA != 0, p.b_batched = strideB != 0, p.batch_reduce = reduce ? 1 : 0, p.splits = 1;
   p.c_batch_stride = strideC;
+  p.tma_store = 0;   // batched outputs (and the row-indexed bias) keep the drain
   p.a_lbo = a_mn ? BLOCK_K * 128 : 16, p.a_sbo = 1024, p.a_kstep = a_mn ? WGMMA_K * 128 : WGMMA_K * 2;
   p.b_lbo = b_mn ? BLOCK_K * 128 : 16, p.b_sbo = 1024, p.b_kstep = b_mn ? WGMMA_K * 128 : WGMMA_K * 2;
   CUtensorMap ta, tb;
@@ -711,10 +812,12 @@ int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_
   else
     rc = b_mn ? make_tmap_2d(ctx, &tb, B, K, N, ldb, 64, BLOCK_K) : make_tmap_2d(ctx, &tb, B, N, K, ldb, BLOCK_K, (uint32_t)block_n);
   if (rc) return rc;
+  CUtensorMap tc;
+  memset(&tc, 0, sizeof(tc));
   ctx->last_gemm_kernel = "wgmma_batched";
 #define NK_TCB(BN, AM, BM_)                                                                          \
-  (c_dtype == NK_BF16 ? launch_cfg<BN, AM, BM_, __nv_bfloat16, true>(ctx, ta, tb, p)                  \
-                      : launch_cfg<BN, AM, BM_, float, true>(ctx, ta, tb, p))
+  (c_dtype == NK_BF16 ? launch_cfg<BN, AM, BM_, __nv_bfloat16, true>(ctx, ta, tb, tc, p)              \
+                      : launch_cfg<BN, AM, BM_, float, true>(ctx, ta, tb, tc, p))
 #define NK_TCB_BN(AM, BM_) (block_n == 256 ? NK_TCB(256, AM, BM_) : block_n == 128 ? NK_TCB(128, AM, BM_) : NK_TCB(64, AM, BM_))
   if (!a_mn && !b_mn) return NK_TCB_BN(false, false);
   if (!a_mn && b_mn) return NK_TCB_BN(false, true);
