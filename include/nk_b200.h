@@ -284,6 +284,35 @@ int nk_convnd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, co
 /* name of the kernel variant the last conv call used */
 const char* nk_last_conv_kernel(nk_ctx* ctx);
 
+/* ---- recurrent cells and `chunks` (SURVEY.md 8-f rank 4; csrc/nk_rnn.cu) ----
+ * The gate pre-activations are f32, written by the cell's own GEMMs; states, outputs and gradients have the cell's element
+ * type `dtype`; all maths is f32.  The backward entry points recompute the activations (and c') from the f32 gates.
+ * LSTM (neuronika-nn/src/lib.rs:510-540 with the intended gate assignment, SURVEY.md 8-c defect 7 = torch.nn.LSTMCell):
+ *   gates = x.W_ih^T + b_ih + h.W_hh^T + b_hh, (n, 4H), chunks [i | f | g | o] along the columns:
+ *   c' = sigmoid(f)*c + sigmoid(i)*tanh(g);  h' = sigmoid(o)*tanh(c').
+ * nk_lstm_cell_bwd writes dgates (beta 0, element type dgates_dtype) and dc_prev = beta_dc*dc_prev + sigmoid(f)*dc_total,
+ * dc_total = dc_out + dh_out*sigmoid(o)*(1 - tanh^2(c')).  dh_out / dc_out may be NULL (an output nobody used: zero
+ * gradient); dc_prev may be NULL (c not differentiable). */
+int nk_lstm_cell_fwd(nk_ctx* ctx, void* c_out, void* h_out, const float* gates, const void* c_prev, int64_t n,
+                     int64_t hidden, int dtype);
+int nk_lstm_cell_bwd(nk_ctx* ctx, void* dgates, int dgates_dtype, void* dc_prev, float beta_dc, const float* gates,
+                     const void* c_prev, const void* dh_out, const void* dc_out, int64_t n, int64_t hidden, int dtype);
+/* GRU (torch.nn.GRUCell = neuronika-nn/src/lib.rs:607-624): igates = x.W_ih^T + b_ih, hgates = h.W_hh^T + b_hh, (n, 3H)
+ * each, chunks [r | z | n]:  r = sigmoid(i_r + h_r); z = sigmoid(i_z + h_z); nn = tanh(i_n + r*h_n); h' = (h - nn)*z + nn.
+ * nk_gru_cell_bwd writes digates and dhgates (beta 0; they differ only in the n chunk) and the pointwise part of the
+ * hidden-state gradient, dh_prev = beta_dh*dh_prev + z*dh_out (dh_prev may be NULL). */
+int nk_gru_cell_fwd(nk_ctx* ctx, void* h_out, const float* igates, const float* hgates, const void* h_prev, int64_t n,
+                    int64_t hidden, int dtype);
+int nk_gru_cell_bwd(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, void* dh_prev, float beta_dh,
+                    const float* igates, const float* hgates, const void* h_prev, const void* dh_out, int64_t n,
+                    int64_t hidden, int dtype);
+/* chunks (chunk/mod.rs): y = block `index` of x in row-major block order (ndarray's exact_chunks: trailing partial blocks
+ * are dropped); a bit-exact copy.  Backward: dx[block] = beta*dx[block] + g, nothing else of dx is touched. */
+int nk_chunk_fwd(nk_ctx* ctx, void* y, const void* x, int ndim, const int64_t* x_shape, const int64_t* chunk_shape,
+                 int64_t index, int dtype);
+int nk_chunk_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* g, int g_dtype, int ndim, const int64_t* x_shape,
+                 const int64_t* chunk_shape, int64_t index, float beta);
+
 /* ---- SGD (neuronika-optim/src/sgd/mod.rs:191-231, penalty.rs:63-67) ----
  *   g' = grad_scale*g + 2*l2*w ; no momentum: w -= lr*g' ;
  *   momentum: buf = mu*buf + (1-damp)*g' ; w -= lr*(nesterov ? g' + mu*buf : buf).

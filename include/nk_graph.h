@@ -115,6 +115,21 @@ int nkg_vv(nkg_var* a, nkg_var* b, nkg_var** out);             /* vector_vector_
 int nkg_convolution_nd(nkg_var* kernel, nkg_var* input, int nsp, const int64_t* stride, const int64_t* dilation,
                        int64_t groups, nkg_var** out);
 
+/* ---- chunks and recurrent cells (SURVEY.md 8-f rank 4) ----
+ * nkg_chunks (var.rs:401-417): every block of ndarray's exact_chunks(chunk_shape) in row-major block order, one lazy
+ * node each (a bit-exact copy; backward adds into that block of the operand's gradient).  *count receives the number of
+ * blocks; nothing is recorded when it exceeds `capacity` (call with capacity 0 to ask).
+ * nkg_lstm_cell / nkg_gru_cell: one step of neuronika-nn's LSTMCell / GRUCell (lib.rs:450-626) as ONE forward and ONE
+ * backward node: x (N, I), hidden and cell_state (N, H), weight_ih (G*H, I), weight_hh (G*H, H), biases (G*H,), G = 4
+ * (LSTM, gate chunks [i | f | g | o], the intended assignment of SURVEY.md 8-c defect 7 = torch.nn.LSTMCell) or 3 (GRU,
+ * [r | z | n] = torch.nn.GRUCell).  All operands share one element type and one context.  The outputs are differentiable
+ * if any operand is; the LSTM's two outputs carry the same node in their histories. */
+int nkg_chunks(nkg_var* a, int ndim, const int64_t* chunk_shape, int capacity, nkg_var** outs, int* count);
+int nkg_lstm_cell(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh,
+                  nkg_var* bias_ih, nkg_var* bias_hh, nkg_var** new_cell_state, nkg_var** new_hidden);
+int nkg_gru_cell(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
+                 nkg_var* bias_hh, nkg_var** new_hidden);
+
 /* ---- gradient-ready hook (data parallel overlap): `cb(user, begin, end)` is called from inside nkg_backward(), on
  * the calling thread, right after the LAST kernel that accumulates into elements [begin, end) of this leaf's gradient
  * in the running backward pass has been launched -- so the caller can start the all-reduce of that range while the

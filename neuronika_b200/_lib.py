@@ -137,6 +137,12 @@ _PROTOS = {
     "nk_comm_rank": (i32, [vp]),
     "nk_allreduce_sum": (i32, [vp, vp, sz, i32]),
     "nk_sgd_step": (i32, [vp, vp, i32, vp, i32, vp, vp, sz, f32, f32, f32, f32, i32, f32, i32]),
+    "nk_lstm_cell_fwd": (i32, [vp, vp, vp, vp, vp, i64, i64, i32]),
+    "nk_lstm_cell_bwd": (i32, [vp, vp, i32, vp, f32, vp, vp, vp, vp, i64, i64, i32]),
+    "nk_gru_cell_fwd": (i32, [vp, vp, vp, vp, vp, i64, i64, i32]),
+    "nk_gru_cell_bwd": (i32, [vp, vp, vp, i32, vp, f32, vp, vp, vp, vp, i64, i64, i32]),
+    "nk_chunk_fwd": (i32, [vp, vp, vp, i32, pi64, pi64, i64, i32]),
+    "nk_chunk_bwd": (i32, [vp, vp, i32, vp, i32, i32, pi64, pi64, i64, f32]),
 }
 
 for _name, (_res, _args) in _PROTOS.items():

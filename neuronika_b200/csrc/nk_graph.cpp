@@ -970,6 +970,178 @@ struct ConvolutionNdBackward : Backward {  // convolution/mod.rs:357-510
   }
 };
 
+// ------------------------------------------------------------------------------- chunks (chunk/mod.rs)
+struct Chunk : Forward {
+  nk_ctx* ctx;
+  TensorP operand, data;
+  int64_t index;
+  const char* name() const override { return "Chunk"; }
+  void forward() override {
+    ck(ctx, nk_chunk_fwd(ctx, data->wptr(), operand->rptr(), (int)operand->shape.size(), operand->shape.data(),
+                         data->shape.data(), index, data->dtype));
+  }
+};
+struct ChunkBackward : Backward {
+  nk_ctx* ctx;
+  GradientP operand_grad;
+  int64_t index;
+  const char* name() const override { return "ChunkBackward"; }
+  void targets(std::vector<Gradient*>& out) override {
+    if (operand_grad) out.push_back(operand_grad->root());
+  }
+  void backward() override {
+    // a write into one block: Gradient::acc() would let the first writer overwrite the whole buffer, so the block is
+    // added onto materialised zeros (get()) instead
+    void* d = operand_grad->get();
+    Gradient* r = operand_grad->root();
+    ck(ctx, nk_chunk_bwd(ctx, d, r->dtype, gradient->get(), gradient->dtype, (int)r->shape.size(), r->shape.data(),
+                         gradient->shape.data(), index, 1.f));
+    r->is_zero = false;
+    grad_written(operand_grad);
+  }
+};
+
+// ------------------------------------------------------------------------------- recurrent cells
+// LSTMCell / GRUCell (neuronika-nn/src/lib.rs:450-626) as ONE forward and ONE backward node per step instead of the
+// ~15 nodes the reference composes them from: the two GEMMs write the gate pre-activations in f32 (kept for the tape's
+// lifetime, so a second backward() still works), one kernel applies the gates (nk_lstm_cell_fwd / nk_gru_cell_fwd).
+// The backward runs the gate kernel, then the weight gradients (dW += dG^T.x, TN), the bias gradients (column sums of
+// dG) and the input / state gradients (dx += dG.W, NN), only for the operands that are differentiable.
+struct CellOperands {
+  TensorP x, h, c, w_ih, w_hh, b_ih, b_hh;   // c: LSTM only
+};
+struct CellGrads {
+  GradientP x, h, c, w_ih, w_hh, b_ih, b_hh;
+};
+struct RnnCell : Forward {
+  nk_ctx* ctx;
+  bool lstm;
+  CellOperands o;
+  TensorP gi, gh;               // f32 gate pre-activations: LSTM (N, 4H) in gi; GRU (N, 3H) in gi (input) and gh (hidden)
+  TensorP h_out, c_out;
+  const char* name() const override { return lstm ? "LSTMCell" : "GRUCell"; }
+  void forward() override {
+    const int64_t N = o.x->shape[0], I = o.x->shape[1], H = o.h->shape[1], G = o.w_ih->shape[0];
+    const int dt = o.x->dtype;
+    gemm(ctx, false, true, N, G, I, o.x->rptr(), I, o.w_ih->rptr(), I, 0.f, gi->wptr(), dt, NK_F32, o.b_ih->rptr(),
+         o.b_ih->dtype);
+    if (lstm) {
+      gemm(ctx, false, true, N, G, H, o.h->rptr(), H, o.w_hh->rptr(), H, 1.f, gi->rptr(), dt, NK_F32, o.b_hh->rptr(),
+           o.b_hh->dtype);
+      ck(ctx, nk_lstm_cell_fwd(ctx, c_out->wptr(), h_out->wptr(), (const float*)gi->rptr(), o.c->rptr(), N, H, dt));
+    } else {
+      gemm(ctx, false, true, N, G, H, o.h->rptr(), H, o.w_hh->rptr(), H, 0.f, gh->wptr(), dt, NK_F32, o.b_hh->rptr(),
+           o.b_hh->dtype);
+      ck(ctx, nk_gru_cell_fwd(ctx, h_out->wptr(), (const float*)gi->rptr(), (const float*)gh->rptr(), o.h->rptr(), N, H,
+                              dt));
+    }
+  }
+};
+// the content of a gradient nobody has written in this pass is known to be zero: the kernels take NULL for it
+static const void* grad_or_null(const GradientP& g) {
+  if (!g) return nullptr;
+  Gradient* r = g->root();
+  if (r->is_zero && !r->is_const) return nullptr;
+  return g->get();
+}
+struct RnnCellBackward : Backward {  // `gradient` is the new hidden state's; c_out_grad the new cell state's (LSTM)
+  nk_ctx* ctx;
+  bool lstm;
+  CellOperands o;
+  CellGrads d;
+  TensorP gi, gh;
+  GradientP c_out_grad;
+  const char* name() const override { return lstm ? "LSTMCellBackward" : "GRUCellBackward"; }
+  void targets(std::vector<Gradient*>& out) override {
+    for (const GradientP* g : {&d.w_hh, &d.w_ih, &d.b_ih, &d.b_hh, &d.x, &d.h, &d.c})
+      if (*g) out.push_back((*g)->root());
+  }
+  // dW += dG^T.A (TN).  A weight with a data-parallel reduce-scatter plan is computed locally and reported as not pushed
+  // ONCE per backward pass, by its last writer: in an unrolled sequence every time step's node accumulates into the same
+  // weight gradient, and the caller exchanges the whole gradient for every report it gets.
+  void weight(const GradientP& g, const void* dG, const TensorP& a, int64_t G, int64_t N, int dt) {
+    if (!g) return;
+    float beta;
+    void* p = g->acc(&beta);
+    const int64_t K = a->shape[1];
+    gemm(ctx, true, false, G, K, N, dG, G, a->rptr(), K, beta, p, dt, g->dtype);
+    Gradient* r = g->root();
+    if (r->rs_world > 1 && r->rs_hook && r->last_writer == g_bwd_pos) r->rs_hook(r->rs_user, 0);
+    grad_written(g);
+  }
+  void bias(const GradientP& g, const void* dG, int64_t G, int64_t N, int dt) {
+    if (!g) return;
+    float beta;
+    void* p = g->acc(&beta);
+    const int64_t ds[1] = {G}, gs[2] = {N, G};
+    ck(ctx, nk_unbroadcast_acc(ctx, p, g->dtype, 1, ds, dG, dt, 2, gs, beta));
+    grad_written(g);
+  }
+  // dA += dG.W (NN)
+  void input(const GradientP& g, const void* dG, const TensorP& w, int64_t G, int64_t N, int dt) {
+    if (!g) return;
+    float beta;
+    void* p = g->acc(&beta);
+    const int64_t K = w->shape[1];
+    gemm(ctx, false, false, N, K, G, dG, G, w->rptr(), K, beta, p, dt, g->dtype);
+    grad_written(g);
+  }
+  void backward() override {
+    const int64_t N = o.x->shape[0], H = o.h->shape[1], G = o.w_ih->shape[0];
+    const int dt = o.x->dtype;
+    const size_t gbytes = size_t(N) * size_t(G) * esize(dt);
+    void* dI = nullptr;
+    void* dH = nullptr;
+    try {
+      ck(ctx, nk_alloc_uninit(ctx, gbytes, &dI));
+      if (lstm) {
+        const void* dh = grad_or_null(gradient);
+        const void* dc = grad_or_null(c_out_grad);
+        if (d.c)
+          acc_typed(ctx, d.c, dt, [&](void* p, float beta) {
+            ck(ctx, nk_lstm_cell_bwd(ctx, dI, dt, p, beta, (const float*)gi->rptr(), o.c->rptr(), dh, dc, N, H, dt));
+          });
+        else
+          ck(ctx, nk_lstm_cell_bwd(ctx, dI, dt, nullptr, 0.f, (const float*)gi->rptr(), o.c->rptr(), dh, dc, N, H, dt));
+        dH = dI;   // one gate gradient for both products
+      } else {
+        ck(ctx, nk_alloc_uninit(ctx, gbytes, &dH));
+        const void* dh = gradient->get();
+        if (d.h)
+          acc_typed(ctx, d.h, dt, [&](void* p, float beta) {
+            ck(ctx, nk_gru_cell_bwd(ctx, dI, dH, dt, p, beta, (const float*)gi->rptr(), (const float*)gh->rptr(),
+                                    o.h->rptr(), dh, N, H, dt));
+          });
+        else
+          ck(ctx, nk_gru_cell_bwd(ctx, dI, dH, dt, nullptr, 0.f, (const float*)gi->rptr(), (const float*)gh->rptr(),
+                                  o.h->rptr(), dh, N, H, dt));
+      }
+      // the parameters first (their data-parallel exchange can then overlap the rest), as MatMulBackward does
+      weight(d.w_hh, dH, o.h, G, N, dt);
+      weight(d.w_ih, dI, o.x, G, N, dt);
+      bias(d.b_ih, dI, G, N, dt);
+      bias(d.b_hh, dH, G, N, dt);
+      input(d.x, dI, o.w_ih, G, N, dt);
+      input(d.h, dH, o.w_hh, G, N, dt);
+      if (d.c) grad_written(d.c);
+    } catch (...) {
+      if (dH && dH != dI) nk_free(ctx, dH);
+      if (dI) nk_free(ctx, dI);
+      throw;
+    }
+    if (dH != dI) ck(ctx, nk_free(ctx, dH));
+    ck(ctx, nk_free(ctx, dI));
+  }
+  void no_grad() override {
+    Backward::no_grad();
+    if (c_out_grad) c_out_grad->no_grad();
+  }
+  void with_grad() override {
+    Backward::with_grad();
+    if (c_out_grad) c_out_grad->with_grad();
+  }
+};
+
 }  // namespace nkg
 
 // ------------------------------------------------------------------------------- Variable (handle)
@@ -1967,6 +2139,141 @@ int nkg_convolution_nd(nkg_var* kernel, nkg_var* input, int nsp, const int64_t* 
     }
     *out = v;
   });
+}
+
+// ---------------------------------------------------------------- chunks / recurrent cells
+int nkg_chunks(nkg_var* a, int ndim, const int64_t* chunk_shape, int capacity, nkg_var** outs, int* count) {
+  return guard([&] {
+    if (!a || !chunk_shape || !count || (capacity > 0 && !outs)) fail(NK_ERR_INVALID_ARG, "chunks: NULL");
+    const Shape& xs = a->data->shape;
+    if (ndim != (int)xs.size()) fail(NK_ERR_INVALID_ARG, "chunks: chunk shape has %d dimensions, the operand %d", ndim, (int)xs.size());
+    int64_t nblocks = 1;
+    for (int k = 0; k < ndim; ++k) {
+      if (chunk_shape[k] < 1 || chunk_shape[k] > xs[k])
+        fail(NK_ERR_INVALID_ARG, "chunks: chunk dimension %d (%lld) must be in [1, %lld]", k, (long long)chunk_shape[k],
+             (long long)xs[k]);
+      nblocks *= xs[k] / chunk_shape[k];
+    }
+    *count = (int)nblocks;
+    if (capacity < nblocks) return;   // size query: nothing recorded
+    const Shape cs(chunk_shape, chunk_shape + ndim);
+    for (int64_t i = 0; i < nblocks; ++i) {
+      TensorP od;
+      nkg_var* v = unary_node(a, cs, a->data->dtype, od);
+      auto fw = std::make_shared<Chunk>();
+      fw->ctx = a->ctx;
+      fw->operand = a->data;
+      fw->data = od;
+      fw->index = i;
+      uint64_t id = push(v, fw);
+      if (a->diff()) {
+        v->grad = std::make_shared<Gradient>(a->ctx, cs, od->dtype);
+        auto bw = std::make_shared<ChunkBackward>();
+        bw->ctx = a->ctx;
+        bw->gradient = v->grad;
+        bw->operand_grad = a->grad;
+        bw->index = i;
+        push_bwd(v, id, bw);
+      }
+      outs[i] = v;
+    }
+  });
+}
+
+static void cell_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih,
+                      nkg_var* b_hh, nkg_var** new_c, nkg_var** new_h) {
+  const char* who = lstm ? "lstm_cell" : "gru_cell";
+  struct Arg {
+    nkg_var* v;
+    const char* name;
+  };
+  std::vector<Arg> args = {{x, "input"}, {h, "hidden"}, {w_ih, "weight_ih"}, {w_hh, "weight_hh"}, {b_ih, "bias_ih"},
+                           {b_hh, "bias_hh"}};
+  if (lstm) args.push_back({c, "cell_state"});
+  for (const Arg& a : args)
+    if (!a.v) fail(NK_ERR_INVALID_ARG, "%s: %s is NULL", who, a.name);
+  if (!new_h || (lstm && !new_c)) fail(NK_ERR_INVALID_ARG, "%s: NULL output", who);
+  for (const Arg& a : args) {
+    if (a.v->data->dtype != x->data->dtype)
+      fail(NK_ERR_INVALID_ARG, "%s: %s has another element type than the input", who, a.name);
+    if (a.v->ctx != x->ctx) fail(NK_ERR_INVALID_ARG, "%s: %s lives on another device than the input", who, a.name);
+  }
+  const int64_t G = lstm ? 4 : 3;
+  auto shape_str = [](const Shape& s) {
+    std::string out = "(";
+    for (size_t i = 0; i < s.size(); ++i) out += (i ? ", " : "") + std::to_string(s[i]);
+    return out + (s.size() == 1 ? ",)" : ")");
+  };
+  const Shape& xs = x->data->shape;
+  if (xs.size() != 2) fail(NK_ERR_INVALID_ARG, "%s: input must be (batch, input_size), got %s", who, shape_str(xs).c_str());
+  const Shape& hs = h->data->shape;
+  if (hs.size() != 2 || hs[0] != xs[0])
+    fail(NK_ERR_INVALID_ARG, "%s: hidden must be (batch = %lld, hidden_size), got %s", who, (long long)xs[0],
+         shape_str(hs).c_str());
+  const int64_t N = xs[0], I = xs[1], H = hs[1];
+  auto expect = [&](nkg_var* v, const char* name, const Shape& want) {
+    if (v->data->shape != want)
+      fail(NK_ERR_INVALID_ARG, "%s: %s must be %s, got %s", who, name, shape_str(want).c_str(),
+           shape_str(v->data->shape).c_str());
+  };
+  if (lstm) expect(c, "cell_state", {N, H});
+  expect(w_ih, "weight_ih", {G * H, I});
+  expect(w_hh, "weight_hh", {G * H, H});
+  expect(b_ih, "bias_ih", {G * H});
+  expect(b_hh, "bias_hh", {G * H});
+
+  nk_ctx* ctx = x->ctx;
+  const int dt = x->data->dtype;
+  auto fw = std::make_shared<RnnCell>();
+  fw->ctx = ctx;
+  fw->lstm = lstm;
+  fw->o = CellOperands{x->data, h->data, lstm ? c->data : nullptr, w_ih->data, w_hh->data, b_ih->data, b_hh->data};
+  fw->gi = std::make_shared<Tensor>(ctx, Shape{N, G * H}, NK_F32);
+  if (!lstm) fw->gh = std::make_shared<Tensor>(ctx, Shape{N, G * H}, NK_F32);
+  fw->h_out = std::make_shared<Tensor>(ctx, Shape{N, H}, dt);
+  if (lstm) fw->c_out = std::make_shared<Tensor>(ctx, Shape{N, H}, dt);
+
+  nkg_var* vh = new_like(x);
+  vh->data = fw->h_out;
+  for (const Arg& a : args) {   // History::merge over every operand
+    vh->fwd.insert(a.v->fwd.begin(), a.v->fwd.end());
+    vh->bwd.insert(a.v->bwd.begin(), a.v->bwd.end());
+  }
+  const uint64_t id = push(vh, fw);
+  bool diff = false;
+  for (const Arg& a : args) diff = diff || a.v->diff();
+  if (diff) {
+    vh->grad = std::make_shared<Gradient>(ctx, Shape{N, H}, dt);
+    auto bw = std::make_shared<RnnCellBackward>();
+    bw->ctx = ctx;
+    bw->lstm = lstm;
+    bw->o = fw->o;
+    bw->gi = fw->gi;
+    bw->gh = fw->gh;
+    bw->gradient = vh->grad;
+    bw->d = CellGrads{x->grad, h->grad, lstm ? c->grad : nullptr, w_ih->grad, w_hh->grad, b_ih->grad, b_hh->grad};
+    if (lstm) bw->c_out_grad = std::make_shared<Gradient>(ctx, Shape{N, H}, dt);
+    push_bwd(vh, id, bw);
+  }
+  if (lstm) {   // the second output: same tapes, same op id (merging the two histories keeps one node)
+    nkg_var* vc = new nkg_var(*vh);
+    vc->data = fw->c_out;
+    if (diff) vc->grad = std::dynamic_pointer_cast<RnnCellBackward>(vh->bwd[id])->c_out_grad;
+    *new_c = vc;
+  }
+  *new_h = vh;
+}
+
+int nkg_lstm_cell(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh,
+                  nkg_var* bias_ih, nkg_var* bias_hh, nkg_var** new_cell_state, nkg_var** new_hidden) {
+  return guard([&] {
+    cell_impl(true, input, cell_state, hidden, weight_ih, weight_hh, bias_ih, bias_hh, new_cell_state, new_hidden);
+  });
+}
+
+int nkg_gru_cell(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
+                 nkg_var* bias_hh, nkg_var** new_hidden) {
+  return guard([&] { cell_impl(false, input, nullptr, hidden, weight_ih, weight_hh, bias_ih, bias_hh, nullptr, new_hidden); });
 }
 
 // ---------------------------------------------------------------- optimizers on a leaf (neuronika-optim)

@@ -1,4 +1,4 @@
-"""Layers: the mirror of neuronika-nn's Linear and Conv2d (neuronika-nn/src/lib.rs:406-448, 724-815)."""
+"""Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell and Conv2d (neuronika-nn/src/lib.rs:406-626, 724-815)."""
 from __future__ import annotations
 
 import math
@@ -68,3 +68,50 @@ class Conv2d:
 
     def parameters(self):
         return [self.weight, self.bias]
+
+
+class LSTMCell:
+    """One LSTM step (neuronika-nn/src/lib.rs:450-540): weight_ih (4H, I), weight_hh (4H, H), bias_ih, bias_hh (4H,),
+    all ~ U(-k, k), k = 1/sqrt(hidden_size) (:471-489).  Gate chunks [i | f | g | o] with i, f, o = sigmoid and
+    g = tanh: the reference's names, and torch.nn.LSTMCell's layout (the reference applies tanh to the forget gate and
+    sigmoid to the candidate, SURVEY.md 8-c defect 7).  The step is one fused graph node (variable.lstm_cell)."""
+
+    def __init__(self, device: Device, input_size: int, hidden_size: int, dtype=F32, grad_dtype=None,
+                 rng: np.random.Generator | None = None):
+        rng = rng or np.random.default_rng()
+        k = 1.0 / math.sqrt(hidden_size)
+        g = 4 * hidden_size
+        self.weight_ih = V.from_ndarray(device, uniform(rng, (g, input_size), -k, k), dtype).requires_grad(grad_dtype)
+        self.weight_hh = V.from_ndarray(device, uniform(rng, (g, hidden_size), -k, k), dtype).requires_grad(grad_dtype)
+        self.bias_ih = V.from_ndarray(device, uniform(rng, (g,), -k, k), dtype).requires_grad(grad_dtype)
+        self.bias_hh = V.from_ndarray(device, uniform(rng, (g,), -k, k), dtype).requires_grad(grad_dtype)
+
+    def forward(self, state, input: V.Var):
+        """`state = (cell_state, hidden)`, both (batch, hidden_size); returns (new_cell_state, new_hidden) (:510-540)."""
+        cell_state, hidden = state
+        return V.lstm_cell(input, cell_state, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+
+    def parameters(self):
+        return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]
+
+
+class GRUCell:
+    """One GRU step (neuronika-nn/src/lib.rs:543-626, = torch.nn.GRUCell): weight_ih (3H, I), weight_hh (3H, H),
+    bias_ih, bias_hh (3H,), all ~ U(-k, k), k = 1/sqrt(hidden_size); gate chunks [r | z | n].  One fused graph node."""
+
+    def __init__(self, device: Device, input_size: int, hidden_size: int, dtype=F32, grad_dtype=None,
+                 rng: np.random.Generator | None = None):
+        rng = rng or np.random.default_rng()
+        k = 1.0 / math.sqrt(hidden_size)
+        g = 3 * hidden_size
+        self.weight_ih = V.from_ndarray(device, uniform(rng, (g, input_size), -k, k), dtype).requires_grad(grad_dtype)
+        self.weight_hh = V.from_ndarray(device, uniform(rng, (g, hidden_size), -k, k), dtype).requires_grad(grad_dtype)
+        self.bias_ih = V.from_ndarray(device, uniform(rng, (g,), -k, k), dtype).requires_grad(grad_dtype)
+        self.bias_hh = V.from_ndarray(device, uniform(rng, (g,), -k, k), dtype).requires_grad(grad_dtype)
+
+    def forward(self, hidden: V.Var, input: V.Var):
+        """(:607-624) returns the new hidden state (batch, hidden_size)."""
+        return V.gru_cell(input, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+
+    def parameters(self):
+        return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]

@@ -350,3 +350,71 @@ def convnd_bwd_kernel(dw: CuArray, g: CuArray, x: CuArray, stride, dilation, gro
     _ck(lib.nk_convnd_bwd_kernel(g.device.ctx, dw.ptr, dw.dtype, g.ptr, x.ptr,
                                  *_convnd_args(x.shape, dw.shape, stride, dilation, groups), g.dtype, float(beta)), g.device)
     return dw
+
+
+# ---------------------------------------------------------------- 8-f: recurrent cells and chunks (csrc/nk_rnn.cu)
+def _ptr(a: CuArray | None):
+    return a.ptr if a is not None else None
+
+
+def lstm_cell(gates: CuArray, c_prev: CuArray, c_out: CuArray | None = None, h_out: CuArray | None = None):
+    """c' = sigmoid(f)*c + sigmoid(i)*tanh(g), h' = sigmoid(o)*tanh(c') from the f32 (n, 4H) pre-activations
+    [i | f | g | o].  Returns (c_out, h_out)."""
+    n, hidden = c_prev.shape
+    if gates.dtype != F32 or tuple(gates.shape) != (n, 4 * hidden):
+        raise ValueError(f"lstm_cell: gates must be f32 ({n}, {4 * hidden}), got {gates}")
+    c_out = c_out or CuArray(c_prev.device, (n, hidden), c_prev.dtype)
+    h_out = h_out or CuArray(c_prev.device, (n, hidden), c_prev.dtype)
+    _ck(lib.nk_lstm_cell_fwd(c_prev.device.ctx, c_out.ptr, h_out.ptr, gates.ptr, c_prev.ptr, n, hidden, c_prev.dtype),
+        c_prev.device)
+    return c_out, h_out
+
+
+def lstm_cell_bwd(dgates: CuArray, gates: CuArray, c_prev: CuArray, dh_out: CuArray | None, dc_out: CuArray | None,
+                  dc_prev: CuArray | None = None, beta_dc=1.0) -> CuArray:
+    """dgates (overwritten, its own element type) and dc_prev = beta_dc*dc_prev + sigmoid(f)*dc_total.  dh_out / dc_out
+    None = a zero gradient; dc_prev None = the cell state is not differentiable."""
+    n, hidden = c_prev.shape
+    _ck(lib.nk_lstm_cell_bwd(c_prev.device.ctx, dgates.ptr, dgates.dtype, _ptr(dc_prev), float(beta_dc), gates.ptr,
+                             c_prev.ptr, _ptr(dh_out), _ptr(dc_out), n, hidden, c_prev.dtype), c_prev.device)
+    return dgates
+
+
+def gru_cell(igates: CuArray, hgates: CuArray, h_prev: CuArray, h_out: CuArray | None = None) -> CuArray:
+    """h' = (h - nn)*z + nn from the f32 (n, 3H) pre-activations [r | z | n] of the input and of the hidden state."""
+    n, hidden = h_prev.shape
+    for g in (igates, hgates):
+        if g.dtype != F32 or tuple(g.shape) != (n, 3 * hidden):
+            raise ValueError(f"gru_cell: gates must be f32 ({n}, {3 * hidden}), got {g}")
+    h_out = h_out or CuArray(h_prev.device, (n, hidden), h_prev.dtype)
+    _ck(lib.nk_gru_cell_fwd(h_prev.device.ctx, h_out.ptr, igates.ptr, hgates.ptr, h_prev.ptr, n, hidden, h_prev.dtype),
+        h_prev.device)
+    return h_out
+
+
+def gru_cell_bwd(digates: CuArray, dhgates: CuArray, igates: CuArray, hgates: CuArray, h_prev: CuArray, dh_out: CuArray,
+                 dh_prev: CuArray | None = None, beta_dh=1.0):
+    """digates, dhgates (overwritten) and the pointwise part of the hidden-state gradient dh_prev = beta_dh*dh_prev +
+    z*dh_out.  Returns (digates, dhgates)."""
+    n, hidden = h_prev.shape
+    if digates.dtype != dhgates.dtype:
+        raise ValueError("gru_cell_bwd: digates and dhgates must have one element type")
+    _ck(lib.nk_gru_cell_bwd(h_prev.device.ctx, digates.ptr, dhgates.ptr, digates.dtype, _ptr(dh_prev), float(beta_dh),
+                            igates.ptr, hgates.ptr, h_prev.ptr, dh_out.ptr, n, hidden, h_prev.dtype), h_prev.device)
+    return digates, dhgates
+
+
+def chunk(x: CuArray, chunk_shape, index: int, out: CuArray | None = None) -> CuArray:
+    """Block `index` of x's exact_chunks(chunk_shape) (row-major block order), bit exact."""
+    cs = tuple(int(c) for c in chunk_shape)
+    out = out or CuArray(x.device, cs, x.dtype)
+    _ck(lib.nk_chunk_fwd(x.device.ctx, out.ptr, x.ptr, x.ndim, L.shape_arr(x.shape), L.shape_arr(cs), int(index),
+                         x.dtype), x.device)
+    return out
+
+
+def chunk_bwd(dx: CuArray, g: CuArray, index: int, beta=1.0) -> CuArray:
+    """dx[block index] = beta*dx[block] + g; the rest of dx is untouched."""
+    _ck(lib.nk_chunk_bwd(dx.device.ctx, dx.ptr, dx.dtype, g.ptr, g.dtype, dx.ndim, L.shape_arr(dx.shape),
+                         L.shape_arr(g.shape), int(index), float(beta)), dx.device)
+    return dx

@@ -78,6 +78,9 @@ _G = {
     "nkg_adagrad_step": (i32, [vp, vp, vp, i64, f32, f32, f32, f32, f32, f32]),
     "nkg_set_grad_hook": (i32, [vp, vp, vp, i32]),
     "nkg_set_grad_rs": (i32, [vp, i32, i32, pvp, vp, vp]),
+    "nkg_chunks": (i32, [vp, i32, pi64, i32, pvp, C.POINTER(i32)]),
+    "nkg_lstm_cell": (i32, [vp, vp, vp, vp, vp, vp, vp, pvp, pvp]),
+    "nkg_gru_cell": (i32, [vp, vp, vp, vp, vp, vp, pvp]),
 }
 for _n, (_r, _a) in _G.items():
     _f = getattr(lib, _n)
@@ -247,6 +250,16 @@ class Var:
         return self._binary(lib.nkg_convolution, input, int(stride[0]), int(stride[1]), int(dilation[0]),
                             int(dilation[1]), int(groups))
 
+    def chunks(self, chunk_shape) -> list:
+        """`chunks(chunk_size)` (var.rs:401-417): the blocks of ndarray's exact_chunks in row-major block order (trailing
+        partial blocks dropped), one lazy node each; differentiable when the receiver is."""
+        cs = tuple(int(c) for c in chunk_shape)
+        count = C.c_int(0)
+        _ck(lib.nkg_chunks(self._h, len(cs), L.shape_arr(cs), 0, None, C.byref(count)))
+        outs = (vp * max(1, count.value))()
+        _ck(lib.nkg_chunks(self._h, len(cs), L.shape_arr(cs), count.value, outs, C.byref(count)))
+        return [self._wrap(vp(outs[i])) for i in range(count.value)]
+
     def item(self) -> float:
         return float(self.data().reshape(()))
 
@@ -314,6 +327,22 @@ class VarDiff(Var):
         cb = GRAD_RS_HOOK(lambda _user, pushed: fn(int(pushed)))
         self._rs_ref = (cb, arr)
         _ck(lib.nkg_set_grad_rs(self._h, int(world), int(rank), arr, C.cast(cb, vp), None))
+
+
+# ---- recurrent cells (one fused node per step; see include/nk_graph.h)
+def lstm_cell(input: Var, cell_state: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: Var, bias_hh: Var):
+    """One LSTM step, gate chunks [i | f | g | o] (torch.nn.LSTMCell): returns (new_cell_state, new_hidden)."""
+    c, h = vp(), vp()
+    _ck(lib.nkg_lstm_cell(input._h, cell_state._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h,
+                          C.byref(c), C.byref(h)))
+    return input._wrap(c), input._wrap(h)
+
+
+def gru_cell(input: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: Var, bias_hh: Var):
+    """One GRU step, gate chunks [r | z | n] (torch.nn.GRUCell): returns the new hidden state."""
+    h = vp()
+    _ck(lib.nkg_gru_cell(input._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h, C.byref(h)))
+    return input._wrap(h)
 
 
 # ---- constructors (neuronika-variable/src/lib.rs:51-240), on a device

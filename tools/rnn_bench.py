@@ -1,0 +1,228 @@
+#!/usr/bin/env python
+"""LSTM / GRU training-step benchmark (development tool; bench.py measures the flagship workload).
+
+Workload: an unrolled sequence of T = 32 steps, bf16 parameters with f32 gradients, the input a `Var`, h0 = c0 = 0, the
+loss the mse of h_T against a seeded target.  One step is zero_grad -> forward -> backward -> SGD, captured once with
+Device.capture and replayed.  Shapes (N, I, H) = (256, 1024, 1024) and (1024, 2048, 2048), LSTM and GRU.
+
+Reported per configuration, in one JSON line each:
+  - ms per sequence and per time step, and kernel launches per time step (the captured graph's kernel count / T);
+  - the cell's GEMMs alone (the same five products per step, timed back to back: x.W_ih^T + b, h.W_hh^T + b,
+    dW_ih, dW_hh, dh), as TFLOP/s from FLOPs counted from the shapes, and their share of the step;
+  - the gate kernels alone (forward and backward, CUDA events over many launches) as GB/s against HBM, from the bytes
+    each must move (f32 gates, bf16 states / gradients) counted from the shapes;
+  - in the same process and alternating with it: the same cell composed from primitives through the graph API
+    (chunks + sigmoid / tanh + mul / add, intended gate assignment), also captured and replayed, and
+    torch.nn.LSTMCell / GRUCell in bf16 on the same GPU in an eager loop ("torch_eager_bf16").
+Card name, power limit and the median SM clock during the timed windows (NVML) are printed beside the numbers.
+
+    python tools/rnn_bench.py [--reps 5] [--window-ms 200]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+
+from gemm_sweep import Clock  # noqa: E402
+
+T = 32
+SHAPES = [(256, 1024, 1024), (1024, 2048, 2048)]
+
+
+def timed(torch, fn, clock, window_ms, reps):
+    """median ms per call over `reps` windows of back-to-back calls, and the median SM clock meanwhile"""
+    for _ in range(2):
+        fn()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    fn()
+    torch.cuda.synchronize()
+    iters = int(min(2000, max(3, window_ms / ((time.perf_counter() - t0) * 1e3))))
+    clock.armed.set()
+    per = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(iters):
+            fn()
+        e1.record()
+        e1.synchronize()
+        per.append(e0.elapsed_time(e1) / iters)
+    clock.armed.clear()
+    return float(np.median(per)), clock.take()
+
+
+def composed_cell(kind, cell, state, x, n, hidden):
+    """the cell written as the reference writes it (intended LSTM gate assignment), through the graph API"""
+    if kind == "lstm":
+        c, h = state
+        gates = x.mm_t(cell.weight_ih) + cell.bias_ih + h.mm_t(cell.weight_hh) + cell.bias_hh
+        i, f, g, o = gates.chunks((n, hidden))
+        c2 = f.sigmoid() * c + i.sigmoid() * g.tanh()
+        return c2, o.sigmoid() * c2.tanh()
+    ig = x.mm_t(cell.weight_ih) + cell.bias_ih
+    hg = state.mm_t(cell.weight_hh) + cell.bias_hh
+    ir, iz, i_n = ig.chunks((n, hidden))
+    hr, hz, hn = hg.chunks((n, hidden))
+    r, z = (hr + ir).sigmoid(), (hz + iz).sigmoid()
+    nn = (i_n + hn * r).tanh()
+    return (state - nn) * z + nn
+
+
+def graph_step(nk, dev, kind, n, n_in, hidden, composed):
+    """(captured step, kernels per replay)"""
+    from neuronika_b200 import optim
+    rng = np.random.default_rng(0)
+    cls = nk.nn.LSTMCell if kind == "lstm" else nk.nn.GRUCell
+    cell = cls(dev, n_in, hidden, nk.BF16, grad_dtype=nk.F32, rng=rng)
+    opt = optim.StochasticGD.new(1e-3)
+    for p in cell.parameters():
+        opt.register(p)
+    xs = [nk.from_ndarray(dev, rng.uniform(-1, 1, (n, n_in)).astype(np.float32), nk.BF16) for _ in range(T)]
+    zero = nk.zeros(dev, (n, hidden), nk.BF16)
+    tgt = nk.from_ndarray(dev, rng.uniform(-0.5, 0.5, (n, hidden)).astype(np.float32), nk.BF16)
+
+    def step():
+        opt.zero_grad()
+        state = (zero, zero) if kind == "lstm" else zero
+        for x in xs:
+            state = composed_cell(kind, cell, state, x, n, hidden) if composed else cell.forward(state, x)
+        loss = (state[1] if kind == "lstm" else state).mse_loss(tgt)
+        loss.forward()
+        loss.backward(1.0)
+        opt.step()
+
+    step()
+    step()
+    dev.synchronize()
+    with dev.capture(8 << 30) as cap:
+        step()
+    return cap.graph
+
+
+def torch_step(torch, kind, n, n_in, hidden):
+    g = torch.Generator(device="cuda").manual_seed(0)
+    cell = (torch.nn.LSTMCell if kind == "lstm" else torch.nn.GRUCell)(n_in, hidden).cuda().to(torch.bfloat16)
+    opt = torch.optim.SGD(cell.parameters(), lr=1e-3)
+    xs = [(torch.rand(n, n_in, device="cuda", generator=g) * 2 - 1).to(torch.bfloat16) for _ in range(T)]
+    tgt = (torch.rand(n, hidden, device="cuda", generator=g) - 0.5).to(torch.bfloat16)
+    zero = torch.zeros(n, hidden, device="cuda", dtype=torch.bfloat16)
+
+    def step():
+        opt.zero_grad(set_to_none=False)
+        state = (zero, zero) if kind == "lstm" else zero
+        for x in xs:
+            state = cell(x, state)
+        h = state[0] if kind == "lstm" else state          # torch returns (h, c)
+        torch.nn.functional.mse_loss(h, tgt).backward()
+        opt.step()
+    return step
+
+
+def gemm_only(nk, dev, torch, kind, n, n_in, hidden):
+    """the five products of one cell step, back to back"""
+    from neuronika_b200 import ops
+    G = (4 if kind == "lstm" else 3) * hidden
+    r = lambda *s: dev.from_ndarray(np.random.default_rng(1).uniform(-1, 1, s).astype(np.float32), nk.BF16)
+    x, h, w_ih, w_hh, b = r(n, n_in), r(n, hidden), r(G, n_in), r(G, hidden), r(G)
+    gates, dg = dev.zeros((n, G), nk.F32), r(n, G)
+    dw_ih, dw_hh, dh = dev.zeros((G, n_in), nk.F32), dev.zeros((G, hidden), nk.F32), dev.zeros((n, hidden), nk.BF16)
+
+    def run():
+        ops.gemm(x, w_ih, gates, trans_b=True, bias=b)
+        ops.gemm(h, w_hh, gates, trans_b=True, bias=b, beta=1.0)
+        ops.gemm(dg, x, dw_ih, trans_a=True, beta=1.0)
+        ops.gemm(dg, h, dw_hh, trans_a=True, beta=1.0)
+        ops.gemm(dg, w_hh, dh)
+    flops = 2.0 * n * G * (n_in + hidden) * 2 + 2.0 * n * G * hidden
+    return run, flops
+
+
+def gate_kernels(nk, dev, kind, n, hidden):
+    """(fwd fn, fwd bytes, bwd fn, bwd bytes)"""
+    from neuronika_b200 import ops
+    rng = np.random.default_rng(2)
+    s = lambda: dev.from_ndarray(rng.uniform(-1, 1, (n, hidden)).astype(np.float32), nk.BF16)
+    if kind == "lstm":
+        gates = dev.from_ndarray(rng.standard_normal((n, 4 * hidden)).astype(np.float32))
+        c, dh, dc = s(), s(), s()
+        co, ho, dcp = dev.zeros((n, hidden), nk.BF16), dev.zeros((n, hidden), nk.BF16), dev.zeros((n, hidden), nk.BF16)
+        dg = dev.zeros((n, 4 * hidden), nk.BF16)
+        fwd = lambda: ops.lstm_cell(gates, c, co, ho)
+        bwd = lambda: ops.lstm_cell_bwd(dg, gates, c, dh, dc, dcp, beta_dc=0.0)
+        return fwd, n * hidden * (16 + 2 + 4), bwd, n * hidden * (16 + 2 * 3 + 8 + 2)
+    ig = dev.from_ndarray(rng.standard_normal((n, 3 * hidden)).astype(np.float32))
+    hg = dev.from_ndarray(rng.standard_normal((n, 3 * hidden)).astype(np.float32))
+    h, dh = s(), s()
+    ho, dhp = dev.zeros((n, hidden), nk.BF16), dev.zeros((n, hidden), nk.BF16)
+    di, dhg = dev.zeros((n, 3 * hidden), nk.BF16), dev.zeros((n, 3 * hidden), nk.BF16)
+    fwd = lambda: ops.gru_cell(ig, hg, h, ho)
+    bwd = lambda: ops.gru_cell_bwd(di, dhg, ig, hg, h, dh, dhp, beta_dh=0.0)
+    return fwd, n * hidden * (24 + 2 + 2), bwd, n * hidden * (24 + 2 * 2 + 12 + 2)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--window-ms", type=float, default=200.0)
+    ap.add_argument("--reps", type=int, default=5)
+    args = ap.parse_args()
+    import torch
+
+    import neuronika_b200 as nk
+
+    torch.cuda.set_device(0)
+    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
+    torch.cuda.set_stream(stream)
+    dev = nk.Device(0, stream=stream.cuda_stream)
+    clock = Clock(0)
+    clock.start()
+    card = clock.card()
+    print(json.dumps({"card": card, "sm_count": dev.sm_count, "T": T}), flush=True)
+    for kind in ("lstm", "gru"):
+        for n, n_in, hidden in SHAPES:
+            fused = graph_step(nk, dev, kind, n, n_in, hidden, composed=False)
+            comp = graph_step(nk, dev, kind, n, n_in, hidden, composed=True)
+            teager = torch_step(torch, kind, n, n_in, hidden)
+            res = {"fused": [], "composed": [], "torch_eager_bf16": []}
+            mhz = []
+            for _ in range(args.reps):      # alternating, one window each
+                for name, fn in (("fused", fused.launch), ("composed", comp.launch), ("torch_eager_bf16", teager)):
+                    ms, m = timed(torch, fn, clock, args.window_ms, 1)
+                    res[name].append(ms)
+                    mhz.append(m)
+            gem, flops = gemm_only(nk, dev, torch, kind, n, n_in, hidden)
+            gms, _ = timed(torch, gem, clock, args.window_ms / 4, args.reps)
+            fwd, fb, bwd, bb = gate_kernels(nk, dev, kind, n, hidden)
+            fms, _ = timed(torch, fwd, clock, args.window_ms / 4, args.reps)
+            bms, _ = timed(torch, bwd, clock, args.window_ms / 4, args.reps)
+            med = {k: float(np.median(v)) for k, v in res.items()}
+            print(json.dumps({
+                "cell": kind, "N": n, "I": n_in, "H": hidden, "T": T,
+                "ms_per_sequence": {k: round(v, 3) for k, v in med.items()},
+                "ms_per_time_step": {k: round(v / T, 4) for k, v in med.items()},
+                "launches_per_time_step": {"fused": round(fused.kernel_count / T, 2),
+                                           "composed": round(comp.kernel_count / T, 2)},
+                "speedup_fused_vs_composed": round(med["composed"] / med["fused"], 2),
+                "speedup_fused_vs_torch_eager_bf16": round(med["torch_eager_bf16"] / med["fused"], 2),
+                "gemm_only_ms_per_time_step": round(gms, 4),
+                "gemm_tflops": round(flops / gms / 1e9, 1),
+                "gemm_share_of_fused_step": round(gms * T / med["fused"], 3),
+                "gate_fwd_us": round(fms * 1e3, 2), "gate_fwd_gbps": round(fb / fms / 1e6, 1),
+                "gate_bwd_us": round(bms * 1e3, 2), "gate_bwd_gbps": round(bb / bms / 1e6, 1),
+                "median_sm_mhz": float(np.median(mhz)), "card": card["name"], "power_limit_w": card["power_limit_w"],
+            }), flush=True)
+            fused.close()
+            comp.close()
+    clock.halt.set()
+
+
+if __name__ == "__main__":
+    main()
