@@ -313,6 +313,22 @@ int nk_chunk_fwd(nk_ctx* ctx, void* y, const void* x, int ndim, const int64_t* x
 int nk_chunk_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* g, int g_dtype, int ndim, const int64_t* x_shape,
                  const int64_t* chunk_shape, int64_t index, float beta);
 
+/* ---- concatenation (multi_concatenate/mod.rs, multi_stack/mod.rs; csrc/nk_cat.cu) ----
+ * Operand i is an (outer, lens[i], inner) block; the output is (outer, sum lens, inner) with operand i at offset
+ * sum_{j<i} lens[j] along the middle axis.  A stack is the same call with every lens[i] = 1.  xs / lens (and the
+ * backward's per-operand arrays) are host arrays of `count` entries, passed to the kernel by value: one launch per
+ * NK_CAT_OPS_PER_LAUNCH operands in each direction, no allocation and no host-to-device copy, so both calls can be
+ * captured (nk_capture_begin).
+ * nk_cat_fwd: a bit-exact copy; an operand with no elements contributes nothing (its pointer may be NULL).
+ * nk_cat_bwd: dxs[i] = betas[i]*dxs[i] + (block i of g), element type dx_dtypes[i] (f32 or bf16, independently of g's;
+ * bf16 results are rounded to nearest even); dxs[i] == NULL: operand i gets no gradient.  The non-NULL dxs must be
+ * pairwise distinct (two slices summed into one buffer are two calls). */
+#define NK_CAT_OPS_PER_LAUNCH 64
+int nk_cat_fwd(nk_ctx* ctx, void* y, const void* const* xs, const int64_t* lens, int count, int64_t outer,
+               int64_t inner, int dtype);
+int nk_cat_bwd(nk_ctx* ctx, void* const* dxs, const int* dx_dtypes, const float* betas, const void* g, int g_dtype,
+               const int64_t* lens, int count, int64_t outer, int64_t inner);
+
 /* ---- SGD (neuronika-optim/src/sgd/mod.rs:191-231, penalty.rs:63-67) ----
  *   g' = grad_scale*g + 2*l2*w ; no momentum: w -= lr*g' ;
  *   momentum: buf = mu*buf + (1-damp)*g' ; w -= lr*(nesterov ? g' + mu*buf : buf).

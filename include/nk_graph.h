@@ -130,6 +130,18 @@ int nkg_lstm_cell(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var*
 int nkg_gru_cell(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
                  nkg_var* bias_hh, nkg_var** new_hidden);
 
+/* ---- concatenation (var.rs:564-645, vardiff.rs:627-; multi_concatenate/mod.rs, multi_stack/mod.rs) ----
+ * nkg_cat: the `count` operands side by side along `axis` (0 <= axis < ndim; equal shapes on every other axis, any length
+ * along `axis`, 0 included).  nkg_stack: identical shapes, joined along a new axis 0 <= axis <= ndim.  Both record ONE
+ * forward and ONE backward node whatever the count; the result's history is the union of the operands' plus that node.
+ * All operands share one element type and one context; the result is differentiable if any operand is, and only the
+ * differentiable operands receive gradients.  count >= 1 (one operand: a copy).
+ * nkg_unsqueeze (var.rs:425-431): a new axis of length 1 at 0 <= axis <= ndim.  A view, like nkg_flatten: no kernel,
+ * no node (the reference records one), and the gradient is the operand's. */
+int nkg_cat(nkg_var* const* vars, int count, int axis, nkg_var** out);
+int nkg_stack(nkg_var* const* vars, int count, int axis, nkg_var** out);
+int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out);
+
 /* ---- gradient-ready hook (data parallel overlap): `cb(user, begin, end)` is called from inside nkg_backward(), on
  * the calling thread, right after the LAST kernel that accumulates into elements [begin, end) of this leaf's gradient
  * in the running backward pass has been launched -- so the caller can start the all-reduce of that range while the

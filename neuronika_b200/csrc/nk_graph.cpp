@@ -19,6 +19,7 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <stdexcept>
@@ -1001,6 +1002,63 @@ struct ChunkBackward : Backward {
   }
 };
 
+// ------------------------------------------------------------------------------- cat / stack
+// MultiConcatenate / MultiStack (multi_concatenate/mod.rs, multi_stack/mod.rs) as ONE node whatever the operand count:
+// operand i is an (outer, lens[i], inner) block of the output (a stacked operand has length 1 along the new axis).
+struct Concatenate : Forward {
+  nk_ctx* ctx;
+  std::vector<TensorP> operands;
+  TensorP data;
+  std::vector<int64_t> lens;
+  int64_t outer, inner;
+  bool stack;
+  const char* name() const override { return stack ? "MultiStack" : "MultiConcatenate"; }
+  void forward() override {
+    if (data->n() == 0) return;
+    std::vector<const void*> xs;
+    for (size_t i = 0; i < operands.size(); ++i) xs.push_back(lens[i] ? operands[i]->rptr() : nullptr);
+    ck(ctx, nk_cat_fwd(ctx, data->wptr(), xs.data(), lens.data(), (int)lens.size(), outer, inner, data->dtype));
+  }
+};
+struct ConcatenateBackward : Backward {
+  nk_ctx* ctx;
+  std::vector<GradientP> operand_grads;   // null for an operand that is not differentiable
+  std::vector<int64_t> lens;
+  int64_t outer, inner;
+  bool stack;
+  const char* name() const override { return stack ? "MultiStackBackward" : "MultiConcatenateBackward"; }
+  void targets(std::vector<Gradient*>& out) override {
+    for (const GradientP& g : operand_grads)
+      if (g && std::find(out.begin(), out.end(), g->root()) == out.end()) out.push_back(g->root());
+  }
+  void backward() override {
+    // Every slice covers its operand's whole gradient, so each one accumulates with Gradient::acc()'s beta.  Operands
+    // that share a gradient (x.cat([x, x]), or gradients the peephole aliased to one root) go to separate calls:
+    // pass p holds the p-th occurrence of each root and adds onto what the earlier passes wrote.
+    const size_t n = operand_grads.size();
+    std::vector<int> pass(n, -1);
+    int passes = 0;
+    std::map<Gradient*, int> seen;
+    for (size_t i = 0; i < n; ++i)
+      if (operand_grads[i] && operand_grads[i]->n() > 0)
+        passes = std::max(passes, (pass[i] = seen[operand_grads[i]->root()]++) + 1);
+    if (passes == 0) return;
+    const void* g = gradient->get();
+    for (int p = 0; p < passes; ++p) {
+      std::vector<void*> dxs(n, nullptr);
+      std::vector<int> dts(n, NK_F32);
+      std::vector<float> betas(n, 0.f);
+      for (size_t i = 0; i < n; ++i) {
+        if (pass[i] != p) continue;
+        dxs[i] = operand_grads[i]->acc(&betas[i]);
+        dts[i] = operand_grads[i]->root()->dtype;
+      }
+      ck(ctx, nk_cat_bwd(ctx, dxs.data(), dts.data(), betas.data(), g, gradient->dtype, lens.data(), (int)n, outer,
+                         inner));
+    }
+  }
+};
+
 // ------------------------------------------------------------------------------- recurrent cells
 // LSTMCell / GRUCell (neuronika-nn/src/lib.rs:450-626) as ONE forward and ONE backward node per step instead of the
 // ~15 nodes the reference composes them from: the two GEMMs write the gate pre-activations in f32 (kept for the tape's
@@ -1394,6 +1452,24 @@ nkg_var* unary_node(nkg_var* a, const Shape& out_shape, int out_dtype, TensorP& 
   merge(v, a);
   out_data = std::make_shared<Tensor>(a->ctx, out_shape, out_dtype);
   v->data = out_data;
+  return v;
+}
+
+// a view: the operand's memory and tapes under another shape (no kernel, no node); the gradient of a view is the same
+// memory with the view's shape
+nkg_var* view_of(nkg_var* a, const Shape& shape) {
+  nkg_var* v = new nkg_var(*a);
+  auto t = std::make_shared<Tensor>(a->ctx, shape, a->data->dtype);
+  t->base = a->data;
+  t->owned = false;
+  v->data = t;
+  if (a->diff()) {
+    auto g = std::make_shared<Gradient>(a->ctx, shape, a->grad->dtype);
+    g->alias = a->grad;
+    v->grad = g;
+  }
+  v->fwd_buf.clear();
+  v->bwd_buf.clear();
   return v;
 }
 
@@ -1866,20 +1942,7 @@ int nkg_flatten(nkg_var* a, nkg_var** out) {
     if (s.size() < 2) fail(NK_ERR_INVALID_ARG, "flatten: needs at least 2 dimensions");
     int64_t rest = 1;
     for (size_t i = 1; i < s.size(); ++i) rest *= s[i];
-    nkg_var* v = new nkg_var(*a);  // same tapes: a view records no node
-    auto t = std::make_shared<Tensor>(a->ctx, Shape{s[0], rest}, a->data->dtype);
-    t->base = a->data;
-    t->owned = false;
-    v->data = t;
-    if (a->diff()) {
-      // the gradient of a view is the same memory with the view's shape
-      auto g = std::make_shared<Gradient>(a->ctx, Shape{s[0], rest}, a->grad->dtype);
-      g->alias = a->grad;
-      v->grad = g;
-    }
-    v->fwd_buf.clear();
-    v->bwd_buf.clear();
-    *out = v;
+    *out = view_of(a, Shape{s[0], rest});
   });
 }
 
@@ -2177,6 +2240,111 @@ int nkg_chunks(nkg_var* a, int ndim, const int64_t* chunk_shape, int capacity, n
       }
       outs[i] = v;
     }
+  });
+}
+
+// var.rs:564-587 / 622-645, vardiff.rs:627-641 / 681-: one node for every operand count and every mix of Var and
+// VarDiff operands (the reference's four homogeneous methods and its Cat / Stack traits for mixed pairs)
+static void cat_impl(nkg_var* const* vars, int count, int axis, bool stack, nkg_var** out) {
+  const char* who = stack ? "stack" : "cat";
+  if (!vars || !out) fail(NK_ERR_INVALID_ARG, "%s: NULL", who);
+  if (count < 1) fail(NK_ERR_INVALID_ARG, "%s: needs at least one operand, got %d", who, count);
+  for (int i = 0; i < count; ++i)
+    if (!vars[i]) fail(NK_ERR_INVALID_ARG, "%s: operand %d is NULL", who, i);
+  nkg_var* a = vars[0];
+  const Shape& s0 = a->data->shape;
+  const int nd = (int)s0.size();
+  for (int i = 1; i < count; ++i) {
+    if (vars[i]->data->dtype != a->data->dtype)
+      fail(NK_ERR_INVALID_ARG, "%s: operand %d has another element type than operand 0", who, i);
+    if (vars[i]->ctx != a->ctx) fail(NK_ERR_INVALID_ARG, "%s: operand %d lives on another device than operand 0", who, i);
+    if ((int)vars[i]->data->shape.size() != nd)
+      fail(NK_ERR_INVALID_ARG, "%s: operand %d has %d dimensions, operand 0 has %d", who, i,
+           (int)vars[i]->data->shape.size(), nd);
+  }
+  Shape os = s0;
+  std::vector<int64_t> lens(count, 1);
+  int64_t outer = 1, inner = 1;
+  if (stack) {
+    if (axis < 0 || axis > nd) fail(NK_ERR_INVALID_ARG, "stack: axis %d out of range for %d-dimensional operands", axis, nd);
+    if (nd + 1 > NK_MAX_DIMS) fail(NK_ERR_INVALID_ARG, "stack: the result would have more than %d dimensions", NK_MAX_DIMS);
+    for (int i = 1; i < count; ++i)
+      for (int k = 0; k < nd; ++k)
+        if (vars[i]->data->shape[k] != s0[k])
+          fail(NK_ERR_INVALID_ARG, "stack: operand %d differs from operand 0 on axis %d (%lld vs %lld)", i, k,
+               (long long)vars[i]->data->shape[k], (long long)s0[k]);
+    for (int k = 0; k < axis; ++k) outer *= s0[k];
+    for (int k = axis; k < nd; ++k) inner *= s0[k];
+    os.insert(os.begin() + axis, count);
+  } else {
+    if (nd < 1) fail(NK_ERR_INVALID_ARG, "cat: operands must have at least one dimension");
+    if (axis < 0 || axis >= nd) fail(NK_ERR_INVALID_ARG, "cat: axis %d out of range for %d-dimensional operands", axis, nd);
+    os[axis] = 0;
+    for (int i = 0; i < count; ++i) {
+      const Shape& si = vars[i]->data->shape;
+      for (int k = 0; k < nd; ++k)
+        if (k != axis && si[k] != s0[k])
+          fail(NK_ERR_INVALID_ARG, "cat: operand %d differs from operand 0 on axis %d (%lld vs %lld)", i, k,
+               (long long)si[k], (long long)s0[k]);
+      lens[i] = si[axis];
+      os[axis] += si[axis];
+    }
+    int64_t len;
+    lanes(os, axis, outer, len, inner);
+  }
+  nk_ctx* ctx = a->ctx;
+  const int dt = a->data->dtype;
+  nkg_var* v = new_like(a);
+  for (int i = 0; i < count; ++i) {   // History::merge over every operand
+    v->fwd.insert(vars[i]->fwd.begin(), vars[i]->fwd.end());
+    v->bwd.insert(vars[i]->bwd.begin(), vars[i]->bwd.end());
+  }
+  v->data = std::make_shared<Tensor>(ctx, os, dt);
+  auto fw = std::make_shared<Concatenate>();
+  fw->ctx = ctx;
+  fw->data = v->data;
+  fw->lens = lens;
+  fw->outer = outer;
+  fw->inner = inner;
+  fw->stack = stack;
+  bool diff = false;
+  for (int i = 0; i < count; ++i) {
+    fw->operands.push_back(vars[i]->data);
+    diff = diff || vars[i]->diff();
+  }
+  const uint64_t id = push(v, fw);
+  if (diff) {
+    v->grad = std::make_shared<Gradient>(ctx, os, dt);
+    auto bw = std::make_shared<ConcatenateBackward>();
+    bw->ctx = ctx;
+    bw->gradient = v->grad;
+    for (int i = 0; i < count; ++i) bw->operand_grads.push_back(vars[i]->grad);
+    bw->lens = lens;
+    bw->outer = outer;
+    bw->inner = inner;
+    bw->stack = stack;
+    push_bwd(v, id, bw);
+  }
+  *out = v;
+}
+
+int nkg_cat(nkg_var* const* vars, int count, int axis, nkg_var** out) {
+  return guard([&] { cat_impl(vars, count, axis, false, out); });
+}
+
+int nkg_stack(nkg_var* const* vars, int count, int axis, nkg_var** out) {
+  return guard([&] { cat_impl(vars, count, axis, true, out); });
+}
+
+int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out) {
+  return guard([&] {
+    if (!a || !out) fail(NK_ERR_INVALID_ARG, "unsqueeze: NULL");
+    Shape s = a->data->shape;
+    if (axis < 0 || axis > (int)s.size())
+      fail(NK_ERR_INVALID_ARG, "unsqueeze: axis %d out of range for a %d-dimensional operand", axis, (int)s.size());
+    if (s.size() + 1 > NK_MAX_DIMS) fail(NK_ERR_INVALID_ARG, "unsqueeze: the result would have more than %d dimensions", NK_MAX_DIMS);
+    s.insert(s.begin() + axis, 1);
+    *out = view_of(a, s);
   });
 }
 

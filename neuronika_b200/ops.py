@@ -418,3 +418,39 @@ def chunk_bwd(dx: CuArray, g: CuArray, index: int, beta=1.0) -> CuArray:
     _ck(lib.nk_chunk_bwd(dx.device.ctx, dx.ptr, dx.dtype, g.ptr, g.dtype, dx.ndim, L.shape_arr(dx.shape),
                          L.shape_arr(g.shape), int(index), float(beta)), dx.device)
     return dx
+
+
+# ---------------------------------------------------------------- concatenation (csrc/nk_cat.cu)
+def _cat_view(shape, axis):
+    if not 0 <= axis < len(shape):
+        raise ValueError(f"cat: axis {axis} out of range for shape {tuple(shape)}")
+    return _lanes(shape, axis)
+
+
+def cat(xs, axis: int, out: CuArray | None = None) -> CuArray:
+    """The arrays side by side along `axis` (equal shapes on every other axis), bit exact; one launch per
+    NK_CAT_OPS_PER_LAUNCH operands."""
+    xs = list(xs)
+    shape = list(xs[0].shape)
+    outer, _, inner = _cat_view(shape, axis)
+    lens = [int(x.shape[axis]) for x in xs]
+    shape[axis] = sum(lens)
+    out = out or CuArray(xs[0].device, tuple(shape), xs[0].dtype)
+    ptrs = (L.vp * len(xs))(*[x.ptr.value for x in xs])
+    _ck(lib.nk_cat_fwd(out.device.ctx, out.ptr, ptrs, (L.i64 * len(xs))(*lens), len(xs), outer, inner, out.dtype),
+        out.device)
+    return out
+
+
+def cat_bwd(dxs, g: CuArray, axis: int, betas, lens=None):
+    """dxs[i] = betas[i]*dxs[i] + (slice i of g along `axis`), each in its own element type; a None entry gets nothing
+    (then `lens` gives every operand's length along `axis`)."""
+    dxs = list(dxs)
+    outer, _, inner = _cat_view(g.shape, axis)
+    lens = [int(d.shape[axis]) for d in dxs] if lens is None else [int(v) for v in lens]
+    n = len(dxs)
+    ptrs = (L.vp * n)(*[_ptr(d).value if d is not None else None for d in dxs])
+    dts = (L.i32 * n)(*[d.dtype if d is not None else F32 for d in dxs])
+    _ck(lib.nk_cat_bwd(g.device.ctx, ptrs, dts, (L.f32 * n)(*[float(b) for b in betas]), g.ptr, g.dtype,
+                       (L.i64 * n)(*lens), n, outer, inner), g.device)
+    return dxs

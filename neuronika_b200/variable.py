@@ -81,6 +81,9 @@ _G = {
     "nkg_chunks": (i32, [vp, i32, pi64, i32, pvp, C.POINTER(i32)]),
     "nkg_lstm_cell": (i32, [vp, vp, vp, vp, vp, vp, vp, pvp, pvp]),
     "nkg_gru_cell": (i32, [vp, vp, vp, vp, vp, vp, pvp]),
+    "nkg_cat": (i32, [pvp, i32, i32, pvp]),
+    "nkg_stack": (i32, [pvp, i32, i32, pvp]),
+    "nkg_unsqueeze": (i32, [vp, i32, pvp]),
 }
 for _n, (_r, _a) in _G.items():
     _f = getattr(lib, _n)
@@ -260,6 +263,21 @@ class Var:
         _ck(lib.nkg_chunks(self._h, len(cs), L.shape_arr(cs), count.value, outs, C.byref(count)))
         return [self._wrap(vp(outs[i])) for i in range(count.value)]
 
+    def cat(self, others, axis: int):
+        """`cat(variables, axis)` (var.rs:564-587, vardiff.rs:627-641): the receiver and `others` side by side along
+        `axis`, as ONE node; differentiable when any operand is, and only those operands receive gradients."""
+        return _join(lib.nkg_cat, [self, *others], axis)
+
+    def stack(self, others, axis: int):
+        """`stack(variables, axis)` (var.rs:622-645, vardiff.rs:681-): the receiver and `others` (one shape) along a new
+        axis, as ONE node."""
+        return _join(lib.nkg_stack, [self, *others], axis)
+
+    def unsqueeze(self, axis: int):
+        """`unsqueeze(axis)` (var.rs:425-431): a new axis of length 1.  A view like flatten(): no kernel and no node
+        (the reference records one)."""
+        return self._unary(lib.nkg_unsqueeze, int(axis))
+
     def item(self) -> float:
         return float(self.data().reshape(()))
 
@@ -327,6 +345,24 @@ class VarDiff(Var):
         cb = GRAD_RS_HOOK(lambda _user, pushed: fn(int(pushed)))
         self._rs_ref = (cb, arr)
         _ck(lib.nkg_set_grad_rs(self._h, int(world), int(rank), arr, C.cast(cb, vp), None))
+
+
+# ---- concatenation (neuronika-variable/src/lib.rs:258, 281)
+def _join(fn, vars, axis):
+    handles = (vp * len(vars))(*[v._h.value for v in vars])
+    out = vp()
+    _ck(fn(handles, len(vars), int(axis), C.byref(out)))
+    return vars[0]._wrap(out)
+
+
+def cat(lhs: Var, rhs: Var, axis: int):
+    """`cat(lhs, rhs, axis)`: the two side by side along `axis`, any mix of Var and VarDiff."""
+    return _join(lib.nkg_cat, [lhs, rhs], axis)
+
+
+def stack(lhs: Var, rhs: Var, axis: int):
+    """`stack(lhs, rhs, axis)`: the two (one shape) along a new axis, any mix of Var and VarDiff."""
+    return _join(lib.nkg_stack, [lhs, rhs], axis)
 
 
 # ---- recurrent cells (one fused node per step; see include/nk_graph.h)
