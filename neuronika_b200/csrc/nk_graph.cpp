@@ -214,13 +214,17 @@ using GradientP = std::shared_ptr<Gradient>;
 
 // ------------------------------------------------------------------------------- node traits
 struct Forward {
+  nk_ctx* ctx;
   bool skip = false;  // fused into a consumer
+  explicit Forward(nk_ctx* c) : ctx(c) {}
   virtual ~Forward() {}
   virtual void forward() = 0;
   virtual const char* name() const = 0;
 };
 // set by nkg_backward around each node: position of the running node in the reverse tape
 static thread_local int g_bwd_pos = -1;
+// A backward node reports every gradient it accumulates into once its last write to it is launched: the hook of a
+// gradient fires when the node that reports it is that gradient's last writer in the running pass.
 static inline void grad_written(const GradientP& g) {
   if (!g) return;
   Gradient* r = g->root();
@@ -231,14 +235,18 @@ static inline void grad_written(const GradientP& g) {
 }
 
 struct Backward {
+  nk_ctx* ctx;
   GradientP gradient;  // gradient of this node's output
   bool skip = false;
   bool single_pass = false;  // a fusion that is exact for ONE backward pass was applied to this node
   int runs = 0;        // backward() calls so far (a second pass over the same tape must see un-aliased gradients)
+  Backward(nk_ctx* c, GradientP g) : ctx(c), gradient(std::move(g)) {}
   virtual ~Backward() {}
   virtual void backward() = 0;
   virtual void targets(std::vector<Gradient*>& out) = 0;  // gradients this node accumulates into
   virtual const char* name() const = 0;
+  // called before every backward pass after the first: undo what a fusion made exact for one pass only
+  virtual void unalias() {}
   virtual void no_grad() {
     if (gradient) gradient->no_grad();
   }
@@ -249,18 +257,24 @@ struct Backward {
 using ForwardP = std::shared_ptr<Forward>;
 using BackwardP = std::shared_ptr<Backward>;
 
+// the non-null operand gradients of a node, as targets()
+static void add_targets(std::vector<Gradient*>& out, std::initializer_list<const GradientP*> grads) {
+  for (const GradientP* g : grads)
+    if (*g) out.push_back((*g)->root());
+}
+
 static void gemm(nk_ctx* ctx, bool ta, bool tb, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda,
                  const void* B, int64_t ldb, float beta, void* C, int ab_dt, int c_dt, const void* bias = nullptr,
                  int bias_dt = NK_F32, int relu = 0) {
   ck(ctx, nk_gemm_bias_act(ctx, ta, tb, M, N, K, 1.f, A, lda, B, ldb, beta, C, N, ab_dt, c_dt, bias, bias_dt, relu));
 }
 
-// A backward kernel that produces its result in element type `kdt` accumulating into a gradient that may have another
-// element type (a bf16 leaf with an f32 gradient, requires_grad(grad_dtype)): same type -> the kernel writes the
-// gradient directly with the accumulate mode `beta`; otherwise it writes a temporary (beta = 0) which is then added
-// with the mixed-type axpy of nk_unbroadcast_acc.
+// The one write protocol of the backward nodes: kernel(dst, beta) accumulates a result it produces in element type
+// `kdt` into the gradient g.  Same type -> the kernel writes the gradient directly with Gradient::acc()'s accumulate
+// mode; otherwise (a bf16 leaf with an f32 gradient, requires_grad(grad_dtype)) it writes a temporary (beta = 0) which
+// is then added with the mixed-type axpy of nk_unbroadcast_acc.
 template <typename F>
-static void acc_typed(nk_ctx* ctx, const GradientP& g, int kdt, F&& kernel) {
+static void accumulate(nk_ctx* ctx, const GradientP& g, int kdt, F&& kernel) {
   float beta;
   void* d = g->acc(&beta);
   if (g->dtype == kdt) {
@@ -279,14 +293,19 @@ static void acc_typed(nk_ctx* ctx, const GradientP& g, int kdt, F&& kernel) {
   }
   ck(ctx, nk_free(ctx, tmp));
 }
+// ... for a kernel that writes the gradient's own element type
+template <typename F>
+static void accumulate(nk_ctx* ctx, const GradientP& g, F&& kernel) {
+  accumulate(ctx, g, g->dtype, kernel);
+}
 
 // ------------------------------------------------------------------------------- matmul nodes
 // MatrixMatrixMul (matrix_matrix_mul/mod.rs:11-41) and MatrixMatrixMulT (matrix_matrix_mul_t/mod.rs:11-41)
 struct MatMul : Forward {
-  nk_ctx* ctx;
   TensorP left, right, data;
   bool t;  // true: C = A.B^T (mm_t)
-  MatMul(nk_ctx* c, TensorP l, TensorP r, TensorP d, bool tt) : ctx(c), left(l), right(r), data(d), t(tt) {}
+  MatMul(nk_ctx* c, TensorP l, TensorP r, TensorP d, bool tt)
+      : Forward(c), left(std::move(l)), right(std::move(r)), data(std::move(d)), t(tt) {}
   const char* name() const override { return t ? "MatrixMatrixMulT" : "MatrixMatrixMul"; }
   void forward() override { run(nullptr); }
   void run(Tensor* bias, Tensor* out = nullptr, int relu = 0) {
@@ -299,7 +318,6 @@ struct MatMul : Forward {
 
 // dA += G.B^T | G.B ; dB += A^T.G | G^T.A   (matrix_matrix_mul/mod.rs:43-126, matrix_matrix_mul_t/mod.rs:43-126)
 struct MatMulBackward : Backward {
-  nk_ctx* ctx;
   TensorP left_data, right_data;
   GradientP left_grad, right_grad;  // either may be null (operand not differentiable)
   bool t;
@@ -310,14 +328,16 @@ struct MatMulBackward : Backward {
   // ... and the bias gradient of the layer below (the un-broadcast of its Addition's (K) row bias) is summed in the
   // same epilogue (nk_gemm_relu_bwd_colsum): the AdditionBackward then skips its right operand
   GradientP left_colsum;
+  MatMulBackward(nk_ctx* c, GradientP g, TensorP ld, TensorP rd, GradientP lg, GradientP rg, bool tt)
+      : Backward(c, std::move(g)), left_data(std::move(ld)), right_data(std::move(rd)), left_grad(std::move(lg)),
+        right_grad(std::move(rg)), t(tt) {}
   const char* name() const override { return t ? "MatrixMatrixMulTBackward" : "MatrixMatrixMulBackward"; }
   void targets(std::vector<Gradient*>& out) override {
     if (left_dst)
-      out.push_back(left_dst->root());
-    else if (left_grad)
-      out.push_back(left_grad->root());
-    if (left_dst && left_colsum) out.push_back(left_colsum->root());
-    if (right_grad) out.push_back(right_grad->root());
+      add_targets(out, {&left_dst, &left_colsum});
+    else
+      add_targets(out, {&left_grad});
+    add_targets(out, {&right_grad});
   }
   void backward() override {
     const int64_t M = left_data->shape[0], K = left_data->shape[1];
@@ -345,7 +365,7 @@ struct MatMulBackward : Backward {
         else
           gemm(ctx, true, false, rows, cols, M, A, rows, B, cols, beta, d, gdt, right_grad->dtype);
         if (r->rs_hook) r->rs_hook(r->rs_user, push ? 1 : 0);
-        chunks = 0;
+        chunks = 0;  // reported after the dX GEMM, below
       } else if (r == right_grad.get() && r->hook && r->hook_chunks > 1 && r->last_writer == g_bwd_pos && !r->hook_fired &&
           rows % (int64_t(r->hook_chunks) * 128) == 0)
         chunks = r->hook_chunks;
@@ -404,17 +424,20 @@ struct MatMulBackward : Backward {
         gemm(ctx, false, true, M, K, N, G, N, right_data->rptr(), N, beta, d, gdt, left_grad->dtype);
       grad_written(left_grad);
     }
+    grad_written(right_grad);  // a gradient with a reduce-scatter plan
   }
 };
 
 // ------------------------------------------------------------------------------- addition
 struct Convolution;
+struct ConvolutionBackward;
 struct Addition : Forward {  // addition/mod.rs:11-50
-  nk_ctx* ctx;
   TensorP left, right, data;
   std::shared_ptr<MatMul> fused_gemm;        // peephole: data = mm_t(..) + right in one kernel
   std::shared_ptr<Convolution> fused_conv;   // peephole: data = convolution(..) + bias(Cout,1,1) in one kernel
   TensorP fused_relu_out;                    // peephole: the consumer ReLU's output, written by the GEMM epilogue
+  Addition(nk_ctx* c, TensorP l, TensorP r, TensorP d)
+      : Forward(c), left(std::move(l)), right(std::move(r)), data(std::move(d)) {}
   void run_fused_conv();
   const char* name() const override { return "Addition"; }
   void forward() override {
@@ -436,51 +459,56 @@ struct Addition : Forward {  // addition/mod.rs:11-50
 };
 
 struct AdditionBackward : Backward {  // addition/mod.rs:52-135 (Left, Right and the composite)
-  nk_ctx* ctx;
   GradientP left_grad, right_grad;
   bool left_aliased = false, right_aliased = false;  // right_aliased: the bias gradient is produced by the fused conv dW
   bool right_fused = false;   // the bias gradient is summed in the epilogue of the dX GEMM above (MatMulBackward::left_colsum)
+  ConvolutionBackward* bias_producer = nullptr;  // the convolution whose dW kernel produces right_grad (right_aliased)
+  AdditionBackward(nk_ctx* c, GradientP g, GradientP lg, GradientP rg)
+      : Backward(c, std::move(g)), left_grad(std::move(lg)), right_grad(std::move(rg)) {}
   const char* name() const override { return "AdditionBackward"; }
-  void acc(GradientP& dst, bool aliased) {
+  void acc(const GradientP& dst, bool aliased) {
     if (!dst || aliased) return;
-    float beta;
-    void* d = dst->acc(&beta);
-    ck(ctx, nk_unbroadcast_acc(ctx, d, dst->dtype, (int)dst->shape.size(), dst->shape.data(), gradient->get(),
-                               gradient->dtype, (int)gradient->shape.size(), gradient->shape.data(), beta));
+    accumulate(ctx, dst, [&](void* d, float beta) {
+      ck(ctx, nk_unbroadcast_acc(ctx, d, dst->dtype, (int)dst->shape.size(), dst->shape.data(), gradient->get(),
+                                 gradient->dtype, (int)gradient->shape.size(), gradient->shape.data(), beta));
+    });
     grad_written(dst);
   }
   void targets(std::vector<Gradient*>& out) override {
-    if (left_grad) out.push_back(left_grad->root());
-    if (right_grad && !right_fused) out.push_back(right_grad->root());
+    add_targets(out, {&left_grad});
+    if (!right_fused) add_targets(out, {&right_grad});
   }
   void backward() override {
     acc(left_grad, left_aliased);
     acc(right_grad, right_aliased || right_fused);
+    if (left_aliased) grad_written(left_grad);    // written by the consumers of this node's output
+    if (right_aliased) grad_written(right_grad);
   }
+  void unalias() override;
 };
 
 // ------------------------------------------------------------------------------- unary / softmax
 struct ReLU : Forward {  // relu/mod.rs:11-38
-  nk_ctx* ctx;
   TensorP operand, data;
+  ReLU(nk_ctx* c, TensorP x, TensorP d) : Forward(c), operand(std::move(x)), data(std::move(d)) {}
   const char* name() const override { return "ReLU"; }
   void forward() override {
     ck(ctx, nk_relu_fwd(ctx, data->wptr(), operand->rptr(), size_t(data->n()), data->dtype));
   }
 };
 struct ReLUBackward : Backward {  // relu/mod.rs:40-79
-  nk_ctx* ctx;
   TensorP operand_data;
   GradientP operand_grad;
+  ReLUBackward(nk_ctx* c, GradientP g, TensorP x, GradientP xg)
+      : Backward(c, std::move(g)), operand_data(std::move(x)), operand_grad(std::move(xg)) {}
   const char* name() const override { return "ReLUBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {
     const void* g = gradient->get();
-    acc_typed(ctx, operand_grad, operand_data->dtype, [&](void* d, float beta) {
+    accumulate(ctx, operand_grad, operand_data->dtype, [&](void* d, float beta) {
       ck(ctx, nk_relu_bwd(ctx, d, operand_data->rptr(), g, size_t(operand_data->n()), operand_data->dtype, beta));
     });
+    grad_written(operand_grad);
   }
 };
 
@@ -492,10 +520,11 @@ static void lanes(const Shape& s, int axis, int64_t& outer, int64_t& len, int64_
 }
 
 struct Softmax : Forward {  // softmax/mod.rs:11-53, logsoftmax/mod.rs:11-53
-  nk_ctx* ctx;
   TensorP operand, data;
   int axis;
   bool log;
+  Softmax(nk_ctx* c, TensorP x, TensorP d, int ax, bool lg)
+      : Forward(c), operand(std::move(x)), data(std::move(d)), axis(ax), log(lg) {}
   const char* name() const override { return log ? "LogSoftmax" : "Softmax"; }
   void forward() override {
     int64_t o, l, i;
@@ -504,55 +533,56 @@ struct Softmax : Forward {  // softmax/mod.rs:11-53, logsoftmax/mod.rs:11-53
   }
 };
 struct SoftmaxBackward : Backward {  // softmax/mod.rs:55-104, logsoftmax/mod.rs:55-102
-  nk_ctx* ctx;
   TensorP data;
   GradientP operand_grad;
   int axis;
   bool log;
+  SoftmaxBackward(nk_ctx* c, GradientP g, TensorP d, GradientP xg, int ax, bool lg)
+      : Backward(c, std::move(g)), data(std::move(d)), operand_grad(std::move(xg)), axis(ax), log(lg) {}
   const char* name() const override { return log ? "LogSoftmaxBackward" : "SoftmaxBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {
     int64_t o, l, i;
     lanes(data->shape, axis, o, l, i);
     const void* g = gradient->get();
-    acc_typed(ctx, operand_grad, data->dtype, [&](void* d, float beta) {
+    accumulate(ctx, operand_grad, data->dtype, [&](void* d, float beta) {
       ck(ctx, (log ? nk_log_softmax_bwd : nk_softmax_bwd)(ctx, d, data->rptr(), g, o, l, i, data->dtype, beta));
     });
+    grad_written(operand_grad);
   }
 };
 
 // ------------------------------------------------------------------------------- reductions / losses
 struct SumMean : Forward {  // sum/mod.rs:11-34, mean/mod.rs:11-34
-  nk_ctx* ctx;
   TensorP operand, data;
   bool mean;
+  SumMean(nk_ctx* c, TensorP x, TensorP d, bool m) : Forward(c), operand(std::move(x)), data(std::move(d)), mean(m) {}
   const char* name() const override { return mean ? "Mean" : "Sum"; }
   void forward() override {
     ck(ctx, nk_sum_fwd(ctx, (float*)data->wptr(), operand->rptr(), size_t(operand->n()), operand->dtype, mean));
   }
 };
 struct SumMeanBackward : Backward {  // sum/mod.rs:36-66, mean/mod.rs:36-71
-  nk_ctx* ctx;
   GradientP operand_grad;
   bool mean;
+  SumMeanBackward(nk_ctx* c, GradientP g, GradientP xg, bool m)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), mean(m) {}
   const char* name() const override { return mean ? "MeanBackward" : "SumBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {
-    float beta;
-    void* d = operand_grad->acc(&beta);
-    ck(ctx, nk_sum_bwd(ctx, d, (const float*)gradient->get(), size_t(operand_grad->n()), operand_grad->dtype, mean,
-                       beta));
+    accumulate(ctx, operand_grad, [&](void* d, float beta) {
+      ck(ctx, nk_sum_bwd(ctx, d, (const float*)gradient->get(), size_t(operand_grad->n()), operand_grad->dtype, mean,
+                         beta));
+    });
+    grad_written(operand_grad);
   }
 };
 
 struct Loss : Forward {  // squared_error/mod.rs:11-58, nll/mod.rs:11-68
-  nk_ctx* ctx;
   TensorP input, target, data;
   bool mean, nll;
+  Loss(nk_ctx* c, TensorP x, TensorP t, TensorP d, bool m, bool n)
+      : Forward(c), input(std::move(x)), target(std::move(t)), data(std::move(d)), mean(m), nll(n) {}
   const char* name() const override { return nll ? "NegativeLogLikelihood" : "SquaredError"; }
   void forward() override {
     if (nll)
@@ -564,32 +594,34 @@ struct Loss : Forward {  // squared_error/mod.rs:11-58, nll/mod.rs:11-68
   }
 };
 struct LossBackward : Backward {  // squared_error/mod.rs:60-122, nll/mod.rs:70-133
-  nk_ctx* ctx;
   TensorP input, target;
   GradientP input_grad;
   bool mean, nll;
+  LossBackward(nk_ctx* c, GradientP g, TensorP x, TensorP t, GradientP xg, bool m, bool n)
+      : Backward(c, std::move(g)), input(std::move(x)), target(std::move(t)), input_grad(std::move(xg)), mean(m),
+        nll(n) {}
   const char* name() const override { return nll ? "NegativeLogLikelihoodBackward" : "SquaredErrorBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (input_grad) out.push_back(input_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad}); }
   void backward() override {
     const float* g = (const float*)gradient->get();
-    acc_typed(ctx, input_grad, input->dtype, [&](void* d, float beta) {
+    accumulate(ctx, input_grad, input->dtype, [&](void* d, float beta) {
       if (nll)
         ck(ctx, nk_nll_bwd(ctx, d, target->rptr(), target->dtype, g, input->shape[0], input->shape[1], input->dtype,
                            mean, beta));
       else
         ck(ctx, nk_mse_bwd(ctx, d, input->rptr(), target->rptr(), g, size_t(input->n()), input->dtype, mean, beta));
     });
+    grad_written(input_grad);
   }
 };
 
 // ------------------------------------------------------------------------------- pad / conv / flatten
 struct Pad : Forward {  // pad/mod.rs:63-129 with Constant / Zero modes
-  nk_ctx* ctx;
   TensorP operand, data;
   int64_t ph, pw;
   float value;
+  Pad(nk_ctx* c, TensorP x, TensorP d, int64_t h, int64_t w, float v)
+      : Forward(c), operand(std::move(x)), data(std::move(d)), ph(h), pw(w), value(v) {}
   const char* name() const override { return "Pad"; }
   void forward() override {
     const Shape& s = operand->shape;
@@ -597,19 +629,19 @@ struct Pad : Forward {  // pad/mod.rs:63-129 with Constant / Zero modes
   }
 };
 struct PadBackward : Backward {  // pad/mod.rs:131-182
-  nk_ctx* ctx;
   GradientP operand_grad;
   int64_t ph, pw;
+  PadBackward(nk_ctx* c, GradientP g, GradientP xg, int64_t h, int64_t w)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), ph(h), pw(w) {}
   const char* name() const override { return "PadBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {
     const Shape& s = operand_grad->shape;
     const void* g = gradient->get();
-    acc_typed(ctx, operand_grad, gradient->dtype, [&](void* d, float beta) {
+    accumulate(ctx, operand_grad, gradient->dtype, [&](void* d, float beta) {
       ck(ctx, nk_pad2d_bwd(ctx, d, g, s[0] * s[1], s[2], s[3], ph, pw, gradient->dtype, beta));
     });
+    grad_written(operand_grad);
   }
 };
 
@@ -617,9 +649,10 @@ struct ConvArgs {
   int64_t n, cin, h, w, cout, kh, kw, sh, sw, dh, dw, groups;
 };
 struct Convolution : Forward {  // convolution/mod.rs:296-355
-  nk_ctx* ctx;
   TensorP input, kernel, data;
   ConvArgs a;
+  Convolution(nk_ctx* c, TensorP x, TensorP k, TensorP d, const ConvArgs& args)
+      : Forward(c), input(std::move(x)), kernel(std::move(k)), data(std::move(d)), a(args) {}
   const char* name() const override { return "Convolution"; }
   void forward() override { run(nullptr, nullptr); }
   void run(Tensor* bias, Tensor* out, int relu = 0) {
@@ -635,17 +668,15 @@ void Addition::run_fused_conv() {
     fused_conv->run(right.get(), data.get());
 }
 struct ConvolutionBackward : Backward {  // convolution/mod.rs:357-510: input first, then kernel (:380-388)
-  nk_ctx* ctx;
   TensorP input, kernel;
   GradientP input_grad, kernel_grad;
   GradientP bias_grad;  // set by the peephole when the (Cout,1,1) bias add was fused: db rides along with dW
   ConvArgs a;
+  ConvolutionBackward(nk_ctx* c, GradientP g, TensorP x, TensorP k, GradientP xg, GradientP kg, const ConvArgs& args)
+      : Backward(c, std::move(g)), input(std::move(x)), kernel(std::move(k)), input_grad(std::move(xg)),
+        kernel_grad(std::move(kg)), a(args) {}
   const char* name() const override { return "ConvolutionBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (input_grad) out.push_back(input_grad->root());
-    if (kernel_grad) out.push_back(kernel_grad->root());
-    if (bias_grad) out.push_back(bias_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad, &kernel_grad, &bias_grad}); }
   void backward() override {
     void* dbias = nullptr;
     if (bias_grad) {
@@ -662,7 +693,7 @@ struct ConvolutionBackward : Backward {  // convolution/mod.rs:357-510: input fi
       }
     }
     // dX is produced in the element type of the output gradient; an input gradient of another type goes through
-    // acc_typed (and then the two halves run as separate kernels)
+    // accumulate()'s temporary (and then the two halves run as separate kernels)
     const bool dx_same = !input_grad || input_grad->dtype == gradient->dtype;
     Gradient* gr = gradient->root();
     if (input_grad && kernel_grad && dx_same) {  // both halves: one pass over the output gradient where the kernels allow it
@@ -686,31 +717,57 @@ struct ConvolutionBackward : Backward {  // convolution/mod.rs:357-510: input fi
     } else {
       if (input_grad) {
         const void* g = gradient->get();
-        acc_typed(ctx, input_grad, gradient->dtype, [&](void* d, float beta) {
+        accumulate(ctx, input_grad, gradient->dtype, [&](void* d, float beta) {
           ck(ctx, nk_conv2d_bwd_input(ctx, d, g, kernel->rptr(), a.n, a.cin, a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw,
                                       a.dh, a.dw, a.groups, gradient->dtype, beta));
         });
         grad_written(input_grad);
       }
       if (kernel_grad) {
-        float beta;
-        void* d = kernel_grad->acc(&beta);
-        ck(ctx, nk_conv2d_bwd_kernel(ctx, d, kernel_grad->dtype, dbias, gradient->get(), input->rptr(), a.n, a.cin,
-                                     a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw, a.dh, a.dw, a.groups, gradient->dtype,
-                                     beta));
+        accumulate(ctx, kernel_grad, [&](void* d, float beta) {
+          ck(ctx, nk_conv2d_bwd_kernel(ctx, d, kernel_grad->dtype, dbias, gradient->get(), input->rptr(), a.n, a.cin,
+                                       a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw, a.dh, a.dw, a.groups, gradient->dtype,
+                                       beta));
+        });
         grad_written(kernel_grad);
       }
     }
-    if (bias_grad) grad_written(bias_grad);
+    grad_written(bias_grad);
   }
 };
+
+// The aliasing peephole (dL += G with one consumer => L.grad IS G) is exact for ONE backward pass per tape.  The
+// reference accumulates into every gradient, intermediates included, on every pass (nothing zeroes them), so on a
+// repeated backward() the addend's gradient and the sum's gradient diverge: give the addend its own buffer, holding
+// what the reference would hold after the passes so far (= the sum's gradient at the end of the last pass).
+void AdditionBackward::unalias() {
+  if (!left_aliased || !left_grad || !left_grad->alias) return;
+  Gradient* g = left_grad.get();
+  Gradient* src = g->root();
+  const size_t bytes = size_t(g->n()) * esize(g->dtype);
+  void* own = nullptr;
+  ck(g->ctx, nk_alloc_uninit(g->ctx, bytes, &own));
+  ck(g->ctx, nk_d2d(g->ctx, own, src->get(), bytes));
+  g->alias.reset();
+  g->ptr = own;
+  g->owned = true;
+  g->is_zero = false;
+  g->stale = false;
+  left_aliased = false;
+  if (right_aliased) {  // the bias gradient rode along with the convolution's dW: back to its own un-broadcast
+    bias_producer->bias_grad.reset();
+    bias_producer = nullptr;
+    right_aliased = false;
+  }
+}
 
 // ------------------------------------------------------------------------------- sub / mul / div (broadcasting)
 // subtraction/mod.rs:11-172, multiplication/mod.rs:11-185, division/mod.rs:11-185
 struct Binary : Forward {
-  nk_ctx* ctx;
   TensorP left, right, data;
   int op;
+  Binary(nk_ctx* c, TensorP l, TensorP r, TensorP d, int o)
+      : Forward(c), left(std::move(l)), right(std::move(r)), data(std::move(d)), op(o) {}
   const char* name() const override {
     return op == NK_BIN_SUB ? "Subtraction" : op == NK_BIN_MUL ? "Multiplication" : "Division";
   }
@@ -721,24 +778,23 @@ struct Binary : Forward {
   }
 };
 struct BinaryBackward : Backward {
-  nk_ctx* ctx;
   TensorP left_data, right_data;
   GradientP left_grad, right_grad;  // either may be null
   int op;
+  BinaryBackward(nk_ctx* c, GradientP g, TensorP ld, TensorP rd, GradientP lg, GradientP rg, int o)
+      : Backward(c, std::move(g)), left_data(std::move(ld)), right_data(std::move(rd)), left_grad(std::move(lg)),
+        right_grad(std::move(rg)), op(o) {}
   const char* name() const override {
     return op == NK_BIN_SUB ? "SubtractionBackward" : op == NK_BIN_MUL ? "MultiplicationBackward" : "DivisionBackward";
   }
-  void targets(std::vector<Gradient*>& out) override {
-    if (left_grad) out.push_back(left_grad->root());
-    if (right_grad) out.push_back(right_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&left_grad, &right_grad}); }
   void side(int sd, const GradientP& dst) {
     if (!dst) return;
-    float beta;
-    void* d = dst->acc(&beta);
-    ck(ctx, nk_binary_bcast_bwd(ctx, op, sd, d, dst->dtype, gradient->get(), left_data->rptr(), right_data->rptr(),
-                                gradient->dtype, (int)left_data->shape.size(), left_data->shape.data(),
-                                (int)right_data->shape.size(), right_data->shape.data(), beta));
+    accumulate(ctx, dst, [&](void* d, float beta) {
+      ck(ctx, nk_binary_bcast_bwd(ctx, op, sd, d, dst->dtype, gradient->get(), left_data->rptr(), right_data->rptr(),
+                                  gradient->dtype, (int)left_data->shape.size(), left_data->shape.data(),
+                                  (int)right_data->shape.size(), right_data->shape.data(), beta));
+    });
     grad_written(dst);
   }
   void backward() override {  // left first, then right, like the composite nodes (e.g. multiplication/mod.rs:176-181)
@@ -756,27 +812,27 @@ static const char* unary_name(int op, bool bwd) {
   return (bwd ? b : f)[op];
 }
 struct Unary : Forward {
-  nk_ctx* ctx;
   TensorP operand, data;
   int op, iparam;
+  Unary(nk_ctx* c, TensorP x, TensorP d, int o, int ip)
+      : Forward(c), operand(std::move(x)), data(std::move(d)), op(o), iparam(ip) {}
   const char* name() const override { return unary_name(op, false); }
   void forward() override {
     ck(ctx, nk_unary_fwd(ctx, op, data->wptr(), operand->rptr(), size_t(data->n()), data->dtype, iparam));
   }
 };
 struct UnaryBackward : Backward {
-  nk_ctx* ctx;
   TensorP saved;  // the node's output (exp, sqrt, sigmoid, tanh) or its input (ln, softplus, leaky_relu, powi)
   GradientP operand_grad;
   int op, iparam;
+  UnaryBackward(nk_ctx* c, GradientP g, TensorP s, GradientP xg, int o, int ip)
+      : Backward(c, std::move(g)), saved(std::move(s)), operand_grad(std::move(xg)), op(o), iparam(ip) {}
   const char* name() const override { return unary_name(op, true); }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {
     const void* g = gradient->get();
     const void* sv = saved ? saved->rptr() : nullptr;
-    acc_typed(ctx, operand_grad, gradient->dtype, [&](void* d, float beta) {
+    accumulate(ctx, operand_grad, gradient->dtype, [&](void* d, float beta) {
       ck(ctx, nk_unary_bwd(ctx, op, d, sv, g, size_t(gradient->n()), gradient->dtype, iparam, beta));
     });
     grad_written(operand_grad);
@@ -785,8 +841,8 @@ struct UnaryBackward : Backward {
 
 // ------------------------------------------------------------------------------- transpose (transpose/mod.rs:11-75)
 struct Transpose : Forward {
-  nk_ctx* ctx;
   TensorP operand, data;
+  Transpose(nk_ctx* c, TensorP x, TensorP d) : Forward(c), operand(std::move(x)), data(std::move(d)) {}
   const char* name() const override { return "Transpose"; }
   void forward() override {
     ck(ctx, nk_transpose(ctx, data->wptr(), data->dtype, operand->rptr(), operand->dtype, (int)operand->shape.size(),
@@ -794,17 +850,15 @@ struct Transpose : Forward {
   }
 };
 struct TransposeBackward : Backward {
-  nk_ctx* ctx;
   GradientP operand_grad;
+  TransposeBackward(nk_ctx* c, GradientP g, GradientP xg) : Backward(c, std::move(g)), operand_grad(std::move(xg)) {}
   const char* name() const override { return "TransposeBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {  // dX += G^T
-    float beta;
-    void* d = operand_grad->acc(&beta);
-    ck(ctx, nk_transpose(ctx, d, operand_grad->dtype, gradient->get(), gradient->dtype, (int)gradient->shape.size(),
-                         gradient->shape.data(), beta));
+    accumulate(ctx, operand_grad, [&](void* d, float beta) {
+      ck(ctx, nk_transpose(ctx, d, operand_grad->dtype, gradient->get(), gradient->dtype, (int)gradient->shape.size(),
+                           gradient->shape.data(), beta));
+    });
     grad_written(operand_grad);
   }
 };
@@ -813,11 +867,12 @@ struct TransposeBackward : Backward {
 // Pad<D, T: PaddingMode> over (N, C, s...) with 1..3 sample dims (pad/mod.rs:20-182; modes pad/{constant,zero,
 // reflective,replicative}/mod.rs).  The 2-d constant case keeps its own node (Pad above).
 struct PadNd : Forward {
-  nk_ctx* ctx;
   TensorP operand, data;
   int nsp, mode;
   int64_t pad[3];
   float value;
+  PadNd(nk_ctx* c, TensorP x, TensorP d, int n, const int64_t* p, int m, float v)
+      : Forward(c), operand(std::move(x)), data(std::move(d)), nsp(n), mode(m), pad{p[0], p[1], p[2]}, value(v) {}
   const char* name() const override { return "Pad"; }
   void forward() override {
     const Shape& s = operand->shape;
@@ -826,18 +881,17 @@ struct PadNd : Forward {
   }
 };
 struct PadNdBackward : Backward {
-  nk_ctx* ctx;
   GradientP operand_grad;
   int nsp;
   int64_t pad[3];
+  PadNdBackward(nk_ctx* c, GradientP g, GradientP xg, int n, const int64_t* p)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), nsp(n), pad{p[0], p[1], p[2]} {}
   const char* name() const override { return "PadBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {
     const Shape& s = operand_grad->shape;
     const void* g = gradient->get();
-    acc_typed(ctx, operand_grad, gradient->dtype, [&](void* d, float beta) {
+    accumulate(ctx, operand_grad, gradient->dtype, [&](void* d, float beta) {
       ck(ctx, nk_padnd_bwd(ctx, d, g, s[0] * s[1], nsp, s.data() + 2, pad, gradient->dtype, beta));
     });
     grad_written(operand_grad);
@@ -847,9 +901,10 @@ struct PadNdBackward : Backward {
 // ------------------------------------------------------------------------------- mv / vm / vv
 // matrix_vector_mul/mod.rs:11-129, vector_matrix_mul/mod.rs:11-129, vector_vector_mul/mod.rs:11-91
 struct MatVec : Forward {
-  nk_ctx* ctx;
   TensorP mat, vec, data;
   bool vm;  // true: y = v.A
+  MatVec(nk_ctx* c, TensorP m, TensorP v, TensorP d, bool tvm)
+      : Forward(c), mat(std::move(m)), vec(std::move(v)), data(std::move(d)), vm(tvm) {}
   const char* name() const override { return vm ? "VectorMatrixMul" : "MatrixVectorMul"; }
   void forward() override {
     ck(ctx, nk_gemv(ctx, vm ? 1 : 0, mat->shape[0], mat->shape[1], mat->rptr(), vec->rptr(), 0.f, data->wptr(),
@@ -857,33 +912,32 @@ struct MatVec : Forward {
   }
 };
 struct MatVecBackward : Backward {
-  nk_ctx* ctx;
   TensorP mat, vec;
   GradientP mat_grad, vec_grad;
   bool vm;
+  MatVecBackward(nk_ctx* c, GradientP g, TensorP m, TensorP v, GradientP mg, GradientP vg, bool tvm)
+      : Backward(c, std::move(g)), mat(std::move(m)), vec(std::move(v)), mat_grad(std::move(mg)),
+        vec_grad(std::move(vg)), vm(tvm) {}
   const char* name() const override { return vm ? "VectorMatrixMulBackward" : "MatrixVectorMulBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (mat_grad) out.push_back(mat_grad->root());
-    if (vec_grad) out.push_back(vec_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&mat_grad, &vec_grad}); }
   void backward() override {
     const void* g = gradient->get();
     const int64_t rows = mat->shape[0], cols = mat->shape[1];
     auto do_mat = [&] {
       if (!mat_grad) return;
-      float beta;
-      void* d = mat_grad->acc(&beta);
       // mv: dA += g (x) v ; vm: dA += v (x) g
-      ck(ctx, nk_outer_acc(ctx, d, mat_grad->dtype, vm ? vec->rptr() : g, vm ? g : vec->rptr(), rows, cols,
-                           gradient->dtype, beta));
+      accumulate(ctx, mat_grad, [&](void* d, float beta) {
+        ck(ctx, nk_outer_acc(ctx, d, mat_grad->dtype, vm ? vec->rptr() : g, vm ? g : vec->rptr(), rows, cols,
+                             gradient->dtype, beta));
+      });
       grad_written(mat_grad);
     };
     auto do_vec = [&] {
       if (!vec_grad) return;
-      float beta;
-      void* d = vec_grad->acc(&beta);
       // mv: dv += A^T.g ; vm: dv += A.g
-      ck(ctx, nk_gemv(ctx, vm ? 0 : 1, rows, cols, mat->rptr(), g, beta, d, mat->dtype, vec_grad->dtype));
+      accumulate(ctx, vec_grad, [&](void* d, float beta) {
+        ck(ctx, nk_gemv(ctx, vm ? 0 : 1, rows, cols, mat->rptr(), g, beta, d, mat->dtype, vec_grad->dtype));
+      });
       grad_written(vec_grad);
     };
     if (vm) {  // left operand first
@@ -896,29 +950,29 @@ struct MatVecBackward : Backward {
   }
 };
 struct VecVec : Forward {
-  nk_ctx* ctx;
   TensorP left, right, data;
+  VecVec(nk_ctx* c, TensorP l, TensorP r, TensorP d)
+      : Forward(c), left(std::move(l)), right(std::move(r)), data(std::move(d)) {}
   const char* name() const override { return "VectorVectorMul"; }
   void forward() override {
     ck(ctx, nk_dot(ctx, (float*)data->wptr(), left->rptr(), right->rptr(), size_t(left->n()), left->dtype));
   }
 };
 struct VecVecBackward : Backward {
-  nk_ctx* ctx;
   TensorP left, right;
   GradientP left_grad, right_grad;
+  VecVecBackward(nk_ctx* c, GradientP g, TensorP l, TensorP r, GradientP lg, GradientP rg)
+      : Backward(c, std::move(g)), left(std::move(l)), right(std::move(r)), left_grad(std::move(lg)),
+        right_grad(std::move(rg)) {}
   const char* name() const override { return "VectorVectorMulBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (left_grad) out.push_back(left_grad->root());
-    if (right_grad) out.push_back(right_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&left_grad, &right_grad}); }
   void backward() override {
     const float* g = (const float*)gradient->get();
     auto one = [&](const GradientP& dst, const TensorP& other) {
       if (!dst) return;
-      float beta;
-      void* d = dst->acc(&beta);
-      ck(ctx, nk_scale_acc(ctx, d, dst->dtype, other->rptr(), other->dtype, g, size_t(other->n()), beta));
+      accumulate(ctx, dst, [&](void* d, float beta) {
+        ck(ctx, nk_scale_acc(ctx, d, dst->dtype, other->rptr(), other->dtype, g, size_t(other->n()), beta));
+      });
       grad_written(dst);
     };
     one(left_grad, right);
@@ -933,9 +987,10 @@ struct ConvNdArgs {
   int64_t in[3], k[3], s[3], d[3];
 };
 struct ConvolutionNd : Forward {  // convolution/mod.rs:296-355 for Ix3 / Ix5 operands
-  nk_ctx* ctx;
   TensorP input, kernel, data;
   ConvNdArgs a;
+  ConvolutionNd(nk_ctx* c, TensorP x, TensorP k, TensorP d, const ConvNdArgs& args)
+      : Forward(c), input(std::move(x)), kernel(std::move(k)), data(std::move(d)), a(args) {}
   const char* name() const override { return "Convolution"; }
   void forward() override {
     ck(ctx, nk_convnd_fwd(ctx, data->wptr(), input->rptr(), kernel->rptr(), a.nsp, a.n, a.cin, a.in, a.cout, a.k, a.s,
@@ -943,29 +998,28 @@ struct ConvolutionNd : Forward {  // convolution/mod.rs:296-355 for Ix3 / Ix5 op
   }
 };
 struct ConvolutionNdBackward : Backward {  // convolution/mod.rs:357-510
-  nk_ctx* ctx;
   TensorP input, kernel;
   GradientP input_grad, kernel_grad;
   ConvNdArgs a;
+  ConvolutionNdBackward(nk_ctx* c, GradientP g, TensorP x, TensorP k, GradientP xg, GradientP kg, const ConvNdArgs& args)
+      : Backward(c, std::move(g)), input(std::move(x)), kernel(std::move(k)), input_grad(std::move(xg)),
+        kernel_grad(std::move(kg)), a(args) {}
   const char* name() const override { return "ConvolutionBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (input_grad) out.push_back(input_grad->root());
-    if (kernel_grad) out.push_back(kernel_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad, &kernel_grad}); }
   void backward() override {
     const void* g = gradient->get();
     if (input_grad) {
-      acc_typed(ctx, input_grad, gradient->dtype, [&](void* d, float beta) {
+      accumulate(ctx, input_grad, gradient->dtype, [&](void* d, float beta) {
         ck(ctx, nk_convnd_bwd_input(ctx, d, g, kernel->rptr(), a.nsp, a.n, a.cin, a.in, a.cout, a.k, a.s, a.d, a.groups,
                                     gradient->dtype, beta));
       });
       grad_written(input_grad);
     }
     if (kernel_grad) {
-      float beta;
-      void* d = kernel_grad->acc(&beta);
-      ck(ctx, nk_convnd_bwd_kernel(ctx, d, kernel_grad->dtype, g, input->rptr(), a.nsp, a.n, a.cin, a.in, a.cout, a.k,
-                                   a.s, a.d, a.groups, gradient->dtype, beta));
+      accumulate(ctx, kernel_grad, [&](void* d, float beta) {
+        ck(ctx, nk_convnd_bwd_kernel(ctx, d, kernel_grad->dtype, g, input->rptr(), a.nsp, a.n, a.cin, a.in, a.cout, a.k,
+                                     a.s, a.d, a.groups, gradient->dtype, beta));
+      });
       grad_written(kernel_grad);
     }
   }
@@ -973,9 +1027,9 @@ struct ConvolutionNdBackward : Backward {  // convolution/mod.rs:357-510
 
 // ------------------------------------------------------------------------------- chunks (chunk/mod.rs)
 struct Chunk : Forward {
-  nk_ctx* ctx;
   TensorP operand, data;
   int64_t index;
+  Chunk(nk_ctx* c, TensorP x, TensorP d, int64_t i) : Forward(c), operand(std::move(x)), data(std::move(d)), index(i) {}
   const char* name() const override { return "Chunk"; }
   void forward() override {
     ck(ctx, nk_chunk_fwd(ctx, data->wptr(), operand->rptr(), (int)operand->shape.size(), operand->shape.data(),
@@ -983,13 +1037,12 @@ struct Chunk : Forward {
   }
 };
 struct ChunkBackward : Backward {
-  nk_ctx* ctx;
   GradientP operand_grad;
   int64_t index;
+  ChunkBackward(nk_ctx* c, GradientP g, GradientP xg, int64_t i)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), index(i) {}
   const char* name() const override { return "ChunkBackward"; }
-  void targets(std::vector<Gradient*>& out) override {
-    if (operand_grad) out.push_back(operand_grad->root());
-  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
   void backward() override {
     // a write into one block: Gradient::acc() would let the first writer overwrite the whole buffer, so the block is
     // added onto materialised zeros (get()) instead
@@ -1006,12 +1059,13 @@ struct ChunkBackward : Backward {
 // MultiConcatenate / MultiStack (multi_concatenate/mod.rs, multi_stack/mod.rs) as ONE node whatever the operand count:
 // operand i is an (outer, lens[i], inner) block of the output (a stacked operand has length 1 along the new axis).
 struct Concatenate : Forward {
-  nk_ctx* ctx;
   std::vector<TensorP> operands;
   TensorP data;
   std::vector<int64_t> lens;
   int64_t outer, inner;
   bool stack;
+  Concatenate(nk_ctx* c, std::vector<TensorP> xs, TensorP d, const std::vector<int64_t>& l, int64_t o, int64_t i, bool s)
+      : Forward(c), operands(std::move(xs)), data(std::move(d)), lens(l), outer(o), inner(i), stack(s) {}
   const char* name() const override { return stack ? "MultiStack" : "MultiConcatenate"; }
   void forward() override {
     if (data->n() == 0) return;
@@ -1021,11 +1075,13 @@ struct Concatenate : Forward {
   }
 };
 struct ConcatenateBackward : Backward {
-  nk_ctx* ctx;
   std::vector<GradientP> operand_grads;   // null for an operand that is not differentiable
   std::vector<int64_t> lens;
   int64_t outer, inner;
   bool stack;
+  ConcatenateBackward(nk_ctx* c, GradientP g, std::vector<GradientP> xg, const std::vector<int64_t>& l, int64_t o,
+                      int64_t i, bool s)
+      : Backward(c, std::move(g)), operand_grads(std::move(xg)), lens(l), outer(o), inner(i), stack(s) {}
   const char* name() const override { return stack ? "MultiStackBackward" : "MultiConcatenateBackward"; }
   void targets(std::vector<Gradient*>& out) override {
     for (const GradientP& g : operand_grads)
@@ -1042,20 +1098,22 @@ struct ConcatenateBackward : Backward {
     for (size_t i = 0; i < n; ++i)
       if (operand_grads[i] && operand_grads[i]->n() > 0)
         passes = std::max(passes, (pass[i] = seen[operand_grads[i]->root()]++) + 1);
-    if (passes == 0) return;
-    const void* g = gradient->get();
-    for (int p = 0; p < passes; ++p) {
-      std::vector<void*> dxs(n, nullptr);
-      std::vector<int> dts(n, NK_F32);
-      std::vector<float> betas(n, 0.f);
-      for (size_t i = 0; i < n; ++i) {
-        if (pass[i] != p) continue;
-        dxs[i] = operand_grads[i]->acc(&betas[i]);
-        dts[i] = operand_grads[i]->root()->dtype;
+    if (passes > 0) {
+      const void* g = gradient->get();
+      for (int p = 0; p < passes; ++p) {
+        std::vector<void*> dxs(n, nullptr);
+        std::vector<int> dts(n, NK_F32);
+        std::vector<float> betas(n, 0.f);
+        for (size_t i = 0; i < n; ++i) {
+          if (pass[i] != p) continue;
+          dxs[i] = operand_grads[i]->acc(&betas[i]);
+          dts[i] = operand_grads[i]->root()->dtype;
+        }
+        ck(ctx, nk_cat_bwd(ctx, dxs.data(), dts.data(), betas.data(), g, gradient->dtype, lens.data(), (int)n, outer,
+                           inner));
       }
-      ck(ctx, nk_cat_bwd(ctx, dxs.data(), dts.data(), betas.data(), g, gradient->dtype, lens.data(), (int)n, outer,
-                         inner));
     }
+    for (const GradientP& g : operand_grads) grad_written(g);
   }
 };
 
@@ -1072,11 +1130,16 @@ struct CellGrads {
   GradientP x, h, c, w_ih, w_hh, b_ih, b_hh;
 };
 struct RnnCell : Forward {
-  nk_ctx* ctx;
   bool lstm;
   CellOperands o;
   TensorP gi, gh;               // f32 gate pre-activations: LSTM (N, 4H) in gi; GRU (N, 3H) in gi (input) and gh (hidden)
   TensorP h_out, c_out;
+  RnnCell(nk_ctx* c, bool l, CellOperands ops, TensorP h) : Forward(c), lstm(l), o(std::move(ops)), h_out(std::move(h)) {
+    const int64_t N = o.x->shape[0], G = o.w_ih->shape[0];
+    gi = std::make_shared<Tensor>(c, Shape{N, G}, NK_F32);
+    if (!lstm) gh = std::make_shared<Tensor>(c, Shape{N, G}, NK_F32);
+    if (lstm) c_out = std::make_shared<Tensor>(c, h_out->shape, h_out->dtype);
+  }
   const char* name() const override { return lstm ? "LSTMCell" : "GRUCell"; }
   void forward() override {
     const int64_t N = o.x->shape[0], I = o.x->shape[1], H = o.h->shape[1], G = o.w_ih->shape[0];
@@ -1103,45 +1166,41 @@ static const void* grad_or_null(const GradientP& g) {
   return g->get();
 }
 struct RnnCellBackward : Backward {  // `gradient` is the new hidden state's; c_out_grad the new cell state's (LSTM)
-  nk_ctx* ctx;
   bool lstm;
   CellOperands o;
   CellGrads d;
   TensorP gi, gh;
   GradientP c_out_grad;
+  RnnCellBackward(nk_ctx* c, GradientP g, const RnnCell& fw, CellGrads grads)
+      : Backward(c, std::move(g)), lstm(fw.lstm), o(fw.o), d(std::move(grads)), gi(fw.gi), gh(fw.gh) {
+    if (lstm) c_out_grad = std::make_shared<Gradient>(c, gradient->shape, gradient->dtype);
+  }
   const char* name() const override { return lstm ? "LSTMCellBackward" : "GRUCellBackward"; }
   void targets(std::vector<Gradient*>& out) override {
-    for (const GradientP* g : {&d.w_hh, &d.w_ih, &d.b_ih, &d.b_hh, &d.x, &d.h, &d.c})
-      if (*g) out.push_back((*g)->root());
+    add_targets(out, {&d.w_hh, &d.w_ih, &d.b_ih, &d.b_hh, &d.x, &d.h, &d.c});
   }
   // dW += dG^T.A (TN).  A weight with a data-parallel reduce-scatter plan is computed locally and reported as not pushed
   // ONCE per backward pass, by its last writer: in an unrolled sequence every time step's node accumulates into the same
   // weight gradient, and the caller exchanges the whole gradient for every report it gets.
   void weight(const GradientP& g, const void* dG, const TensorP& a, int64_t G, int64_t N, int dt) {
     if (!g) return;
-    float beta;
-    void* p = g->acc(&beta);
     const int64_t K = a->shape[1];
-    gemm(ctx, true, false, G, K, N, dG, G, a->rptr(), K, beta, p, dt, g->dtype);
+    accumulate(ctx, g, [&](void* p, float beta) { gemm(ctx, true, false, G, K, N, dG, G, a->rptr(), K, beta, p, dt, g->dtype); });
     Gradient* r = g->root();
     if (r->rs_world > 1 && r->rs_hook && r->last_writer == g_bwd_pos) r->rs_hook(r->rs_user, 0);
     grad_written(g);
   }
   void bias(const GradientP& g, const void* dG, int64_t G, int64_t N, int dt) {
     if (!g) return;
-    float beta;
-    void* p = g->acc(&beta);
     const int64_t ds[1] = {G}, gs[2] = {N, G};
-    ck(ctx, nk_unbroadcast_acc(ctx, p, g->dtype, 1, ds, dG, dt, 2, gs, beta));
+    accumulate(ctx, g, [&](void* p, float beta) { ck(ctx, nk_unbroadcast_acc(ctx, p, g->dtype, 1, ds, dG, dt, 2, gs, beta)); });
     grad_written(g);
   }
   // dA += dG.W (NN)
   void input(const GradientP& g, const void* dG, const TensorP& w, int64_t G, int64_t N, int dt) {
     if (!g) return;
-    float beta;
-    void* p = g->acc(&beta);
     const int64_t K = w->shape[1];
-    gemm(ctx, false, false, N, K, G, dG, G, w->rptr(), K, beta, p, dt, g->dtype);
+    accumulate(ctx, g, [&](void* p, float beta) { gemm(ctx, false, false, N, K, G, dG, G, w->rptr(), K, beta, p, dt, g->dtype); });
     grad_written(g);
   }
   void backward() override {
@@ -1156,7 +1215,7 @@ struct RnnCellBackward : Backward {  // `gradient` is the new hidden state's; c_
         const void* dh = grad_or_null(gradient);
         const void* dc = grad_or_null(c_out_grad);
         if (d.c)
-          acc_typed(ctx, d.c, dt, [&](void* p, float beta) {
+          accumulate(ctx, d.c, dt, [&](void* p, float beta) {
             ck(ctx, nk_lstm_cell_bwd(ctx, dI, dt, p, beta, (const float*)gi->rptr(), o.c->rptr(), dh, dc, N, H, dt));
           });
         else
@@ -1166,7 +1225,7 @@ struct RnnCellBackward : Backward {  // `gradient` is the new hidden state's; c_
         ck(ctx, nk_alloc_uninit(ctx, gbytes, &dH));
         const void* dh = gradient->get();
         if (d.h)
-          acc_typed(ctx, d.h, dt, [&](void* p, float beta) {
+          accumulate(ctx, d.h, dt, [&](void* p, float beta) {
             ck(ctx, nk_gru_cell_bwd(ctx, dI, dH, dt, p, beta, (const float*)gi->rptr(), (const float*)gh->rptr(),
                                     o.h->rptr(), dh, N, H, dt));
           });
@@ -1181,7 +1240,7 @@ struct RnnCellBackward : Backward {  // `gradient` is the new hidden state's; c_
       bias(d.b_hh, dH, G, N, dt);
       input(d.x, dI, o.w_ih, G, N, dt);
       input(d.h, dH, o.w_hh, G, N, dt);
-      if (d.c) grad_written(d.c);
+      grad_written(d.c);
     } catch (...) {
       if (dH && dH != dI) nk_free(ctx, dH);
       if (dI) nk_free(ctx, dI);
@@ -1218,31 +1277,21 @@ struct nkg_var {
 
 namespace {
 
-nkg_var* new_like(nkg_var* a) {
-  nkg_var* v = new nkg_var();
-  v->ctx = a->ctx;
-  return v;
+void not_null(std::initializer_list<const void*> ptrs, const char* who) {
+  for (const void* p : ptrs)
+    if (!p) fail(NK_ERR_INVALID_ARG, "%s: NULL", who);
 }
-
-void merge(nkg_var* dst, const nkg_var* a, const nkg_var* b = nullptr) {  // History::merge
-  dst->fwd = a->fwd;
-  dst->bwd = a->bwd;
-  if (b) {
-    dst->fwd.insert(b->fwd.begin(), b->fwd.end());
-    dst->bwd.insert(b->bwd.begin(), b->bwd.end());
-  }
-}
-
-uint64_t push(nkg_var* v, ForwardP op) {
-  uint64_t id = g_next_op_id++;
-  v->fwd[id] = std::move(op);
-  return id;
-}
-void push_bwd(nkg_var* v, uint64_t id, BackwardP op) { v->bwd[id] = std::move(op); }
 
 void require_same_dtype(nkg_var* a, nkg_var* b, const char* who) {
   if (a->data->dtype != b->data->dtype) fail(NK_ERR_INVALID_ARG, "%s: operands have different element types", who);
   if (a->ctx != b->ctx) fail(NK_ERR_INVALID_ARG, "%s: operands live on different devices", who);
+}
+
+// check_groups_args, utils.rs:427-496 (same messages): shared by the 2-d and the n-d convolution
+void check_conv_channels(const Shape& ks, const Shape& is, int64_t groups) {
+  if (is[1] % groups) fail(NK_ERR_INVALID_ARG, "In channels %lld is not divisible by groups %lld", (long long)is[1], (long long)groups);
+  if (ks[0] % groups) fail(NK_ERR_INVALID_ARG, "Out channels %lld is not divisible by groups %lld", (long long)ks[0], (long long)groups);
+  if (ks[1] * groups != is[1]) fail(NK_ERR_INVALID_ARG, "convolution: kernel in-channels %lld x groups %lld != input channels %lld", (long long)ks[1], (long long)groups, (long long)is[1]);
 }
 
 Shape cobroadcast(const Shape& l, const Shape& r) {  // utils.rs:97-125
@@ -1262,94 +1311,91 @@ Shape cobroadcast(const Shape& l, const Shape& r) {  // utils.rs:97-125
   return out;
 }
 
+// Records one op: the result's history is the union of the operands' (History::merge) plus one node; its data is a
+// new (shape, dtype) tensor written by the Forward node make_fwd(data); if any operand is differentiable, the result
+// gets a gradient of the same shape and type and the Backward node make_bwd(data, gradient) under the same op id.
+template <typename MakeFwd, typename MakeBwd>
+nkg_var* record(const std::vector<nkg_var*>& operands, const Shape& shape, int dtype, MakeFwd&& make_fwd,
+                MakeBwd&& make_bwd) {
+  nkg_var* v = new nkg_var();
+  v->ctx = operands.front()->ctx;
+  bool diff = false;
+  for (nkg_var* a : operands) {
+    v->fwd.insert(a->fwd.begin(), a->fwd.end());
+    v->bwd.insert(a->bwd.begin(), a->bwd.end());
+    diff = diff || a->diff();
+  }
+  v->data = std::make_shared<Tensor>(v->ctx, shape, dtype);
+  const uint64_t id = g_next_op_id++;  // creation order == a topological order (history.rs:84-88)
+  v->fwd[id] = make_fwd(v->data);
+  if (diff) {
+    v->grad = std::make_shared<Gradient>(v->ctx, shape, dtype);
+    v->bwd[id] = make_bwd(v->data, v->grad);
+  }
+  return v;
+}
+
 // ---- peephole fusion, run when the tapes are materialised by forward()
 void fuse(nkg_var* v) {
   if (!g_fusion) return;
-  // producer lookup: output tensor -> MatMul op
-  std::map<Tensor*, std::shared_ptr<MatMul>> producers;
-  for (auto& kv : v->fwd)
-    if (auto mm = std::dynamic_pointer_cast<MatMul>(kv.second)) producers[mm->data.get()] = mm;
+  // lookups over the tapes, built once: output tensor -> its producer (matmul or convolution), operand tensor -> the
+  // LAST ReLU backward reading it, output gradient -> its addition backward, left operand gradient -> the FIRST matmul
+  // backward accumulating into it
+  std::map<Tensor*, std::shared_ptr<MatMul>> gemms;
+  std::map<Tensor*, std::shared_ptr<Convolution>> convs;
   for (auto& kv : v->fwd) {
-    auto add = std::dynamic_pointer_cast<Addition>(kv.second);
-    if (!add || add->fused_gemm) continue;
-    auto it = producers.find(add->left.get());
-    if (it == producers.end()) continue;
-    auto mm = it->second;
-    // bias must be a (N) row broadcast of the (M,N) product, same element type; the product must have no
-    // other holder than its producer and this consumer (no live variable handle, no second consumer)
-    const Shape& os = add->data->shape;
-    if (!mm->t || os.size() != 2 || add->right->shape.size() != 1 || add->right->shape[0] != os[1]) continue;
-    if (add->right->dtype != add->data->dtype || add->left->shape != os) continue;
-    if (add->left.use_count() != 2) continue;
-    add->fused_gemm = mm;
-    mm->skip = true;
+    if (auto mm = std::dynamic_pointer_cast<MatMul>(kv.second)) gemms[mm->data.get()] = mm;
+    if (auto cv = std::dynamic_pointer_cast<Convolution>(kv.second)) convs[cv->data.get()] = cv;
   }
-  // ... followed by ReLU: relu(mm_t + bias) in the same epilogue.  The pre-activation z is then never stored, so the
-  // ReLU backward node masks with y > 0 instead of z > 0 (identical: y = max(z, 0)).
-  {
-    std::map<Tensor*, std::shared_ptr<Addition>> fused_adds;
-    for (auto& kv : v->fwd)
-      if (auto add = std::dynamic_pointer_cast<Addition>(kv.second))
-        if (add->fused_gemm && !add->fused_relu_out) fused_adds[add->data.get()] = add;
-    for (auto& kv : v->fwd) {
-      auto relu = std::dynamic_pointer_cast<ReLU>(kv.second);
-      if (!relu || relu->skip) continue;
-      auto it = fused_adds.find(relu->operand.get());
-      if (it == fused_adds.end()) continue;
-      auto add = it->second;
-      std::shared_ptr<ReLUBackward> rb;
-      for (auto& kb : v->bwd)
-        if (auto c = std::dynamic_pointer_cast<ReLUBackward>(kb.second))
-          if (c->operand_data.get() == add->data.get()) rb = c;
-      // holders of z: the Addition, the ReLU, (the ReLU backward) -- anything else (a live handle, another consumer)
-      // needs z in memory
-      if (add->data.use_count() != (rb ? 3 : 2)) continue;
-      if (relu->data->dtype != add->data->dtype) continue;
-      add->fused_relu_out = relu->data;
-      relu->skip = true;
-      if (rb) rb->operand_data = relu->data;
-    }
+  std::map<Tensor*, std::shared_ptr<ReLUBackward>> relu_bwds;
+  std::map<Gradient*, std::shared_ptr<AdditionBackward>> add_bwds;
+  std::map<Gradient*, std::shared_ptr<MatMulBackward>> mm_bwds;
+  for (auto& kv : v->bwd) {
+    if (auto rb = std::dynamic_pointer_cast<ReLUBackward>(kv.second)) relu_bwds[rb->operand_data.get()] = rb;
+    if (auto ab = std::dynamic_pointer_cast<AdditionBackward>(kv.second)) add_bwds[ab->gradient.get()] = ab;
+    if (auto mb = std::dynamic_pointer_cast<MatMulBackward>(kv.second)) mm_bwds.emplace(mb->left_grad.get(), mb);
   }
-  // convolution + (Cout,1,1) bias add -> one kernel with a bias epilogue (the Conv2d layer's intended forward)
-  std::map<Tensor*, std::shared_ptr<Convolution>> conv_producers;
-  for (auto& kv : v->fwd)
-    if (auto cv = std::dynamic_pointer_cast<Convolution>(kv.second)) conv_producers[cv->data.get()] = cv;
+
+  // producer + bias add -> one kernel with a bias epilogue: mm_t + (N) row bias (the Linear layer) or convolution +
+  // (Cout,1,1) bias (the Conv2d layer).  The bias has the sum's element type; the product has no other holder than its
+  // producer and this consumer (no live variable handle, no second consumer).
+  std::map<Tensor*, std::shared_ptr<Addition>> fused_adds;  // sum -> addition, for the ReLU pass below
   for (auto& kv : v->fwd) {
     auto add = std::dynamic_pointer_cast<Addition>(kv.second);
     if (!add || add->fused_gemm || add->fused_conv) continue;
-    auto it = conv_producers.find(add->left.get());
-    if (it == conv_producers.end()) continue;
     const Shape& os = add->data->shape;
     const Shape& bs = add->right->shape;
-    if (os.size() != 4 || bs.size() != 3 || bs[0] != os[1] || bs[1] != 1 || bs[2] != 1) continue;
-    if (add->right->dtype != add->data->dtype || add->left->shape != os) continue;
-    if (add->left.use_count() != 2) continue;
-    add->fused_conv = it->second;
-    it->second->skip = true;
-  }
-  // ... followed by ReLU: relu(conv + bias) in the convolution's epilogue, exactly as for the Linear layer above (the
-  // ReLU backward masks with y > 0, identical to z > 0)
-  {
-    std::map<Tensor*, std::shared_ptr<Addition>> fused_adds;
-    for (auto& kv : v->fwd)
-      if (auto add = std::dynamic_pointer_cast<Addition>(kv.second))
-        if (add->fused_conv && !add->fused_relu_out) fused_adds[add->data.get()] = add;
-    for (auto& kv : v->fwd) {
-      auto relu = std::dynamic_pointer_cast<ReLU>(kv.second);
-      if (!relu || relu->skip || fused_adds.empty()) continue;
-      auto it = fused_adds.find(relu->operand.get());
-      if (it == fused_adds.end()) continue;
-      auto add = it->second;
-      std::shared_ptr<ReLUBackward> rb;
-      for (auto& kb : v->bwd)
-        if (auto c = std::dynamic_pointer_cast<ReLUBackward>(kb.second))
-          if (c->operand_data.get() == add->data.get()) rb = c;
-      if (add->data.use_count() != (rb ? 3 : 2)) continue;
-      if (relu->data->dtype != add->data->dtype) continue;
-      add->fused_relu_out = relu->data;
-      relu->skip = true;
-      if (rb) rb->operand_data = relu->data;
+    if (add->right->dtype != add->data->dtype || add->left->shape != os || add->left.use_count() != 2) continue;
+    auto mm = gemms.find(add->left.get());
+    auto cv = convs.find(add->left.get());
+    if (mm != gemms.end() && mm->second->t && os.size() == 2 && bs.size() == 1 && bs[0] == os[1]) {
+      add->fused_gemm = mm->second;
+      mm->second->skip = true;
+    } else if (cv != convs.end() && os.size() == 4 && bs.size() == 3 && bs[0] == os[1] && bs[1] == 1 && bs[2] == 1) {
+      add->fused_conv = cv->second;
+      cv->second->skip = true;
     }
+  }
+  for (auto& kv : v->fwd)
+    if (auto add = std::dynamic_pointer_cast<Addition>(kv.second))
+      if ((add->fused_gemm || add->fused_conv) && !add->fused_relu_out) fused_adds[add->data.get()] = add;
+  // ... followed by ReLU: relu(producer + bias) in the same epilogue.  The pre-activation z is then never stored, so the
+  // ReLU backward node masks with y > 0 instead of z > 0 (identical: y = max(z, 0)).
+  for (auto& kv : v->fwd) {
+    auto relu = std::dynamic_pointer_cast<ReLU>(kv.second);
+    if (!relu || relu->skip) continue;
+    auto it = fused_adds.find(relu->operand.get());
+    if (it == fused_adds.end()) continue;
+    auto add = it->second;
+    auto rbi = relu_bwds.find(add->data.get());
+    ReLUBackward* rb = rbi == relu_bwds.end() ? nullptr : rbi->second.get();
+    // holders of z: the Addition, the ReLU, (the ReLU backward) -- anything else (a live handle, another consumer)
+    // needs z in memory
+    if (add->data.use_count() != (rb ? 3 : 2)) continue;
+    if (relu->data->dtype != add->data->dtype) continue;
+    add->fused_relu_out = relu->data;
+    relu->skip = true;
+    if (rb) rb->operand_data = relu->data;
   }
   // level 2: ReLU backward into the epilogue of the matmul that produces its output gradient
   if (g_fusion >= 2) {
@@ -1359,50 +1405,43 @@ void fuse(nkg_var* v) {
       Gradient* gh = rb->gradient.get();
       if (gh->alias || gh->ptr || gh->is_leaf || gh->hook || rb->gradient.use_count() != 2) continue;
       if (rb->operand_grad->dtype != gh->dtype || rb->operand_data->dtype != gh->dtype) continue;
-      for (auto& kv2 : v->bwd) {
-        auto mb = std::dynamic_pointer_cast<MatMulBackward>(kv2.second);
-        if (!mb || mb->left_dst || mb->left_grad.get() != gh) continue;
-        mb->left_mask = rb->operand_data;
-        mb->left_dst = rb->operand_grad;
-        mb->single_pass = true;
-        rb->skip = true;
-        // the Addition below the ReLU (z = x.W^T + b): its (K) row-bias gradient is the column sum of the dZ this GEMM
-        // writes -- take it in the same epilogue when it is an f32 gradient nobody else aliases.  LEVEL 3 ONLY: correct
-        // (the GPU suite runs it) and four launches fewer per config-4 step, but no faster: 0.791 vs 0.793 ms -- the
-        // butterfly and the 1.3 M f32 atomics cost what the two column-sum passes did (a first version with scalar mask
-        // loads was 0.2 ms SLOWER: its epilogue outlasted the main loop).  One atomic per column and CTA would be next.
-        for (auto& kv3 : v->bwd) {
-          if (g_fusion < 3) break;
-          auto ab = std::dynamic_pointer_cast<AdditionBackward>(kv3.second);
-          if (!ab || ab->skip || ab->right_fused || ab->right_aliased || !ab->right_grad) continue;
-          if (ab->gradient.get() != rb->operand_grad.get()) continue;
-          Gradient* bg = ab->right_grad.get();
-          const Shape& gs = rb->operand_grad->shape;
-          if (bg->alias || bg->dtype != NK_F32 || gs.size() != 2 || bg->shape.size() != 1 || bg->shape[0] != gs[1]) continue;
-          mb->left_colsum = ab->right_grad;
-          ab->right_fused = true;
-          break;
-        }
-        break;
-      }
+      auto mbi = mm_bwds.find(gh);
+      if (mbi == mm_bwds.end() || mbi->second->left_dst) continue;
+      MatMulBackward* mb = mbi->second.get();
+      mb->left_mask = rb->operand_data;
+      mb->left_dst = rb->operand_grad;
+      mb->single_pass = true;
+      rb->skip = true;
+      // the Addition below the ReLU (z = x.W^T + b): its (K) row-bias gradient is the column sum of the dZ this GEMM
+      // writes -- take it in the same epilogue when it is an f32 gradient nobody else aliases.  LEVEL 3 ONLY: correct
+      // (the GPU suite runs it) and four launches fewer per config-4 step, but no faster: 0.791 vs 0.793 ms -- the
+      // butterfly and the 1.3 M f32 atomics cost what the two column-sum passes did (a first version with scalar mask
+      // loads was 0.2 ms SLOWER: its epilogue outlasted the main loop).  One atomic per column and CTA would be next.
+      auto abi = add_bwds.find(rb->operand_grad.get());
+      if (g_fusion < 3 || abi == add_bwds.end()) continue;
+      AdditionBackward* ab = abi->second.get();
+      if (ab->skip || ab->right_fused || ab->right_aliased || !ab->right_grad) continue;
+      Gradient* bg = ab->right_grad.get();
+      const Shape& gs = rb->operand_grad->shape;
+      if (bg->alias || bg->dtype != NK_F32 || gs.size() != 2 || bg->shape.size() != 1 || bg->shape[0] != gs[1]) continue;
+      mb->left_colsum = ab->right_grad;
+      ab->right_fused = true;
     }
   }
   // gradient aliasing: dL += G with identical shape/dtype and a single consumer => L.grad is G
   for (auto& kv : v->bwd) {
     auto ab = std::dynamic_pointer_cast<AdditionBackward>(kv.second);
     if (!ab) continue;
-    auto try_alias = [&](GradientP& g, bool& flag) {
-      if (!g || flag || g->alias || g->ptr) return;
-      if (g->shape != ab->gradient->shape || g->dtype != ab->gradient->dtype) return;
-      if (!g->owned) return;
-      // only a gradient produced by a Backward node may be aliased: a leaf's gradient belongs to the user (hooks and
-      // reduce-scatter plans sit on it, it accumulates over backward() calls and outlives this graph)
-      if (g->is_leaf || g->hook || g->rs_world > 1) return;
-      if (g.use_count() != 2) return;  // the producer's Backward node + this node
-      g->alias = ab->gradient;
-      flag = true;
-    };
-    try_alias(ab->left_grad, ab->left_aliased);
+    GradientP& g = ab->left_grad;
+    if (!g || ab->left_aliased || g->alias || g->ptr) continue;
+    if (g->shape != ab->gradient->shape || g->dtype != ab->gradient->dtype) continue;
+    if (!g->owned) continue;
+    // only a gradient produced by a Backward node may be aliased: a leaf's gradient belongs to the user (hooks and
+    // reduce-scatter plans sit on it, it accumulates over backward() calls and outlives this graph)
+    if (g->is_leaf || g->hook || g->rs_world > 1) continue;
+    if (g.use_count() != 2) continue;  // the producer's Backward node + this node
+    g->alias = ab->gradient;
+    ab->left_aliased = true;
   }
   // bias gradient of a fused Conv2d: let the dW kernel produce it (its all-ones K-row) instead of re-reading G
   for (auto& kv : v->bwd) {
@@ -1415,6 +1454,7 @@ void fuse(nkg_var* v) {
       auto cb = std::dynamic_pointer_cast<ConvolutionBackward>(kv2.second);
       if (!cb || cb->bias_grad || cb->gradient->root() != ab->gradient->root()) continue;
       cb->bias_grad = ab->right_grad;
+      ab->bias_producer = cb.get();
       ab->right_aliased = true;
       break;
     }
@@ -1445,14 +1485,6 @@ int guard(F&& f) {
     g_error = e.what();
     return NK_ERR_INVALID_ARG;
   }
-}
-
-nkg_var* unary_node(nkg_var* a, const Shape& out_shape, int out_dtype, TensorP& out_data) {
-  nkg_var* v = new_like(a);
-  merge(v, a);
-  out_data = std::make_shared<Tensor>(a->ctx, out_shape, out_dtype);
-  v->data = out_data;
-  return v;
 }
 
 // a view: the operand's memory and tapes under another shape (no kernel, no node); the gradient of a view is the same
@@ -1491,7 +1523,7 @@ int nkg_leaf(nk_ctx* ctx, int ndim, const int64_t* shape, int dtype, nkg_var** o
     nkg_var* v = new nkg_var();
     v->ctx = ctx;
     v->data = std::make_shared<Tensor>(ctx, Shape(shape, shape + ndim), dtype);
-    v->data->wptr();  // leaves are allocated (zero-filled) eagerly
+    v->data->rptr();  // leaves are allocated (zero-filled) eagerly
     *out = v;
   });
 }
@@ -1511,7 +1543,7 @@ int nkg_leaf_external(nk_ctx* ctx, int ndim, const int64_t* shape, int dtype, vo
 
 int nkg_requires_grad(nkg_var* a, int grad_dtype, void* grad_ptr, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "nkg_requires_grad: NULL");
+    not_null({a, out}, "nkg_requires_grad");
     nkg_var* v = new nkg_var(*a);  // shares data and forward tape (VarDiff::leaf(self, zeros))
     v->grad = std::make_shared<Gradient>(a->ctx, a->data->shape, grad_dtype < 0 ? a->data->dtype : grad_dtype);
     v->grad->is_leaf = true;
@@ -1528,7 +1560,7 @@ int nkg_requires_grad(nkg_var* a, int grad_dtype, void* grad_ptr, nkg_var** out)
 
 int nkg_clone(nkg_var* a, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "nkg_clone: NULL");
+    not_null({a, out}, "nkg_clone");
     *out = new nkg_var(*a);
   });
 }
@@ -1564,7 +1596,7 @@ int nkg_backward_history_len(nkg_var* v) { return v ? (int)v->bwd.size() : -1; }
 
 int nkg_forward(nkg_var* v) {
   return guard([&] {
-    if (!v) fail(NK_ERR_INVALID_ARG, "nkg_forward: NULL");
+    not_null({v}, "nkg_forward");
     materialise(v);
     for (auto& op : v->fwd_buf)
       if (!op->skip) op->forward();
@@ -1576,38 +1608,15 @@ int nkg_backward(nkg_var* v, float seed) {
     if (!v || !v->diff()) fail(NK_ERR_INVALID_ARG, "nkg_backward: not a differentiable variable");
     if (v->fwd_buf.size() != v->fwd.size() || v->bwd_buf.size() != v->bwd.size())
       fail(NK_ERR_INVALID_ARG, "Perhaps you forgot to call .forward()?");  // vardiff.rs:126-130
-    // The aliasing peephole (dL += G with one consumer => L.grad IS G) is exact for ONE backward pass per tape.  The
-    // reference accumulates into every gradient, intermediates included, on every pass (nothing zeroes them), so on a
-    // repeated backward() the addend's gradient and the sum's gradient diverge: give the addend its own buffer, holding
-    // what the reference would hold after the passes so far (= the sum's gradient at the end of the last pass).
     for (auto& op : v->bwd_buf)
       if (op->single_pass && op->runs > 0)
         fail(NK_ERR_UNSUPPORTED, "this tape was optimised for ONE backward pass (fusion level 2: %s never stores the "
              "gradient it would have to accumulate); build the graph again or use nkg_set_fusion(1)", op->name());
-    for (auto& op : v->bwd_buf) {
-      auto ab = std::dynamic_pointer_cast<AdditionBackward>(op);
-      if (!ab || !ab->left_aliased || ab->runs == 0 || !ab->left_grad || !ab->left_grad->alias) continue;
-      Gradient* g = ab->left_grad.get();
-      Gradient* src = g->root();
-      const size_t bytes = size_t(g->n()) * esize(g->dtype);
-      void* own = nullptr;
-      ck(g->ctx, nk_alloc_uninit(g->ctx, bytes, &own));
-      ck(g->ctx, nk_d2d(g->ctx, own, src->get(), bytes));
-      g->alias.reset();
-      g->ptr = own;
-      g->owned = true;
-      g->is_zero = false;
-      g->stale = false;
-      ab->left_aliased = false;
-      if (ab->right_aliased) {  // the bias gradient rode along with the convolution's dW: back to its own un-broadcast
-        for (auto& op2 : v->bwd_buf)
-          if (auto cb = std::dynamic_pointer_cast<ConvolutionBackward>(op2))
-            if (cb->bias_grad == ab->right_grad) cb->bias_grad.reset();
-        ab->right_aliased = false;
-      }
-    }
+    for (auto& op : v->bwd_buf)
+      if (op->runs > 0) op->unalias();
     v->grad->fill(seed);
-    // last writer (reverse tape position) of every hooked gradient in this pass
+    // last writer (reverse tape position) of every hooked gradient in this pass; every node reports its writes
+    // (grad_written), and the hook fires on the report of the last writer
     std::vector<Gradient*> tg;
     bool any_hook = false;
     int pos = 0;
@@ -1631,20 +1640,10 @@ int nkg_backward(nkg_var* v, float seed) {
     }
     pos = 0;
     for (auto it = v->bwd_buf.rbegin(); it != v->bwd_buf.rend(); ++it, ++pos) {
+      if ((*it)->skip) continue;
       g_bwd_pos = any_hook ? pos : -2;
-      if (!(*it)->skip) {
-        (*it)->backward();
-        (*it)->runs++;
-      }
-      if (any_hook) {  // nodes that do not report their writes individually: fire at node granularity
-        tg.clear();
-        (*it)->targets(tg);
-        for (Gradient* g : tg)
-          if (g->hook && g->last_writer == pos && !g->hook_fired) {
-            g->hook_fired = true;
-            g->hook(g->hook_user, 0, g->n());
-          }
-      }
+      (*it)->backward();
+      (*it)->runs++;
     }
     g_bwd_pos = -1;
   });
@@ -1676,7 +1675,7 @@ int nkg_with_grad(nkg_var* v) {
 // ---------------------------------------------------------------- operators
 static int matmul_impl(nkg_var* a, nkg_var* b, bool t, nkg_var** out) {
   return guard([&] {
-    if (!a || !b || !out) fail(NK_ERR_INVALID_ARG, "mm: NULL");
+    not_null({a, b, out}, "mm");
     require_same_dtype(a, b, t ? "mm_t" : "mm");
     const Shape &ls = a->data->shape, &rs = b->data->shape;
     if (ls.size() != 2 || rs.size() != 2) fail(NK_ERR_INVALID_ARG, "mm: operands must be 2-dimensional");
@@ -1684,24 +1683,13 @@ static int matmul_impl(nkg_var* a, nkg_var* b, bool t, nkg_var** out) {
     if (ls[1] != inner_r)
       fail(NK_ERR_INVALID_ARG, "mm: incompatible shapes (%lld, %lld) and (%lld, %lld)%s", (long long)ls[0],
            (long long)ls[1], (long long)rs[0], (long long)rs[1], t ? " (transposed rhs)" : "");
-    nkg_var* v = new_like(a);
-    merge(v, a, b);
-    Shape os{ls[0], t ? rs[0] : rs[1]};
-    v->data = std::make_shared<Tensor>(a->ctx, os, a->data->dtype);
-    uint64_t id = push(v, std::make_shared<MatMul>(a->ctx, a->data, b->data, v->data, t));
-    if (a->diff() || b->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, os, a->data->dtype);
-      auto bw = std::make_shared<MatMulBackward>();
-      bw->ctx = a->ctx;
-      bw->t = t;
-      bw->gradient = v->grad;
-      bw->left_data = a->data;
-      bw->right_data = b->data;
-      bw->left_grad = a->grad;   // null when the operand is a Var: that half is never built
-      bw->right_grad = b->grad;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a, b}, Shape{ls[0], t ? rs[0] : rs[1]}, a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<MatMul>(a->ctx, a->data, b->data, d, t); },
+        // a null operand gradient (a Var) is a half that is never built
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<MatMulBackward>(a->ctx, g, a->data, b->data, a->grad, b->grad, t);
+        });
   });
 }
 
@@ -1710,79 +1698,36 @@ int nkg_mm_t(nkg_var* a, nkg_var* b, nkg_var** out) { return matmul_impl(a, b, t
 
 int nkg_add(nkg_var* a, nkg_var* b, nkg_var** out) {
   return guard([&] {
-    if (!a || !b || !out) fail(NK_ERR_INVALID_ARG, "add: NULL");
+    not_null({a, b, out}, "add");
     require_same_dtype(a, b, "add");
-    Shape os = cobroadcast(a->data->shape, b->data->shape);
-    nkg_var* v = new_like(a);
-    merge(v, a, b);
-    v->data = std::make_shared<Tensor>(a->ctx, os, a->data->dtype);
-    auto op = std::make_shared<Addition>();
-    op->ctx = a->ctx;
-    op->left = a->data;
-    op->right = b->data;
-    op->data = v->data;
-    uint64_t id = push(v, op);
-    if (a->diff() || b->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, os, a->data->dtype);
-      auto bw = std::make_shared<AdditionBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->left_grad = a->grad;
-      bw->right_grad = b->grad;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a, b}, cobroadcast(a->data->shape, b->data->shape), a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Addition>(a->ctx, a->data, b->data, d); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<AdditionBackward>(a->ctx, g, a->grad, b->grad);
+        });
   });
 }
 
 int nkg_relu(nkg_var* a, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "relu: NULL");
-    TensorP od;
-    nkg_var* v = unary_node(a, a->data->shape, a->data->dtype, od);
-    auto op = std::make_shared<ReLU>();
-    op->ctx = a->ctx;
-    op->operand = a->data;
-    op->data = od;
-    uint64_t id = push(v, op);
-    if (a->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, od->shape, od->dtype);
-      auto bw = std::make_shared<ReLUBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->operand_data = a->data;
-      bw->operand_grad = a->grad;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    not_null({a, out}, "relu");
+    *out = record(
+        {a}, a->data->shape, a->data->dtype, [&](const TensorP& d) { return std::make_shared<ReLU>(a->ctx, a->data, d); },
+        [&](const TensorP&, const GradientP& g) { return std::make_shared<ReLUBackward>(a->ctx, g, a->data, a->grad); });
   });
 }
 
 static int softmax_impl(nkg_var* a, int axis, bool log, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "softmax: NULL");
+    not_null({a, out}, "softmax");
     if (axis < 0 || axis >= (int)a->data->shape.size()) fail(NK_ERR_INVALID_ARG, "softmax: axis %d out of range", axis);
-    TensorP od;
-    nkg_var* v = unary_node(a, a->data->shape, a->data->dtype, od);
-    auto op = std::make_shared<Softmax>();
-    op->ctx = a->ctx;
-    op->operand = a->data;
-    op->data = od;
-    op->axis = axis;
-    op->log = log;
-    uint64_t id = push(v, op);
-    if (a->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, od->shape, od->dtype);
-      auto bw = std::make_shared<SoftmaxBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->data = od;
-      bw->operand_grad = a->grad;
-      bw->axis = axis;
-      bw->log = log;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a}, a->data->shape, a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Softmax>(a->ctx, a->data, d, axis, log); },
+        [&](const TensorP& d, const GradientP& g) {
+          return std::make_shared<SoftmaxBackward>(a->ctx, g, d, a->grad, axis, log);
+        });
   });
 }
 int nkg_softmax(nkg_var* a, int axis, nkg_var** out) { return softmax_impl(a, axis, false, out); }
@@ -1790,25 +1735,10 @@ int nkg_log_softmax(nkg_var* a, int axis, nkg_var** out) { return softmax_impl(a
 
 static int summean_impl(nkg_var* a, bool mean, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "sum: NULL");
-    TensorP od;
-    nkg_var* v = unary_node(a, Shape{}, NK_F32, od);
-    auto op = std::make_shared<SumMean>();
-    op->ctx = a->ctx;
-    op->operand = a->data;
-    op->data = od;
-    op->mean = mean;
-    uint64_t id = push(v, op);
-    if (a->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, Shape{}, NK_F32);
-      auto bw = std::make_shared<SumMeanBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->operand_grad = a->grad;
-      bw->mean = mean;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    not_null({a, out}, "sum");
+    *out = record(
+        {a}, Shape{}, NK_F32, [&](const TensorP& d) { return std::make_shared<SumMean>(a->ctx, a->data, d, mean); },
+        [&](const TensorP&, const GradientP& g) { return std::make_shared<SumMeanBackward>(a->ctx, g, a->grad, mean); });
   });
 }
 int nkg_sum(nkg_var* a, nkg_var** out) { return summean_impl(a, false, out); }
@@ -1816,7 +1746,7 @@ int nkg_mean(nkg_var* a, nkg_var** out) { return summean_impl(a, true, out); }
 
 static int loss_impl(nkg_var* input, nkg_var* target, int reduction, bool nll, nkg_var** out) {
   return guard([&] {
-    if (!input || !target || !out) fail(NK_ERR_INVALID_ARG, "loss: NULL");
+    not_null({input, target, out}, "loss");
     if (nll) {
       // class ids are stored as floats (nll/mod.rs:55 `target as usize`): an f32 target is accepted whatever the
       // input's element type; a bf16 target represents integers exactly only up to 256
@@ -1834,30 +1764,13 @@ static int loss_impl(nkg_var* input, nkg_var* target, int reduction, bool nll, n
       fail(NK_ERR_INVALID_ARG, "mse_loss: input and target shapes differ");
     }
     if (target->diff()) fail(NK_ERR_INVALID_ARG, "loss: the target must not be differentiable");
-    nkg_var* v = new_like(input);
-    merge(v, input, target);
-    v->data = std::make_shared<Tensor>(input->ctx, Shape{}, NK_F32);
-    auto op = std::make_shared<Loss>();
-    op->ctx = input->ctx;
-    op->input = input->data;
-    op->target = target->data;
-    op->data = v->data;
-    op->mean = reduction == NKG_MEAN;
-    op->nll = nll;
-    uint64_t id = push(v, op);
-    if (input->diff()) {
-      v->grad = std::make_shared<Gradient>(input->ctx, Shape{}, NK_F32);
-      auto bw = std::make_shared<LossBackward>();
-      bw->ctx = input->ctx;
-      bw->gradient = v->grad;
-      bw->input = input->data;
-      bw->target = target->data;
-      bw->input_grad = input->grad;
-      bw->mean = op->mean;
-      bw->nll = nll;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    const bool mean = reduction == NKG_MEAN;
+    *out = record(
+        {input, target}, Shape{}, NK_F32,
+        [&](const TensorP& d) { return std::make_shared<Loss>(input->ctx, input->data, target->data, d, mean, nll); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<LossBackward>(input->ctx, g, input->data, target->data, input->grad, mean, nll);
+        });
   });
 }
 int nkg_mse_loss(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, false, o); }
@@ -1865,37 +1778,20 @@ int nkg_nll_loss(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(
 
 int nkg_pad(nkg_var* a, int64_t ph, int64_t pw, float value, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "pad: NULL");
+    not_null({a, out}, "pad");
     const Shape& s = a->data->shape;
     if (s.size() != 4 || ph < 0 || pw < 0) fail(NK_ERR_INVALID_ARG, "pad: expects a (N, C, H, W) operand and padding >= 0");
-    TensorP od;
-    nkg_var* v = unary_node(a, Shape{s[0], s[1], s[2] + 2 * ph, s[3] + 2 * pw}, a->data->dtype, od);
-    auto op = std::make_shared<Pad>();
-    op->ctx = a->ctx;
-    op->operand = a->data;
-    op->data = od;
-    op->ph = ph;
-    op->pw = pw;
-    op->value = value;
-    uint64_t id = push(v, op);
-    if (a->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, od->shape, od->dtype);
-      auto bw = std::make_shared<PadBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->operand_grad = a->grad;
-      bw->ph = ph;
-      bw->pw = pw;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a}, Shape{s[0], s[1], s[2] + 2 * ph, s[3] + 2 * pw}, a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Pad>(a->ctx, a->data, d, ph, pw, value); },
+        [&](const TensorP&, const GradientP& g) { return std::make_shared<PadBackward>(a->ctx, g, a->grad, ph, pw); });
   });
 }
 
 int nkg_convolution(nkg_var* kernel, nkg_var* input, int64_t sh, int64_t sw, int64_t dh, int64_t dw, int64_t groups,
                     nkg_var** out) {
   return guard([&] {
-    if (!kernel || !input || !out) fail(NK_ERR_INVALID_ARG, "convolution: NULL");
+    not_null({kernel, input, out}, "convolution");
     require_same_dtype(kernel, input, "convolution");
     const Shape &ks = kernel->data->shape, &is = input->data->shape;
     // check_conv_args / check_groups_args, utils.rs:427-496 (same messages)
@@ -1904,40 +1800,23 @@ int nkg_convolution(nkg_var* kernel, nkg_var* input, int64_t sh, int64_t sw, int
     if (sh < 1 || sw < 1 || dh < 1 || dw < 1 || groups < 1) fail(NK_ERR_INVALID_ARG, "Invalid stride/dilation/groups for 2d conv.");
     if (is[2] < (ks[2] - 1) * dh + 1 || is[3] < (ks[3] - 1) * dw + 1)
       fail(NK_ERR_INVALID_ARG, "The kernel size can't be greater than actual input size.");
-    if (is[1] % groups) fail(NK_ERR_INVALID_ARG, "In channels %lld is not divisible by groups %lld", (long long)is[1], (long long)groups);
-    if (ks[0] % groups) fail(NK_ERR_INVALID_ARG, "Out channels %lld is not divisible by groups %lld", (long long)ks[0], (long long)groups);
-    if (ks[1] * groups != is[1]) fail(NK_ERR_INVALID_ARG, "convolution: kernel in-channels %lld x groups %lld != input channels %lld", (long long)ks[1], (long long)groups, (long long)is[1]);
-    ConvArgs a{is[0], is[1], is[2], is[3], ks[0], ks[2], ks[3], sh, sw, dh, dw, groups};
-    Shape os{is[0], ks[0], (is[2] - dh * (ks[2] - 1) - 1) / sh + 1, (is[3] - dw * (ks[3] - 1) - 1) / sw + 1};
-    nkg_var* v = new_like(kernel);
-    merge(v, kernel, input);
-    v->data = std::make_shared<Tensor>(kernel->ctx, os, input->data->dtype);
-    auto op = std::make_shared<Convolution>();
-    op->ctx = kernel->ctx;
-    op->input = input->data;
-    op->kernel = kernel->data;
-    op->data = v->data;
-    op->a = a;
-    uint64_t id = push(v, op);
-    if (kernel->diff() || input->diff()) {
-      v->grad = std::make_shared<Gradient>(kernel->ctx, os, input->data->dtype);
-      auto bw = std::make_shared<ConvolutionBackward>();
-      bw->ctx = kernel->ctx;
-      bw->gradient = v->grad;
-      bw->input = input->data;
-      bw->kernel = kernel->data;
-      bw->input_grad = input->grad;
-      bw->kernel_grad = kernel->grad;
-      bw->a = a;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    check_conv_channels(ks, is, groups);
+    const ConvArgs a{is[0], is[1], is[2], is[3], ks[0], ks[2], ks[3], sh, sw, dh, dw, groups};
+    *out = record(
+        {kernel, input},
+        Shape{is[0], ks[0], (is[2] - dh * (ks[2] - 1) - 1) / sh + 1, (is[3] - dw * (ks[3] - 1) - 1) / sw + 1},
+        input->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Convolution>(kernel->ctx, input->data, kernel->data, d, a); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<ConvolutionBackward>(kernel->ctx, g, input->data, kernel->data, input->grad,
+                                                       kernel->grad, a);
+        });
   });
 }
 
 int nkg_flatten(nkg_var* a, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "flatten: NULL");
+    not_null({a, out}, "flatten");
     const Shape& s = a->data->shape;
     if (s.size() < 2) fail(NK_ERR_INVALID_ARG, "flatten: needs at least 2 dimensions");
     int64_t rest = 1;
@@ -1949,32 +1828,14 @@ int nkg_flatten(nkg_var* a, nkg_var** out) {
 // ---------------------------------------------------------------- 8-f operators
 static int binary_impl(nkg_var* a, nkg_var* b, int op, nkg_var** out) {
   return guard([&] {
-    if (!a || !b || !out) fail(NK_ERR_INVALID_ARG, "binary op: NULL");
+    not_null({a, b, out}, "binary op");
     require_same_dtype(a, b, op == NK_BIN_SUB ? "sub" : op == NK_BIN_MUL ? "mul" : "div");
-    Shape os = cobroadcast(a->data->shape, b->data->shape);
-    nkg_var* v = new_like(a);
-    merge(v, a, b);
-    v->data = std::make_shared<Tensor>(a->ctx, os, a->data->dtype);
-    auto fw = std::make_shared<Binary>();
-    fw->ctx = a->ctx;
-    fw->left = a->data;
-    fw->right = b->data;
-    fw->data = v->data;
-    fw->op = op;
-    uint64_t id = push(v, fw);
-    if (a->diff() || b->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, os, a->data->dtype);
-      auto bw = std::make_shared<BinaryBackward>();
-      bw->ctx = a->ctx;
-      bw->op = op;
-      bw->gradient = v->grad;
-      bw->left_data = a->data;
-      bw->right_data = b->data;
-      bw->left_grad = a->grad;
-      bw->right_grad = b->grad;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a, b}, cobroadcast(a->data->shape, b->data->shape), a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Binary>(a->ctx, a->data, b->data, d, op); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<BinaryBackward>(a->ctx, g, a->data, b->data, a->grad, b->grad, op);
+        });
   });
 }
 int nkg_sub(nkg_var* a, nkg_var* b, nkg_var** out) { return binary_impl(a, b, NK_BIN_SUB, out); }
@@ -1983,30 +1844,16 @@ int nkg_div(nkg_var* a, nkg_var* b, nkg_var** out) { return binary_impl(a, b, NK
 
 int nkg_unary(nkg_var* a, int op, int iparam, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "unary op: NULL");
+    not_null({a, out}, "unary op");
     if (op < NK_UN_NEG || op > NK_UN_POWI) fail(NK_ERR_INVALID_ARG, "unary op: bad op %d", op);
-    TensorP od;
-    nkg_var* v = unary_node(a, a->data->shape, a->data->dtype, od);
-    auto fw = std::make_shared<Unary>();
-    fw->ctx = a->ctx;
-    fw->operand = a->data;
-    fw->data = od;
-    fw->op = op;
-    fw->iparam = iparam;
-    uint64_t id = push(v, fw);
-    if (a->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, od->shape, od->dtype);
-      auto bw = std::make_shared<UnaryBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->operand_grad = a->grad;
-      bw->op = op;
-      bw->iparam = iparam;
-      const bool keeps_output = op == NK_UN_EXP || op == NK_UN_SQRT || op == NK_UN_SIGMOID || op == NK_UN_TANH;
-      bw->saved = op == NK_UN_NEG ? nullptr : (keeps_output ? od : a->data);
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a}, a->data->shape, a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Unary>(a->ctx, a->data, d, op, iparam); },
+        [&](const TensorP& d, const GradientP& g) {
+          const bool keeps_output = op == NK_UN_EXP || op == NK_UN_SQRT || op == NK_UN_SIGMOID || op == NK_UN_TANH;
+          TensorP saved = op == NK_UN_NEG ? nullptr : (keeps_output ? d : a->data);
+          return std::make_shared<UnaryBackward>(a->ctx, g, std::move(saved), a->grad, op, iparam);
+        });
   });
 }
 int nkg_neg(nkg_var* a, nkg_var** out) { return nkg_unary(a, NK_UN_NEG, 0, out); }
@@ -2021,70 +1868,41 @@ int nkg_pow(nkg_var* a, int exp, nkg_var** out) { return nkg_unary(a, NK_UN_POWI
 
 int nkg_transpose(nkg_var* a, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "t: NULL");
-    Shape os(a->data->shape.rbegin(), a->data->shape.rend());
-    TensorP od;
-    nkg_var* v = unary_node(a, os, a->data->dtype, od);
-    auto fw = std::make_shared<Transpose>();
-    fw->ctx = a->ctx;
-    fw->operand = a->data;
-    fw->data = od;
-    uint64_t id = push(v, fw);
-    if (a->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, os, od->dtype);
-      auto bw = std::make_shared<TransposeBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->operand_grad = a->grad;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    not_null({a, out}, "t");
+    *out = record(
+        {a}, Shape(a->data->shape.rbegin(), a->data->shape.rend()), a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Transpose>(a->ctx, a->data, d); },
+        [&](const TensorP&, const GradientP& g) { return std::make_shared<TransposeBackward>(a->ctx, g, a->grad); });
   });
 }
 
 int nkg_pad_mode(nkg_var* a, int nsp, const int64_t* padding, int mode, float value, nkg_var** out) {
   return guard([&] {
-    if (!a || !out || !padding) fail(NK_ERR_INVALID_ARG, "pad: NULL");
+    not_null({a, out, padding}, "pad");
     const Shape& s = a->data->shape;
     if (nsp < 1 || nsp > 3 || (int)s.size() != nsp + 2)
       fail(NK_ERR_INVALID_ARG, "pad: expects a (N, C, ...) operand with %d sample dimensions", nsp);
     if (mode < NK_PAD_CONSTANT || mode > NK_PAD_REPLICATIVE) fail(NK_ERR_INVALID_ARG, "pad: bad mode %d", mode);
     Shape os = s;
+    int64_t pad[3] = {0, 0, 0};
     for (int k = 0; k < nsp; ++k) {
       if (padding[k] < 0) fail(NK_ERR_INVALID_ARG, "pad: padding must be >= 0");
       if (mode == NK_PAD_REFLECTIVE && padding[k] > 0 && padding[k] >= s[2 + k])
         fail(NK_ERR_INVALID_ARG, "pad: reflective padding %lld must be smaller than the dimension %lld",
              (long long)padding[k], (long long)s[2 + k]);
       os[2 + k] += 2 * padding[k];
+      pad[k] = padding[k];
     }
-    TensorP od;
-    nkg_var* v = unary_node(a, os, a->data->dtype, od);
-    auto fw = std::make_shared<PadNd>();
-    fw->ctx = a->ctx;
-    fw->operand = a->data;
-    fw->data = od;
-    fw->nsp = nsp;
-    fw->mode = mode;
-    fw->value = value;
-    for (int k = 0; k < 3; ++k) fw->pad[k] = k < nsp ? padding[k] : 0;
-    uint64_t id = push(v, fw);
-    if (a->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, os, od->dtype);
-      auto bw = std::make_shared<PadNdBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->operand_grad = a->grad;
-      bw->nsp = nsp;
-      for (int k = 0; k < 3; ++k) bw->pad[k] = fw->pad[k];
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a}, os, a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<PadNd>(a->ctx, a->data, d, nsp, pad, mode, value); },
+        [&](const TensorP&, const GradientP& g) { return std::make_shared<PadNdBackward>(a->ctx, g, a->grad, nsp, pad); });
   });
 }
 
 static int matvec_impl(nkg_var* mat, nkg_var* vec, bool vm, nkg_var** out) {
   return guard([&] {
-    if (!mat || !vec || !out) fail(NK_ERR_INVALID_ARG, "mv: NULL");
+    not_null({mat, vec, out}, "mv");
     require_same_dtype(mat, vec, vm ? "vm" : "mv");
     const Shape &ms = mat->data->shape, &vs = vec->data->shape;
     if (ms.size() != 2 || vs.size() != 1) fail(NK_ERR_INVALID_ARG, "%s: needs a matrix and a vector", vm ? "vm" : "mv");
@@ -2092,32 +1910,12 @@ static int matvec_impl(nkg_var* mat, nkg_var* vec, bool vm, nkg_var** out) {
     if (vs[0] != need)
       fail(NK_ERR_INVALID_ARG, "%s: incompatible shapes (%lld, %lld) and (%lld)", vm ? "vm" : "mv", (long long)ms[0],
            (long long)ms[1], (long long)vs[0]);
-    nkg_var* first = vm ? vec : mat;
-    nkg_var* second = vm ? mat : vec;
-    nkg_var* v = new_like(first);
-    merge(v, first, second);
-    Shape os{vm ? ms[1] : ms[0]};
-    v->data = std::make_shared<Tensor>(mat->ctx, os, mat->data->dtype);
-    auto fw = std::make_shared<MatVec>();
-    fw->ctx = mat->ctx;
-    fw->mat = mat->data;
-    fw->vec = vec->data;
-    fw->data = v->data;
-    fw->vm = vm;
-    uint64_t id = push(v, fw);
-    if (mat->diff() || vec->diff()) {
-      v->grad = std::make_shared<Gradient>(mat->ctx, os, mat->data->dtype);
-      auto bw = std::make_shared<MatVecBackward>();
-      bw->ctx = mat->ctx;
-      bw->gradient = v->grad;
-      bw->mat = mat->data;
-      bw->vec = vec->data;
-      bw->mat_grad = mat->grad;
-      bw->vec_grad = vec->grad;
-      bw->vm = vm;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {vm ? vec : mat, vm ? mat : vec}, Shape{vm ? ms[1] : ms[0]}, mat->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<MatVec>(mat->ctx, mat->data, vec->data, d, vm); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<MatVecBackward>(mat->ctx, g, mat->data, vec->data, mat->grad, vec->grad, vm);
+        });
   });
 }
 int nkg_mv(nkg_var* mat, nkg_var* vec, nkg_var** out) { return matvec_impl(mat, vec, false, out); }
@@ -2125,38 +1923,22 @@ int nkg_vm(nkg_var* vec, nkg_var* mat, nkg_var** out) { return matvec_impl(mat, 
 
 int nkg_vv(nkg_var* a, nkg_var* b, nkg_var** out) {
   return guard([&] {
-    if (!a || !b || !out) fail(NK_ERR_INVALID_ARG, "vv: NULL");
+    not_null({a, b, out}, "vv");
     require_same_dtype(a, b, "vv");
     if (a->data->shape.size() != 1 || b->data->shape.size() != 1 || a->data->shape[0] != b->data->shape[0])
       fail(NK_ERR_INVALID_ARG, "vv: needs two vectors of the same length");
-    nkg_var* v = new_like(a);
-    merge(v, a, b);
-    v->data = std::make_shared<Tensor>(a->ctx, Shape{}, NK_F32);
-    auto fw = std::make_shared<VecVec>();
-    fw->ctx = a->ctx;
-    fw->left = a->data;
-    fw->right = b->data;
-    fw->data = v->data;
-    uint64_t id = push(v, fw);
-    if (a->diff() || b->diff()) {
-      v->grad = std::make_shared<Gradient>(a->ctx, Shape{}, NK_F32);
-      auto bw = std::make_shared<VecVecBackward>();
-      bw->ctx = a->ctx;
-      bw->gradient = v->grad;
-      bw->left = a->data;
-      bw->right = b->data;
-      bw->left_grad = a->grad;
-      bw->right_grad = b->grad;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    *out = record(
+        {a, b}, Shape{}, NK_F32, [&](const TensorP& d) { return std::make_shared<VecVec>(a->ctx, a->data, b->data, d); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<VecVecBackward>(a->ctx, g, a->data, b->data, a->grad, b->grad);
+        });
   });
 }
 
 int nkg_convolution_nd(nkg_var* kernel, nkg_var* input, int nsp, const int64_t* stride, const int64_t* dilation,
                        int64_t groups, nkg_var** out) {
   return guard([&] {
-    if (!kernel || !input || !out || !stride || !dilation) fail(NK_ERR_INVALID_ARG, "convolution: NULL");
+    not_null({kernel, input, out, stride, dilation}, "convolution");
     if (nsp == 2)
       fail(NK_ERR_INVALID_ARG, "convolution: use nkg_convolution for 2d operands");
     require_same_dtype(kernel, input, "convolution");
@@ -2175,32 +1957,14 @@ int nkg_convolution_nd(nkg_var* kernel, nkg_var* input, int nsp, const int64_t* 
       a.in[k] = is[2 + k], a.k[k] = ks[2 + k], a.s[k] = stride[k], a.d[k] = dilation[k];
       os.push_back((is[2 + k] - dilation[k] * (ks[2 + k] - 1) - 1) / stride[k] + 1);
     }
-    if (is[1] % groups) fail(NK_ERR_INVALID_ARG, "In channels %lld is not divisible by groups %lld", (long long)is[1], (long long)groups);
-    if (ks[0] % groups) fail(NK_ERR_INVALID_ARG, "Out channels %lld is not divisible by groups %lld", (long long)ks[0], (long long)groups);
-    if (ks[1] * groups != is[1]) fail(NK_ERR_INVALID_ARG, "convolution: kernel in-channels %lld x groups %lld != input channels %lld", (long long)ks[1], (long long)groups, (long long)is[1]);
-    nkg_var* v = new_like(kernel);
-    merge(v, kernel, input);
-    v->data = std::make_shared<Tensor>(kernel->ctx, os, input->data->dtype);
-    auto fw = std::make_shared<ConvolutionNd>();
-    fw->ctx = kernel->ctx;
-    fw->input = input->data;
-    fw->kernel = kernel->data;
-    fw->data = v->data;
-    fw->a = a;
-    uint64_t id = push(v, fw);
-    if (kernel->diff() || input->diff()) {
-      v->grad = std::make_shared<Gradient>(kernel->ctx, os, input->data->dtype);
-      auto bw = std::make_shared<ConvolutionNdBackward>();
-      bw->ctx = kernel->ctx;
-      bw->gradient = v->grad;
-      bw->input = input->data;
-      bw->kernel = kernel->data;
-      bw->input_grad = input->grad;
-      bw->kernel_grad = kernel->grad;
-      bw->a = a;
-      push_bwd(v, id, bw);
-    }
-    *out = v;
+    check_conv_channels(ks, is, groups);
+    *out = record(
+        {kernel, input}, os, input->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<ConvolutionNd>(kernel->ctx, input->data, kernel->data, d, a); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<ConvolutionNdBackward>(kernel->ctx, g, input->data, kernel->data, input->grad,
+                                                         kernel->grad, a);
+        });
   });
 }
 
@@ -2220,26 +1984,10 @@ int nkg_chunks(nkg_var* a, int ndim, const int64_t* chunk_shape, int capacity, n
     *count = (int)nblocks;
     if (capacity < nblocks) return;   // size query: nothing recorded
     const Shape cs(chunk_shape, chunk_shape + ndim);
-    for (int64_t i = 0; i < nblocks; ++i) {
-      TensorP od;
-      nkg_var* v = unary_node(a, cs, a->data->dtype, od);
-      auto fw = std::make_shared<Chunk>();
-      fw->ctx = a->ctx;
-      fw->operand = a->data;
-      fw->data = od;
-      fw->index = i;
-      uint64_t id = push(v, fw);
-      if (a->diff()) {
-        v->grad = std::make_shared<Gradient>(a->ctx, cs, od->dtype);
-        auto bw = std::make_shared<ChunkBackward>();
-        bw->ctx = a->ctx;
-        bw->gradient = v->grad;
-        bw->operand_grad = a->grad;
-        bw->index = i;
-        push_bwd(v, id, bw);
-      }
-      outs[i] = v;
-    }
+    for (int64_t i = 0; i < nblocks; ++i)
+      outs[i] = record(
+          {a}, cs, a->data->dtype, [&](const TensorP& d) { return std::make_shared<Chunk>(a->ctx, a->data, d, i); },
+          [&](const TensorP&, const GradientP& g) { return std::make_shared<ChunkBackward>(a->ctx, g, a->grad, i); });
   });
 }
 
@@ -2247,7 +1995,7 @@ int nkg_chunks(nkg_var* a, int ndim, const int64_t* chunk_shape, int capacity, n
 // VarDiff operands (the reference's four homogeneous methods and its Cat / Stack traits for mixed pairs)
 static void cat_impl(nkg_var* const* vars, int count, int axis, bool stack, nkg_var** out) {
   const char* who = stack ? "stack" : "cat";
-  if (!vars || !out) fail(NK_ERR_INVALID_ARG, "%s: NULL", who);
+  not_null({vars, out}, who);
   if (count < 1) fail(NK_ERR_INVALID_ARG, "%s: needs at least one operand, got %d", who, count);
   for (int i = 0; i < count; ++i)
     if (!vars[i]) fail(NK_ERR_INVALID_ARG, "%s: operand %d is NULL", who, i);
@@ -2292,40 +2040,19 @@ static void cat_impl(nkg_var* const* vars, int count, int axis, bool stack, nkg_
     int64_t len;
     lanes(os, axis, outer, len, inner);
   }
-  nk_ctx* ctx = a->ctx;
-  const int dt = a->data->dtype;
-  nkg_var* v = new_like(a);
-  for (int i = 0; i < count; ++i) {   // History::merge over every operand
-    v->fwd.insert(vars[i]->fwd.begin(), vars[i]->fwd.end());
-    v->bwd.insert(vars[i]->bwd.begin(), vars[i]->bwd.end());
-  }
-  v->data = std::make_shared<Tensor>(ctx, os, dt);
-  auto fw = std::make_shared<Concatenate>();
-  fw->ctx = ctx;
-  fw->data = v->data;
-  fw->lens = lens;
-  fw->outer = outer;
-  fw->inner = inner;
-  fw->stack = stack;
-  bool diff = false;
-  for (int i = 0; i < count; ++i) {
-    fw->operands.push_back(vars[i]->data);
-    diff = diff || vars[i]->diff();
-  }
-  const uint64_t id = push(v, fw);
-  if (diff) {
-    v->grad = std::make_shared<Gradient>(ctx, os, dt);
-    auto bw = std::make_shared<ConcatenateBackward>();
-    bw->ctx = ctx;
-    bw->gradient = v->grad;
-    for (int i = 0; i < count; ++i) bw->operand_grads.push_back(vars[i]->grad);
-    bw->lens = lens;
-    bw->outer = outer;
-    bw->inner = inner;
-    bw->stack = stack;
-    push_bwd(v, id, bw);
-  }
-  *out = v;
+  std::vector<nkg_var*> operands(vars, vars + count);
+  *out = record(
+      operands, os, a->data->dtype,
+      [&](const TensorP& d) {
+        std::vector<TensorP> xs;
+        for (nkg_var* x : operands) xs.push_back(x->data);
+        return std::make_shared<Concatenate>(a->ctx, std::move(xs), d, lens, outer, inner, stack);
+      },
+      [&](const TensorP&, const GradientP& g) {
+        std::vector<GradientP> grads;
+        for (nkg_var* x : operands) grads.push_back(x->grad);
+        return std::make_shared<ConcatenateBackward>(a->ctx, g, std::move(grads), lens, outer, inner, stack);
+      });
 }
 
 int nkg_cat(nkg_var* const* vars, int count, int axis, nkg_var** out) {
@@ -2338,7 +2065,7 @@ int nkg_stack(nkg_var* const* vars, int count, int axis, nkg_var** out) {
 
 int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out) {
   return guard([&] {
-    if (!a || !out) fail(NK_ERR_INVALID_ARG, "unsqueeze: NULL");
+    not_null({a, out}, "unsqueeze");
     Shape s = a->data->shape;
     if (axis < 0 || axis > (int)s.size())
       fail(NK_ERR_INVALID_ARG, "unsqueeze: axis %d out of range for a %d-dimensional operand", axis, (int)s.size());
@@ -2390,43 +2117,28 @@ static void cell_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_
   expect(b_ih, "bias_ih", {G * H});
   expect(b_hh, "bias_hh", {G * H});
 
-  nk_ctx* ctx = x->ctx;
-  const int dt = x->data->dtype;
-  auto fw = std::make_shared<RnnCell>();
-  fw->ctx = ctx;
-  fw->lstm = lstm;
-  fw->o = CellOperands{x->data, h->data, lstm ? c->data : nullptr, w_ih->data, w_hh->data, b_ih->data, b_hh->data};
-  fw->gi = std::make_shared<Tensor>(ctx, Shape{N, G * H}, NK_F32);
-  if (!lstm) fw->gh = std::make_shared<Tensor>(ctx, Shape{N, G * H}, NK_F32);
-  fw->h_out = std::make_shared<Tensor>(ctx, Shape{N, H}, dt);
-  if (lstm) fw->c_out = std::make_shared<Tensor>(ctx, Shape{N, H}, dt);
-
-  nkg_var* vh = new_like(x);
-  vh->data = fw->h_out;
-  for (const Arg& a : args) {   // History::merge over every operand
-    vh->fwd.insert(a.v->fwd.begin(), a.v->fwd.end());
-    vh->bwd.insert(a.v->bwd.begin(), a.v->bwd.end());
-  }
-  const uint64_t id = push(vh, fw);
-  bool diff = false;
-  for (const Arg& a : args) diff = diff || a.v->diff();
-  if (diff) {
-    vh->grad = std::make_shared<Gradient>(ctx, Shape{N, H}, dt);
-    auto bw = std::make_shared<RnnCellBackward>();
-    bw->ctx = ctx;
-    bw->lstm = lstm;
-    bw->o = fw->o;
-    bw->gi = fw->gi;
-    bw->gh = fw->gh;
-    bw->gradient = vh->grad;
-    bw->d = CellGrads{x->grad, h->grad, lstm ? c->grad : nullptr, w_ih->grad, w_hh->grad, b_ih->grad, b_hh->grad};
-    if (lstm) bw->c_out_grad = std::make_shared<Gradient>(ctx, Shape{N, H}, dt);
-    push_bwd(vh, id, bw);
-  }
+  std::vector<nkg_var*> operands;   // History::merge over every operand
+  for (const Arg& a : args) operands.push_back(a.v);
+  std::shared_ptr<RnnCell> cell;
+  std::shared_ptr<RnnCellBackward> cell_bwd;
+  nkg_var* vh = record(
+      operands, Shape{N, H}, x->data->dtype,
+      [&](const TensorP& d) {
+        cell = std::make_shared<RnnCell>(
+            x->ctx, lstm, CellOperands{x->data, h->data, lstm ? c->data : nullptr, w_ih->data, w_hh->data, b_ih->data, b_hh->data},
+            d);
+        return cell;
+      },
+      [&](const TensorP&, const GradientP& g) {
+        cell_bwd = std::make_shared<RnnCellBackward>(
+            x->ctx, g, *cell,
+            CellGrads{x->grad, h->grad, lstm ? c->grad : nullptr, w_ih->grad, w_hh->grad, b_ih->grad, b_hh->grad});
+        return cell_bwd;
+      });
   if (lstm) {   // the second output: same tapes, same op id (merging the two histories keeps one node)
     nkg_var* vc = new nkg_var(*vh);
-    vc->data = fw->c_out;
-    if (diff) vc->grad = std::dynamic_pointer_cast<RnnCellBackward>(vh->bwd[id])->c_out_grad;
+    vc->data = cell->c_out;
+    if (cell_bwd) vc->grad = cell_bwd->c_out_grad;
     *new_c = vc;
   }
   *new_h = vh;

@@ -46,6 +46,20 @@ def test_history_and_laziness(nk, dev):
         e.backward(1.0)
 
 
+@pytest.mark.parametrize("dtype", ["f32", "bf16"])
+def test_zeros_after_the_pool_reuses_memory(nk, dev, dtype):
+    """nk.zeros() (a leaf) is zero-filled even when the memory pool hands it a block that held other data: the LSTM /
+    GRU tests take their initial states from it."""
+    dt = nk.F32 if dtype == "f32" else nk.BF16
+    shape = (257, 129)
+    for _ in range(4):
+        junk = dev.full(shape, 3.5, dt)
+        dev.synchronize()
+        del junk
+        z = nk.zeros(dev, shape, dt)
+        assert np.array_equal(z.data(), np.zeros(shape, F32))
+
+
 def test_accumulate_protocol_and_zero_grad(nk, dev, O):
     """second backward() doubles leaf gradients (matrix_matrix_mul/test.rs:138-185), zero_grad clears"""
     rng = np.random.default_rng(0)
