@@ -174,6 +174,50 @@ int nk_nll_bwd(nk_ctx* ctx, void* dlogp, const void* target, int target_dtype, c
 int nk_sum_fwd(nk_ctx* ctx, float* out, const void* x, size_t n, int dtype, int mean);
 int nk_sum_bwd(nk_ctx* ctx, void* dx, const float* g, size_t n, int dtype, int mean, float beta);
 
+/* ---- the other criteria (csrc/nk_criteria.cu): absolute_error/mod.rs, bce/mod.rs, bce_with_logits/mod.rs,
+ * kldiv/mod.rs.  x and t share the element type `dtype`; the loss is a device f32 scalar; the backward writes
+ * dx = beta*dx + dloss/dx * (*g) in its own element type dx_dtype (f32 gradients of bf16 data).  The forward sums in a
+ * fixed order (f32 partials carried into double, one block summing the per-block partials), so repeated calls are
+ * bitwise equal.  mean divides by n for mae / bce / bce_with_logits and by `batch` (x's leading dimension) for kldiv --
+ * the reference's batch mean, torch's reduction='batchmean', not torch's 'mean'.
+ *   mae              |x - t|                                          dx: sign(x - t) * g, 0 where x == t
+ *   bce              -t*max(ln x, -100) + (t - 1)*max(ln(1 - x), -100)  dx: (x - t) / max((1 - x)*x, FLT_EPSILON) * g
+ *   bce_with_logits  (1 - t)*x + m + ln(e^-m + e^(-x-m)), m = max(-x, 0)  dx: (sigmoid(x) - t) * g
+ *   kldiv            t*(ln t - x) where t > 0, else 0 (x = log-probabilities)   dx: -t * g */
+int nk_mae_fwd(nk_ctx* ctx, float* loss, const void* x, const void* t, size_t n, int dtype, int mean);
+int nk_mae_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* x, const void* t, const float* g, size_t n, int dtype,
+               int mean, float beta);
+int nk_bce_fwd(nk_ctx* ctx, float* loss, const void* x, const void* t, size_t n, int dtype, int mean);
+int nk_bce_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* x, const void* t, const float* g, size_t n, int dtype,
+               int mean, float beta);
+int nk_bce_with_logits_fwd(nk_ctx* ctx, float* loss, const void* x, const void* t, size_t n, int dtype, int mean);
+int nk_bce_with_logits_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* x, const void* t, const float* g, size_t n,
+                           int dtype, int mean, float beta);
+int nk_kldiv_fwd(nk_ctx* ctx, float* loss, const void* x, const void* t, size_t n, int64_t batch, int dtype, int mean);
+int nk_kldiv_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* t, const float* g, size_t n, int64_t batch, int dtype,
+                 int mean, float beta);
+
+/* ---- dropout (dropout/mod.rs; csrc/nk_dropout.cu) with a counter-based generator ----
+ * Philox4x32-10 (Salmon et al., SC'11, the Random123 generator): key = the context's 64-bit seed; counter = (e/4 as a
+ * 64-bit value in words 0-1, the call id as a 64-bit value in words 2-3); element e uses output word e%4:
+ *   u = (r >> 8) * 2^-24,  q = 1 - (float)p,  keep iff u < q,  y = x / q in f32 (then rounded to dtype), else 0.
+ * The call id is a 64-bit counter kept in device memory by the context: every nk_dropout_fwd that draws a mask reads it
+ * and the last of its blocks to start advances it by one (a ticket in the same device state), so a captured step draws
+ * a new mask on every replay.  The state is allocated on first use (run one step eagerly before capturing), seeded from
+ * OS entropy unless nk_rng_seed ran first.
+ * nk_dropout_fwd: p == 0 copies x (no draw, mask untouched, may be NULL); p == 1 writes zeros (no draw); otherwise draws
+ * and writes the keep mask, bit e%32 of word e/32 (ceil(n/32) words, bits past n are 0).  p outside [0, 1] is an error.
+ * nk_dropout_bwd: dx = beta*dx + g*keep/q in dx's element type; g has element type dtype.  p == 0: the identity
+ * (dx = beta*dx + g); p == 1: dx = beta*dx; otherwise mask == NULL is the identity too (the backward of a forward that
+ * ran in eval mode).
+ * nk_rng_seed sets the seed and resets the call counter; it cannot be captured (NK_ERR_UNSUPPORTED while capturing).
+ * nk_rng_state reads both back (blocks). */
+int nk_dropout_fwd(nk_ctx* ctx, void* y, uint32_t* mask, const void* x, size_t n, int dtype, double p);
+int nk_dropout_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const uint32_t* mask, const void* g, size_t n, int dtype,
+                   double p, float beta);
+int nk_rng_seed(nk_ctx* ctx, uint64_t seed);
+int nk_rng_state(nk_ctx* ctx, uint64_t* seed, uint64_t* calls);
+
 /* ---- the rest of the elementwise family (SURVEY.md 8-f rank 1; csrc/nk_pointwise.cu) ----
  * binary ops broadcast like nk_add_bcast_fwd (utils.rs:97-125):
  *   subtraction/mod.rs:44-49, multiplication/mod.rs:44-49, division/mod.rs:44-49.

@@ -142,6 +142,27 @@ int nkg_cat(nkg_var* const* vars, int count, int axis, nkg_var** out);
 int nkg_stack(nkg_var* const* vars, int count, int axis, nkg_var** out);
 int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out);
 
+/* ---- the other criteria and dropout (var.rs:375-521, vardiff.rs:418-583) ----
+ * nkg_mae / nkg_bce / nkg_bce_with_logits / nkg_kldiv take (input, target, reduction) like nkg_mse_loss: same shape and
+ * element type, a non-differentiable target, a 0-d f32 result; ONE forward node and, for a differentiable input, ONE
+ * backward node (nk_b200.h gives the maths).  kldiv's Mean divides by the input's leading dimension (batch mean).
+ * Dropout's status is a shared flag (the reference's Rc<Cell<bool>>): 1 = train, 0 = eval; every node built with it
+ * sees later changes.  nkg_dropout: p outside [0, 1] fails with "Wrong probability received" and records nothing.
+ * The node owns its keep mask (allocated when the node is built, for 0 < p < 1).  Every forward() reads the status:
+ * train with 0 < p < 1 draws a new mask (nk_dropout_fwd), train with p == 1 writes zeros, eval or p == 0 copies.  The
+ * backward applies what the last forward did, whatever the status says by then.  A captured step replays the status it
+ * was captured with: the choice between drawing and copying is made on the host when the kernels are recorded. */
+typedef struct nkg_status nkg_status;
+int nkg_mae(nkg_var* input, nkg_var* target, int reduction, nkg_var** out);
+int nkg_bce(nkg_var* input, nkg_var* target, int reduction, nkg_var** out);
+int nkg_bce_with_logits(nkg_var* input, nkg_var* target, int reduction, nkg_var** out);
+int nkg_kldiv(nkg_var* input, nkg_var* target, int reduction, nkg_var** out);
+int nkg_status_create(int train, nkg_status** out);
+int nkg_status_set(nkg_status* status, int train);
+int nkg_status_get(nkg_status* status);   /* 1 train, 0 eval */
+int nkg_status_release(nkg_status* status);
+int nkg_dropout(nkg_var* a, double p, nkg_status* status, nkg_var** out);
+
 /* ---- gradient-ready hook (data parallel overlap): `cb(user, begin, end)` is called from inside nkg_backward(), on
  * the calling thread, right after the LAST kernel that accumulates into elements [begin, end) of this leaf's gradient
  * in the running backward pass has been launched -- so the caller can start the all-reduce of that range while the

@@ -8,7 +8,7 @@ from ._lib import NkError
 from .device import BF16, F32, CuArray, Device
 from . import ops
 from . import variable, nn, optim
-from .variable import (Reduction, Var, VarDiff, cat, from_ndarray, full, ones, rand, set_fusion, stack, zeros)
+from .variable import (Reduction, Status, Var, VarDiff, cat, from_ndarray, full, ones, rand, set_fusion, stack, zeros)
 
 __all__ = ["Device", "CuArray", "F32", "BF16", "NkError", "ops", "variable", "nn", "optim", "Var", "VarDiff",
-           "Reduction", "zeros", "ones", "full", "rand", "from_ndarray", "set_fusion", "cat", "stack"]
+           "Reduction", "Status", "zeros", "ones", "full", "rand", "from_ndarray", "set_fusion", "cat", "stack"]

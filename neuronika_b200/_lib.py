@@ -145,6 +145,18 @@ _PROTOS = {
     "nk_chunk_bwd": (i32, [vp, vp, i32, vp, i32, i32, pi64, pi64, i64, f32]),
     "nk_cat_fwd": (i32, [vp, vp, pvp, pi64, i32, i64, i64, i32]),
     "nk_cat_bwd": (i32, [vp, pvp, C.POINTER(i32), C.POINTER(f32), vp, i32, pi64, i32, i64, i64]),
+    "nk_mae_fwd": (i32, [vp, vp, vp, vp, sz, i32, i32]),
+    "nk_mae_bwd": (i32, [vp, vp, i32, vp, vp, vp, sz, i32, i32, f32]),
+    "nk_bce_fwd": (i32, [vp, vp, vp, vp, sz, i32, i32]),
+    "nk_bce_bwd": (i32, [vp, vp, i32, vp, vp, vp, sz, i32, i32, f32]),
+    "nk_bce_with_logits_fwd": (i32, [vp, vp, vp, vp, sz, i32, i32]),
+    "nk_bce_with_logits_bwd": (i32, [vp, vp, i32, vp, vp, vp, sz, i32, i32, f32]),
+    "nk_kldiv_fwd": (i32, [vp, vp, vp, vp, sz, i64, i32, i32]),
+    "nk_kldiv_bwd": (i32, [vp, vp, i32, vp, vp, sz, i64, i32, i32, f32]),
+    "nk_dropout_fwd": (i32, [vp, vp, vp, vp, sz, i32, C.c_double]),
+    "nk_dropout_bwd": (i32, [vp, vp, i32, vp, vp, sz, i32, C.c_double, f32]),
+    "nk_rng_seed": (i32, [vp, u64]),
+    "nk_rng_state": (i32, [vp, C.POINTER(u64), C.POINTER(u64)]),
 }
 
 for _name, (_res, _args) in _PROTOS.items():

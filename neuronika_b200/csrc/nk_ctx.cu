@@ -143,6 +143,7 @@ int nk_ctx_destroy(nk_ctx* ctx) {
     nk_graph_destroy(ctx, g);
   }
   if (ctx->workspace) cudaFree(ctx->workspace);
+  if (ctx->rng_state) cudaFree(ctx->rng_state);
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);

@@ -542,6 +542,12 @@ __global__ void __launch_bounds__(kThreads) sgd_kernel_vec4(TW* __restrict__ w, 
 
 }  // namespace
 
+int nk_reduce_finish(nk_ctx* ctx, float* out, const double* partials, int nparts, double scale) {
+  reduce_stage2<<<1, 32, 0, ctx->stream>>>(out, partials, nparts, scale);
+  NK_LAUNCHED(ctx, "reduce_stage2");
+  return NK_OK;
+}
+
 extern "C" {
 
 int nk_fill(nk_ctx* ctx, void* dptr, int dtype, size_t n, float value) {

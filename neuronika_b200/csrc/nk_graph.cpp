@@ -578,40 +578,118 @@ struct SumMeanBackward : Backward {  // sum/mod.rs:36-66, mean/mod.rs:36-71
   }
 };
 
-struct Loss : Forward {  // squared_error/mod.rs:11-58, nll/mod.rs:11-68
+// the criteria: squared_error/, nll/, absolute_error/, bce/, bce_with_logits/, kldiv/ (node/*/mod.rs)
+enum LossKind { kMse, kNll, kMae, kBce, kBceWithLogits, kKlDiv };
+static const char* loss_name(int kind, bool bwd) {
+  static const char* const fwd_names[] = {"SquaredError", "NegativeLogLikelihood", "AbsoluteError",
+                                          "BinaryCrossEntropy", "BCEWithLogits", "KLDiv"};
+  static const char* const bwd_names[] = {"SquaredErrorBackward", "NegativeLogLikelihoodBackward",
+                                          "AbsoluteErrorBackward", "BinaryCrossEntropyBackward",
+                                          "BCEWithLogitsBackward", "KLDivBackward"};
+  return bwd ? bwd_names[kind] : fwd_names[kind];
+}
+
+struct Loss : Forward {  // squared_error/mod.rs:11-58, nll/mod.rs:11-68, and the four above
   TensorP input, target, data;
-  bool mean, nll;
-  Loss(nk_ctx* c, TensorP x, TensorP t, TensorP d, bool m, bool n)
-      : Forward(c), input(std::move(x)), target(std::move(t)), data(std::move(d)), mean(m), nll(n) {}
-  const char* name() const override { return nll ? "NegativeLogLikelihood" : "SquaredError"; }
+  bool mean;
+  int kind;
+  Loss(nk_ctx* c, TensorP x, TensorP t, TensorP d, bool m, int k)
+      : Forward(c), input(std::move(x)), target(std::move(t)), data(std::move(d)), mean(m), kind(k) {}
+  const char* name() const override { return loss_name(kind, false); }
   void forward() override {
-    if (nll)
-      ck(ctx, nk_nll_fwd(ctx, (float*)data->wptr(), input->rptr(), target->rptr(), target->dtype, input->shape[0],
-                         input->shape[1], input->dtype, mean));
-    else
-      ck(ctx, nk_mse_fwd(ctx, (float*)data->wptr(), input->rptr(), target->rptr(), size_t(input->n()), input->dtype,
-                         mean));
+    float* out = (float*)data->wptr();
+    const void *x = input->rptr(), *t = target->rptr();
+    const size_t n = size_t(input->n());
+    const int dt = input->dtype;
+    switch (kind) {
+      case kNll:
+        ck(ctx, nk_nll_fwd(ctx, out, x, t, target->dtype, input->shape[0], input->shape[1], dt, mean));
+        break;
+      case kMse: ck(ctx, nk_mse_fwd(ctx, out, x, t, n, dt, mean)); break;
+      case kMae: ck(ctx, nk_mae_fwd(ctx, out, x, t, n, dt, mean)); break;
+      case kBce: ck(ctx, nk_bce_fwd(ctx, out, x, t, n, dt, mean)); break;
+      case kBceWithLogits: ck(ctx, nk_bce_with_logits_fwd(ctx, out, x, t, n, dt, mean)); break;
+      default: ck(ctx, nk_kldiv_fwd(ctx, out, x, t, n, input->shape[0], dt, mean)); break;
+    }
   }
 };
-struct LossBackward : Backward {  // squared_error/mod.rs:60-122, nll/mod.rs:70-133
+struct LossBackward : Backward {  // squared_error/mod.rs:60-122, nll/mod.rs:70-133, and the four above
   TensorP input, target;
   GradientP input_grad;
-  bool mean, nll;
-  LossBackward(nk_ctx* c, GradientP g, TensorP x, TensorP t, GradientP xg, bool m, bool n)
+  bool mean;
+  int kind;
+  LossBackward(nk_ctx* c, GradientP g, TensorP x, TensorP t, GradientP xg, bool m, int k)
       : Backward(c, std::move(g)), input(std::move(x)), target(std::move(t)), input_grad(std::move(xg)), mean(m),
-        nll(n) {}
-  const char* name() const override { return nll ? "NegativeLogLikelihoodBackward" : "SquaredErrorBackward"; }
+        kind(k) {}
+  const char* name() const override { return loss_name(kind, true); }
   void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad}); }
   void backward() override {
     const float* g = (const float*)gradient->get();
-    accumulate(ctx, input_grad, input->dtype, [&](void* d, float beta) {
-      if (nll)
-        ck(ctx, nk_nll_bwd(ctx, d, target->rptr(), target->dtype, g, input->shape[0], input->shape[1], input->dtype,
-                           mean, beta));
-      else
-        ck(ctx, nk_mse_bwd(ctx, d, input->rptr(), target->rptr(), g, size_t(input->n()), input->dtype, mean, beta));
-    });
+    if (kind == kNll || kind == kMse) {  // kernels that write the input's element type
+      accumulate(ctx, input_grad, input->dtype, [&](void* d, float beta) {
+        if (kind == kNll)
+          ck(ctx, nk_nll_bwd(ctx, d, target->rptr(), target->dtype, g, input->shape[0], input->shape[1], input->dtype,
+                             mean, beta));
+        else
+          ck(ctx, nk_mse_bwd(ctx, d, input->rptr(), target->rptr(), g, size_t(input->n()), input->dtype, mean, beta));
+      });
+    } else {  // kernels that write the gradient's own element type
+      accumulate(ctx, input_grad, [&](void* d, float beta) {
+        const int ddt = input_grad->dtype, dt = input->dtype;
+        const size_t n = size_t(input->n());
+        const void* t = target->rptr();
+        switch (kind) {
+          case kMae: ck(ctx, nk_mae_bwd(ctx, d, ddt, input->rptr(), t, g, n, dt, mean, beta)); break;
+          case kBce: ck(ctx, nk_bce_bwd(ctx, d, ddt, input->rptr(), t, g, n, dt, mean, beta)); break;
+          case kBceWithLogits: ck(ctx, nk_bce_with_logits_bwd(ctx, d, ddt, input->rptr(), t, g, n, dt, mean, beta)); break;
+          default: ck(ctx, nk_kldiv_bwd(ctx, d, ddt, t, g, n, input->shape[0], dt, mean, beta)); break;
+        }
+      });
+    }
     grad_written(input_grad);
+  }
+};
+
+// ------------------------------------------------------------------------------- dropout
+// What a Dropout forward did last; its backward applies exactly that, whatever the status says by then.
+enum DropoutDraw { kDropIdentity, kDropMasked, kDropZero };
+struct DropoutState {
+  int draw = kDropIdentity;
+};
+
+struct Dropout : Forward {  // dropout/mod.rs:15-78
+  TensorP operand, data, mask;  // mask: ceil(n/32) keep words, allocated when the node is built (the reference's noise)
+  double p;
+  std::shared_ptr<bool> train;  // the shared status, Rc<Cell<bool>>
+  std::shared_ptr<DropoutState> state;
+  Dropout(nk_ctx* c, TensorP x, TensorP d, TensorP m, double pp, std::shared_ptr<bool> st, std::shared_ptr<DropoutState> s)
+      : Forward(c), operand(std::move(x)), data(std::move(d)), mask(std::move(m)), p(pp), train(std::move(st)),
+        state(std::move(s)) {}
+  const char* name() const override { return "Dropout"; }
+  void forward() override {
+    const bool draw = *train && p != 0.0;
+    ck(ctx, nk_dropout_fwd(ctx, data->wptr(), draw && mask ? (uint32_t*)mask->wptr() : nullptr, operand->rptr(),
+                           size_t(data->n()), data->dtype, draw ? p : 0.0));
+    state->draw = !draw ? kDropIdentity : (1.0 - p == 0.0 ? kDropZero : kDropMasked);
+  }
+};
+struct DropoutBackward : Backward {  // dropout/mod.rs:80-132, with the forward's 1/(1-p) (SURVEY.md 8-c defect 8)
+  GradientP operand_grad;
+  TensorP mask;
+  double p;
+  std::shared_ptr<DropoutState> state;
+  DropoutBackward(nk_ctx* c, GradientP g, GradientP xg, TensorP m, double pp, std::shared_ptr<DropoutState> s)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), mask(std::move(m)), p(pp), state(std::move(s)) {}
+  const char* name() const override { return "DropoutBackward"; }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
+  void backward() override {
+    const void* g = gradient->get();
+    const bool identity = state->draw == kDropIdentity;
+    accumulate(ctx, operand_grad, [&](void* d, float beta) {
+      ck(ctx, nk_dropout_bwd(ctx, d, operand_grad->dtype, identity || !mask ? nullptr : (const uint32_t*)mask->rptr(), g,
+                             size_t(operand_grad->n()), gradient->dtype, identity ? 0.0 : p, beta));
+    });
+    grad_written(operand_grad);
   }
 };
 
@@ -1275,6 +1353,10 @@ struct nkg_var {
   bool diff() const { return grad != nullptr; }
 };
 
+struct nkg_status {  // the dropout status shared by the handle and every node built with it, Rc<Cell<bool>>
+  std::shared_ptr<bool> train;
+};
+
 namespace {
 
 void not_null(std::initializer_list<const void*> ptrs, const char* who) {
@@ -1744,9 +1826,11 @@ static int summean_impl(nkg_var* a, bool mean, nkg_var** out) {
 int nkg_sum(nkg_var* a, nkg_var** out) { return summean_impl(a, false, out); }
 int nkg_mean(nkg_var* a, nkg_var** out) { return summean_impl(a, true, out); }
 
-static int loss_impl(nkg_var* input, nkg_var* target, int reduction, bool nll, nkg_var** out) {
+static int loss_impl(nkg_var* input, nkg_var* target, int reduction, int kind, nkg_var** out) {
   return guard([&] {
     not_null({input, target, out}, "loss");
+    const bool nll = kind == kNll;
+    static const char* const who[] = {"mse_loss", "nll_loss", "mae", "bce", "bce_with_logits", "kldiv"};
     if (nll) {
       // class ids are stored as floats (nll/mod.rs:55 `target as usize`): an f32 target is accepted whatever the
       // input's element type; a bf16 target represents integers exactly only up to 256
@@ -1754,27 +1838,70 @@ static int loss_impl(nkg_var* input, nkg_var* target, int reduction, bool nll, n
       if (target->data->dtype == NK_BF16 && input->data->shape.size() == 2 && input->data->shape[1] > 256)
         fail(NK_ERR_INVALID_ARG, "nll_loss: a bf16 target cannot hold class ids above 256; pass the target as f32");
     } else {
-      require_same_dtype(input, target, "mse_loss");
+      require_same_dtype(input, target, who[kind]);
     }
     if (nll) {
       if (input->data->shape.size() != 2 || target->data->shape.size() != 1 ||
           target->data->shape[0] != input->data->shape[0])
         fail(NK_ERR_INVALID_ARG, "nll_loss: input must be (N, C) and target (N)");
     } else if (input->data->shape != target->data->shape) {
-      fail(NK_ERR_INVALID_ARG, "mse_loss: input and target shapes differ");
+      fail(NK_ERR_INVALID_ARG, "%s: input and target shapes differ", who[kind]);
     }
+    if (kind == kKlDiv && (input->data->shape.empty() || input->data->shape[0] == 0))
+      fail(NK_ERR_INVALID_ARG, "kldiv: the input needs a leading (batch) dimension");
     if (target->diff()) fail(NK_ERR_INVALID_ARG, "loss: the target must not be differentiable");
     const bool mean = reduction == NKG_MEAN;
     *out = record(
         {input, target}, Shape{}, NK_F32,
-        [&](const TensorP& d) { return std::make_shared<Loss>(input->ctx, input->data, target->data, d, mean, nll); },
+        [&](const TensorP& d) { return std::make_shared<Loss>(input->ctx, input->data, target->data, d, mean, kind); },
         [&](const TensorP&, const GradientP& g) {
-          return std::make_shared<LossBackward>(input->ctx, g, input->data, target->data, input->grad, mean, nll);
+          return std::make_shared<LossBackward>(input->ctx, g, input->data, target->data, input->grad, mean, kind);
         });
   });
 }
-int nkg_mse_loss(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, false, o); }
-int nkg_nll_loss(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, true, o); }
+int nkg_mse_loss(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, kMse, o); }
+int nkg_nll_loss(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, kNll, o); }
+int nkg_mae(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, kMae, o); }
+int nkg_bce(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, kBce, o); }
+int nkg_bce_with_logits(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, kBceWithLogits, o); }
+int nkg_kldiv(nkg_var* i, nkg_var* t, int r, nkg_var** o) { return loss_impl(i, t, r, kKlDiv, o); }
+
+int nkg_status_create(int train, nkg_status** out) {
+  return guard([&] {
+    not_null({out}, "nkg_status_create");
+    *out = new nkg_status{std::make_shared<bool>(train != 0)};
+  });
+}
+int nkg_status_set(nkg_status* s, int train) {
+  return guard([&] {
+    not_null({s}, "nkg_status_set");
+    *s->train = train != 0;
+  });
+}
+int nkg_status_get(nkg_status* s) { return s ? int(*s->train) : NK_ERR_INVALID_ARG; }
+int nkg_status_release(nkg_status* s) {
+  delete s;
+  return NK_OK;
+}
+
+int nkg_dropout(nkg_var* a, double p, nkg_status* status, nkg_var** out) {
+  return guard([&] {
+    not_null({a, status, out}, "dropout");
+    if (!(p >= 0.0 && p <= 1.0)) fail(NK_ERR_INVALID_ARG, "Wrong probability received: %g.", p);  // dropout/mod.rs:38-40
+    TensorP mask;
+    if (p != 0.0 && 1.0 - p != 0.0) {  // only a drawing forward has a mask
+      mask = std::make_shared<Tensor>(a->ctx, Shape{(a->data->n() + 31) / 32}, NK_F32);  // 32-bit words
+      mask->wptr();
+    }
+    auto state = std::make_shared<DropoutState>();
+    *out = record(
+        {a}, a->data->shape, a->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Dropout>(a->ctx, a->data, d, mask, p, status->train, state); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<DropoutBackward>(a->ctx, g, a->grad, mask, p, state);
+        });
+  });
+}
 
 int nkg_pad(nkg_var* a, int64_t ph, int64_t pw, float value, nkg_var** out) {
   return guard([&] {

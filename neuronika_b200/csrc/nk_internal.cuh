@@ -54,10 +54,15 @@ struct nk_ctx {
   // NCCL communicator owned by the context (nk_comm.cu; libnccl is bound at run time)
   void* comm = nullptr;
   int comm_world = 0, comm_rank = 0;
+  // dropout generator state in device memory (nk_dropout.cu): {seed, call counter, block ticket}, allocated on first use
+  unsigned long long* rng_state = nullptr;
 };
 
 int nk_set_error(nk_ctx* ctx, int code, const char* fmt, ...);
 int nk_workspace(nk_ctx* ctx, size_t bytes, void** out);
+// stage 2 of the fixed-order scalar reductions (nk_elementwise.cu): *out = float(scale * sum of the nparts double
+// partials), summed by one warp in a fixed order
+int nk_reduce_finish(nk_ctx* ctx, float* out, const double* partials, int nparts, double scale);
 
 #define NK_REQUIRE(ctx, cond, ...)                                      \
   do {                                                                  \
@@ -108,6 +113,24 @@ struct NkVec {
   __device__ __forceinline__ void set(int i, float v) { reinterpret_cast<T*>(&raw)[i] = nk_from_f32<T>(v); }
   __device__ __forceinline__ void load(const T* p) { raw = *reinterpret_cast<const uint4*>(p); }
   __device__ __forceinline__ void store(T* p) const { *reinterpret_cast<uint4*>(p) = raw; }
+};
+
+// 8 consecutive elements of T (one 16-byte vector of bf16, two of f32) with float accessors: lets kernels whose
+// operands have different element types step through all of them 8 elements at a time
+template <typename T>
+struct NkPack8 {
+  static constexpr int R = sizeof(T) / 2;
+  uint4 raw[R];
+  __device__ __forceinline__ float get(int i) const { return nk_to_f32<T>(reinterpret_cast<const T*>(raw)[i]); }
+  __device__ __forceinline__ void set(int i, float v) { reinterpret_cast<T*>(raw)[i] = nk_from_f32<T>(v); }
+  __device__ __forceinline__ void load(const T* p) {
+#pragma unroll
+    for (int r = 0; r < R; ++r) raw[r] = reinterpret_cast<const uint4*>(p)[r];
+  }
+  __device__ __forceinline__ void store(T* p) const {
+#pragma unroll
+    for (int r = 0; r < R; ++r) reinterpret_cast<uint4*>(p)[r] = raw[r];
+  }
 };
 
 __device__ __forceinline__ float nk_warp_sum(float v) {

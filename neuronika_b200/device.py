@@ -72,6 +72,18 @@ class Device:
     def last_conv_kernel(self) -> str:
         return L.lib.nk_last_conv_kernel(self.ctx).decode()
 
+    def manual_seed(self, seed: int) -> None:
+        """Seed the device's dropout generator and reset its call counter (nk_rng_seed): the masks drawn afterwards are
+        a function of the seed and of how many dropout forwards ran since.  Not while capturing.  Without it the seed
+        comes from OS entropy.  Data-parallel replicas that should draw different masks need different seeds."""
+        L.check(L.lib.nk_rng_seed(self.ctx, int(seed) & (2 ** 64 - 1)), self.ctx)
+
+    def rng_state(self) -> Tuple[int, int]:
+        """(seed, dropout calls since seeding) of the device's generator (nk_rng_state; synchronises)."""
+        seed, calls = C.c_uint64(), C.c_uint64()
+        L.check(L.lib.nk_rng_state(self.ctx, C.byref(seed), C.byref(calls)), self.ctx)
+        return int(seed.value), int(calls.value)
+
     def timer_start(self) -> None:
         L.check(L.lib.nk_timer_start(self.ctx), self.ctx)
 

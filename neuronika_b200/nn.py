@@ -95,6 +95,30 @@ class LSTMCell:
         return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]
 
 
+class Dropout:
+    """Dropout with probability p and a status of its own: `train()` (the initial mode) draws a new mask on every
+    forward() of the graph, `eval()` passes the input through.  The reference's docs name `nn::Dropout`; its crate
+    defines only the op (var.rs:375-397)."""
+
+    def __init__(self, p: float):
+        if not 0.0 <= p <= 1.0:
+            raise ValueError(f"Wrong probability received: {p}.")
+        self.p = float(p)
+        self.status = V.Status(True)
+
+    def forward(self, input: V.Var) -> V.Var:
+        return input.dropout(self.p, self.status)
+
+    def train(self) -> None:
+        self.status.train()
+
+    def eval(self) -> None:
+        self.status.eval()
+
+    def parameters(self):
+        return []
+
+
 class GRUCell:
     """One GRU step (neuronika-nn/src/lib.rs:543-626, = torch.nn.GRUCell): weight_ih (3H, I), weight_hh (3H, H),
     bias_ih, bias_hh (3H,), all ~ U(-k, k), k = 1/sqrt(hidden_size); gate chunks [r | z | n].  One fused graph node."""

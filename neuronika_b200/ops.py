@@ -137,6 +137,48 @@ def nll_bwd(dlogp, target, g, mean=True, beta=1.0):
     return dlogp
 
 
+_CRITERIA = {"mae": (lib.nk_mae_fwd, lib.nk_mae_bwd), "bce": (lib.nk_bce_fwd, lib.nk_bce_bwd),
+             "bce_with_logits": (lib.nk_bce_with_logits_fwd, lib.nk_bce_with_logits_bwd),
+             "kldiv": (lib.nk_kldiv_fwd, lib.nk_kldiv_bwd)}
+
+
+def criterion(name: str, x: CuArray, t: CuArray, mean=True, out=None) -> CuArray:
+    """the loss of one of "mae", "bce", "bce_with_logits", "kldiv" into a 0-d f32 array (kldiv's mean: by x.shape[0])"""
+    out = out or CuArray(x.device, (), F32)
+    fwd = _CRITERIA[name][0]
+    if name == "kldiv":
+        _ck(fwd(x.device.ctx, out.ptr, x.ptr, t.ptr, x.size, x.shape[0] if x.shape else 1, x.dtype, int(mean)), x.device)
+    else:
+        _ck(fwd(x.device.ctx, out.ptr, x.ptr, t.ptr, x.size, x.dtype, int(mean)), x.device)
+    return out
+
+
+def criterion_bwd(name: str, dx: CuArray, x: CuArray, t: CuArray, g: CuArray, mean=True, beta=1.0) -> CuArray:
+    """dx = beta*dx + dloss/dx * g, dx in its own element type"""
+    bwd = _CRITERIA[name][1]
+    if name == "kldiv":
+        _ck(bwd(x.device.ctx, dx.ptr, dx.dtype, t.ptr, g.ptr, x.size, x.shape[0] if x.shape else 1, x.dtype, int(mean),
+                float(beta)), x.device)
+    else:
+        _ck(bwd(x.device.ctx, dx.ptr, dx.dtype, x.ptr, t.ptr, g.ptr, x.size, x.dtype, int(mean), float(beta)), x.device)
+    return dx
+
+
+def dropout(x: CuArray, p: float, mask: CuArray | None = None, out=None) -> CuArray:
+    """y = x*keep/(1-p) with a new mask from the device's generator; `mask` (ceil(n/32) 32-bit words, e.g. an f32 array
+    of that many elements) receives the keep bits"""
+    out = out or CuArray(x.device, x.shape, x.dtype)
+    _ck(lib.nk_dropout_fwd(x.device.ctx, out.ptr, mask.ptr if mask is not None else None, x.ptr, x.size, x.dtype,
+                           float(p)), x.device)
+    return out
+
+
+def dropout_bwd(dx: CuArray, mask: CuArray | None, g: CuArray, p: float, beta=1.0) -> CuArray:
+    _ck(lib.nk_dropout_bwd(g.device.ctx, dx.ptr, dx.dtype, mask.ptr if mask is not None else None, g.ptr, g.size,
+                           g.dtype, float(p), float(beta)), g.device)
+    return dx
+
+
 def reduce_sum(x: CuArray, mean=False, out=None) -> CuArray:
     out = out or CuArray(x.device, (), F32)
     _ck(lib.nk_sum_fwd(x.device.ctx, out.ptr, x.ptr, x.size, x.dtype, int(mean)), x.device)

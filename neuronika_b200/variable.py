@@ -84,6 +84,15 @@ _G = {
     "nkg_cat": (i32, [pvp, i32, i32, pvp]),
     "nkg_stack": (i32, [pvp, i32, i32, pvp]),
     "nkg_unsqueeze": (i32, [vp, i32, pvp]),
+    "nkg_mae": (i32, [vp, vp, i32, pvp]),
+    "nkg_bce": (i32, [vp, vp, i32, pvp]),
+    "nkg_bce_with_logits": (i32, [vp, vp, i32, pvp]),
+    "nkg_kldiv": (i32, [vp, vp, i32, pvp]),
+    "nkg_status_create": (i32, [i32, pvp]),
+    "nkg_status_set": (i32, [vp, i32]),
+    "nkg_status_get": (i32, [vp]),
+    "nkg_status_release": (i32, [vp]),
+    "nkg_dropout": (i32, [vp, C.c_double, vp, pvp]),
 }
 for _n, (_r, _a) in _G.items():
     _f = getattr(lib, _n)
@@ -117,6 +126,34 @@ class Reduction:
     """neuronika-variable/src/lib.rs:29-36"""
     Mean = 0
     Sum = 1
+
+
+class Status:
+    """The train / eval flag that dropout nodes share (the reference's `Rc<Cell<bool>>`): every node built with it reads
+    it on each forward().  A captured step keeps the flag it was captured with."""
+
+    def __init__(self, train: bool = True):
+        h = vp()
+        _ck(lib.nkg_status_create(int(bool(train)), C.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib.nkg_status_release(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def train(self) -> None:
+        _ck(lib.nkg_status_set(self._h, 1))
+
+    def eval(self) -> None:
+        _ck(lib.nkg_status_set(self._h, 0))
+
+    def get(self) -> bool:
+        """True in training mode."""
+        return bool(lib.nkg_status_get(self._h))
 
 
 class Var:
@@ -225,6 +262,23 @@ class Var:
     def mean(self): return self._unary(lib.nkg_mean)
     def mse_loss(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_mse_loss, target, int(reduction))
     def nll_loss(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_nll_loss, target, int(reduction))
+    def mae(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_mae, target, int(reduction))
+    def bce(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_bce, target, int(reduction))
+
+    def bce_with_logits(self, target, reduction=Reduction.Mean):
+        return self._binary(lib.nkg_bce_with_logits, target, int(reduction))
+
+    def kldiv(self, target, reduction=Reduction.Mean):
+        """KL divergence of `target` (probabilities) from the receiver (log-probabilities).  Mean divides by the
+        leading (batch) dimension, like torch's reduction='batchmean', not by the element count."""
+        return self._binary(lib.nkg_kldiv, target, int(reduction))
+
+    def dropout(self, p: float, status: Status | None = None):
+        """`dropout(p, status)` (var.rs:375-397): zeroes each element with probability p and scales the rest by 1/(1-p)
+        while `status` is in training mode; a copy in eval mode.  Each forward() draws a new mask from the device's
+        Philox generator (Device.manual_seed).  Without a status the node has its own, in training mode."""
+        return self._unary(lib.nkg_dropout, float(p), (status or Status())._h)
+
     def flatten(self): return self._unary(lib.nkg_flatten)
 
     def pad(self, padding, value: float = 0.0, mode: str = "constant"):
