@@ -141,7 +141,7 @@ int nk_gemm_relu_bwd_colsum(nk_ctx* ctx, int transA, int transB, int64_t M, int6
 int nk_add_bcast_fwd(nk_ctx* ctx, void* y, const void* l, const void* r, int dtype,
                      int y_ndim, const int64_t* y_shape, int l_ndim, const int64_t* l_shape,
                      int r_ndim, const int64_t* r_shape);
-/* dst = beta*dst + unbroadcast(g -> dst_shape) */
+/* dst = beta*dst + unbroadcast(g -> dst_shape); an empty g leaves dst = beta*dst (g may then be NULL) */
 int nk_unbroadcast_acc(nk_ctx* ctx, void* dst, int dst_dtype, int dst_ndim,
                        const int64_t* dst_shape, const void* g, int g_dtype, int g_ndim,
                        const int64_t* g_shape, float beta);
@@ -281,7 +281,8 @@ int nk_pad2d_bwd(nk_ctx* ctx, void* dx, const void* g, int64_t planes, int64_t h
  *   Ho = (H - dh*(kh-1) - 1)/sh + 1.
  *   fwd optionally fuses + bias[Cout] (the Conv2d layer's (Cout,1,1) bias,
  *   neuronika-nn/src/lib.rs:774) and ReLU; bwd_kernel optionally also accumulates
- *   dbias[Cout] += sum_{n,p,q} g. */
+ *   dbias[Cout] += sum_{n,p,q} g.  With N = 0, bwd_kernel scales dW (and dbias) by beta and
+ *   g / x may be NULL. */
 int nk_conv2d_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int relu,
                   int64_t n, int64_t cin, int64_t h, int64_t wd, int64_t cout, int64_t kh,
                   int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw, int64_t groups,

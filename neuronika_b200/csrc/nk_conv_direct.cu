@@ -215,9 +215,9 @@ int nk_conv2d_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbias, cons
   int rc = check_dims(ctx, "nk_conv2d_bwd_kernel", d);
   if (rc) return rc;
   const int64_t nw = d.cout * (d.cin / d.groups) * d.kh * d.kw;
-  NK_REQUIRE(ctx, dwt && g && x, "nk_conv2d_bwd_kernel: NULL pointer");
-  if (d.n * d.ho * d.wo == 0) return NK_OK;
-  if (dtype == NK_BF16 && groups == 1 && ctx->conv_engine != NK_CONV_DIRECT) {
+  // an empty batch adds nothing: dW (and dbias) = beta * dW, as in nk_convnd_bwd_kernel; g and x may then be NULL
+  NK_REQUIRE(ctx, dwt && (d.n == 0 || (g && x)), "nk_conv2d_bwd_kernel: NULL pointer");
+  if (d.n > 0 && dtype == NK_BF16 && groups == 1 && ctx->conv_engine != NK_CONV_DIRECT) {
     rc = nk_conv_gemm_bwd_kernel(ctx, dwt, dw_dtype, g, x, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw, beta);
     if (rc == NK_OK && dbias) {
       int64_t dshape[3] = {d.cout, 1, 1};
@@ -237,18 +237,20 @@ int nk_conv2d_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbias, cons
   rc = nk_workspace(ctx, size_t(nw) * sizeof(float), (void**)&scratch);
   if (rc) return rc;
   NK_CUDA(ctx, cudaMemsetAsync(scratch, 0, size_t(nw) * sizeof(float), ctx->stream));
-  int64_t want_y = (int64_t(ctx->sm_count) * 4 + nw - 1) / nw;
-  if (want_y > d.n) want_y = d.n;
-  if (want_y < 1) want_y = 1;
-  const int64_t n_per_block = (d.n + want_y - 1) / want_y;
-  const int64_t gy = (d.n + n_per_block - 1) / n_per_block;
-  NK_REQUIRE(ctx, gy <= 65535, "nk_conv2d_bwd_kernel: batch grid too large");
-  dim3 grid((unsigned)nw, (unsigned)gy);
-  if (dtype == NK_BF16)
-    conv_bwd_kernel_direct<__nv_bfloat16><<<grid, kThreads, 0, ctx->stream>>>(scratch, (const __nv_bfloat16*)g, (const __nv_bfloat16*)x, d, n_per_block);
-  else
-    conv_bwd_kernel_direct<float><<<grid, kThreads, 0, ctx->stream>>>(scratch, (const float*)g, (const float*)x, d, n_per_block);
-  NK_LAUNCHED(ctx, "conv_bwd_kernel_direct");
+  if (d.n > 0) {
+    int64_t want_y = (int64_t(ctx->sm_count) * 4 + nw - 1) / nw;
+    if (want_y > d.n) want_y = d.n;
+    if (want_y < 1) want_y = 1;
+    const int64_t n_per_block = (d.n + want_y - 1) / want_y;
+    const int64_t gy = (d.n + n_per_block - 1) / n_per_block;
+    NK_REQUIRE(ctx, gy <= 65535, "nk_conv2d_bwd_kernel: batch grid too large");
+    dim3 grid((unsigned)nw, (unsigned)gy);
+    if (dtype == NK_BF16)
+      conv_bwd_kernel_direct<__nv_bfloat16><<<grid, kThreads, 0, ctx->stream>>>(scratch, (const __nv_bfloat16*)g, (const __nv_bfloat16*)x, d, n_per_block);
+    else
+      conv_bwd_kernel_direct<float><<<grid, kThreads, 0, ctx->stream>>>(scratch, (const float*)g, (const float*)x, d, n_per_block);
+    NK_LAUNCHED(ctx, "conv_bwd_kernel_direct");
+  }
   int blocks = int((nw + kThreads - 1) / kThreads);
   if (dw_dtype == NK_BF16)
     finalize_dw<__nv_bfloat16><<<blocks, kThreads, 0, ctx->stream>>>((__nv_bfloat16*)dwt, scratch, nw, beta);

@@ -697,7 +697,12 @@ int nk_unbroadcast_acc(nk_ctx* ctx, void* dst, int dst_dtype, int dst_ndim, cons
     n_dst *= size_t(dsh[k]);
     n_g *= size_t(g_shape[k]);
   }
-  if (n_dst == 0 || n_g == 0) return NK_OK;
+  if (n_dst == 0) return NK_OK;
+  if (n_g == 0) {  // nothing to sum: dst = beta*dst (a fill of 0 when beta = 0); g may be NULL
+    NK_REQUIRE(ctx, dst, "nk_unbroadcast_acc: NULL pointer");
+    if (beta == 1.f) return NK_OK;
+    NK_DISPATCH_DTYPE(dst_dtype, T, return (launch_ew<T, 0>(ctx, "scale", dst, nullptr, nullptr, nullptr, n_dst, beta, OpFill{0.f})));
+  }
   NK_REQUIRE(ctx, dst && g, "nk_unbroadcast_acc: NULL pointer");
   if (n_dst == n_g) {  // same shape: dst = beta*dst + g
     int blocks = ew_blocks(ctx, n_g);

@@ -155,6 +155,7 @@ int launch(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K,
   }
   int64_t k_per_split = (K + splits - 1) / splits;
   k_per_split = (k_per_split + BK - 1) / BK * BK;
+  if (k_per_split == 0) k_per_split = BK;   // K = 0: one pass of no steps, the epilogue alone (C = beta*C + bias)
   splits = int((K + k_per_split - 1) / k_per_split);
   if (splits < 1) splits = 1;
   float* partial = nullptr;
