@@ -351,6 +351,18 @@ int nk_gru_cell_fwd(nk_ctx* ctx, void* h_out, const float* igates, const float* 
 int nk_gru_cell_bwd(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, void* dh_prev, float beta_dh,
                     const float* igates, const float* hgates, const void* h_prev, const void* dh_out, int64_t n,
                     int64_t hidden, int dtype);
+/* Backward time steps of the LSTM / GRU sequence nodes (nk_graph.h, nkg_lstm / nkg_gru).  As nk_lstm_cell_bwd /
+ * nk_gru_cell_bwd, except that the hidden-state gradient of the step is the sum of two sources, dh_out (element type
+ * `dtype`: this step's slice of the output gradient) and dh_rec (f32: what the later steps sent back through the hidden
+ * state), either of which may be NULL = zero, and that the gradient carried from step to step is f32 whatever `dtype`
+ * and is updated in place:
+ *   LSTM  dc (n, H) f32 holds dc_out on entry and dc_prev = sigmoid(f)*dc_total on return;
+ *   GRU   dh_rec holds the pointwise part z*dh of the previous step's gradient on return (the caller adds
+ *         dhgates.W_hh); it is left alone when NULL. */
+int nk_lstm_seq_bwd_step(nk_ctx* ctx, void* dgates, int dgates_dtype, float* dc, const float* gates, const void* c_prev,
+                         const void* dh_out, const float* dh_rec, int64_t n, int64_t hidden, int dtype);
+int nk_gru_seq_bwd_step(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, float* dh_rec, const float* igates,
+                        const float* hgates, const void* h_prev, const void* dh_out, int64_t n, int64_t hidden, int dtype);
 /* chunks (chunk/mod.rs): y = block `index` of x in row-major block order (ndarray's exact_chunks: trailing partial blocks
  * are dropped); a bit-exact copy.  Backward: dx[block] = beta*dx[block] + g, nothing else of dx is touched. */
 int nk_chunk_fwd(nk_ctx* ctx, void* y, const void* x, int ndim, const int64_t* x_shape, const int64_t* chunk_shape,

@@ -130,6 +130,21 @@ int nkg_lstm_cell(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var*
 int nkg_gru_cell(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
                  nkg_var* bias_hh, nkg_var** new_hidden);
 
+/* ---- recurrent sequence layers (one layer, one direction, time-major) ----
+ * nkg_lstm / nkg_gru: the cell above applied to every step of input (T, N, I), T >= 1, from the initial states hidden
+ * (and cell_state) (N, H), with the cells' weight layout.  `output` (T, N, H) holds every step's hidden state, so the
+ * last hidden state is output[T-1]; `last_cell_state` (N, H) is the LSTM's cell state after step T-1.  Each call records
+ * ONE forward and ONE backward node whatever T is: the products that do not depend on the recurrence (x.W_ih^T + b_ih,
+ * dW_ih, dW_hh, dx, the bias gradients) run once over all T*N rows, and the state gradient is carried from step to step
+ * in f32.  The node keeps the f32 gate pre-activations of all steps (T*N*G values; twice that for the GRU, as T cell nodes
+ * do) and the backward allocates T*N*G elements of the operands' type for its own duration.  Operands are validated as
+ * the cells': one element type, one context, any mix of differentiable and plain operands; only the differentiable
+ * ones get gradient work, and the outputs are differentiable if any operand is. */
+int nkg_lstm(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
+             nkg_var* bias_hh, nkg_var** output, nkg_var** last_cell_state);
+int nkg_gru(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih, nkg_var* bias_hh,
+            nkg_var** output);
+
 /* ---- concatenation (var.rs:564-645, vardiff.rs:627-; multi_concatenate/mod.rs, multi_stack/mod.rs) ----
  * nkg_cat: the `count` operands side by side along `axis` (0 <= axis < ndim; equal shapes on every other axis, any length
  * along `axis`, 0 included).  nkg_stack: identical shapes, joined along a new axis 0 <= axis <= ndim.  Both record ONE

@@ -141,6 +141,8 @@ _PROTOS = {
     "nk_lstm_cell_bwd": (i32, [vp, vp, i32, vp, f32, vp, vp, vp, vp, i64, i64, i32]),
     "nk_gru_cell_fwd": (i32, [vp, vp, vp, vp, vp, i64, i64, i32]),
     "nk_gru_cell_bwd": (i32, [vp, vp, vp, i32, vp, f32, vp, vp, vp, vp, i64, i64, i32]),
+    "nk_lstm_seq_bwd_step": (i32, [vp, vp, i32, vp, vp, vp, vp, vp, i64, i64, i32]),
+    "nk_gru_seq_bwd_step": (i32, [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, i64, i32]),
     "nk_chunk_fwd": (i32, [vp, vp, vp, i32, pi64, pi64, i64, i32]),
     "nk_chunk_bwd": (i32, [vp, vp, i32, vp, i32, i32, pi64, pi64, i64, f32]),
     "nk_cat_fwd": (i32, [vp, vp, pvp, pi64, i32, i64, i64, i32]),

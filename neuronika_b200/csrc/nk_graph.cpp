@@ -1201,6 +1201,7 @@ struct ConcatenateBackward : Backward {
 // lifetime, so a second backward() still works), one kernel applies the gates (nk_lstm_cell_fwd / nk_gru_cell_fwd).
 // The backward runs the gate kernel, then the weight gradients (dW += dG^T.x, TN), the bias gradients (column sums of
 // dG) and the input / state gradients (dx += dG.W, NN), only for the operands that are differentiable.
+// A whole sequence of such steps as one node is RnnSeq / RnnSeqBackward below ("recurrent sequence layers").
 struct CellOperands {
   TensorP x, h, c, w_ih, w_hh, b_ih, b_hh;   // c: LSTM only
 };
@@ -1334,6 +1335,181 @@ struct RnnCellBackward : Backward {  // `gradient` is the new hidden state's; c_
   void with_grad() override {
     Backward::with_grad();
     if (c_out_grad) c_out_grad->with_grad();
+  }
+};
+
+// ------------------------------------------------------------------------------- recurrent sequence layers
+// nn.LSTM / nn.GRU (one layer, one direction, time-major) as ONE forward and ONE backward node whatever T is.  Of a
+// cell's products only h_{t-1}.W_hh^T (forward) and dG_t.W_hh (backward) depend on the recurrence; the others run once
+// over all T*N rows: X.W_ih^T + b_ih, dW_ih, dW_hh, dX and the bias column sums.  The node keeps the f32 gate
+// pre-activations of every step (what T cell nodes keep) and, for the LSTM, the cell states.  The backward carries the
+// state gradients (dc, and the part of dh that comes back through W_hh) in f32 from step T-1 down to step 0
+// (nk_lstm_seq_bwd_step / nk_gru_seq_bwd_step) and converts them once, into the gradients of the initial states.
+static inline char* at(void* p, int64_t elems, int dt) { return static_cast<char*>(p) + size_t(elems) * esize(dt); }
+static inline const char* at(const void* p, int64_t elems, int dt) {
+  return static_cast<const char*>(p) + size_t(elems) * esize(dt);
+}
+struct RnnSeq : Forward {
+  bool lstm;
+  CellOperands o;      // x is (T, N, I)
+  TensorP gi, gh;      // f32 gate pre-activations of every step: LSTM (T*N, 4H) in gi; GRU (T*N, 3H) in gi and gh
+  TensorP out;         // (T, N, H): every step's hidden state
+  TensorP cs, c_last;  // LSTM: the cell states of steps 0 .. T-2, (T-1, N, H), and the last one, (N, H)
+  RnnSeq(nk_ctx* c, bool l, CellOperands ops, TensorP output) : Forward(c), lstm(l), o(std::move(ops)), out(std::move(output)) {
+    const int64_t T = o.x->shape[0], N = o.x->shape[1], H = o.h->shape[1], G = o.w_ih->shape[0];
+    gi = std::make_shared<Tensor>(c, Shape{T * N, G}, NK_F32);
+    if (!lstm) gh = std::make_shared<Tensor>(c, Shape{T * N, G}, NK_F32);
+    if (lstm) {
+      cs = std::make_shared<Tensor>(c, Shape{T - 1, N, H}, out->dtype);
+      c_last = std::make_shared<Tensor>(c, Shape{N, H}, out->dtype);
+    }
+  }
+  const char* name() const override { return lstm ? "LSTM" : "GRU"; }
+  // the state before step t: the initial one, or what step t-1 wrote
+  const void* h_prev(int64_t t, int64_t NH) const { return t ? at(out->rptr(), (t - 1) * NH, out->dtype) : o.h->rptr(); }
+  const void* c_prev(int64_t t, int64_t NH) const { return t ? at(cs->rptr(), (t - 1) * NH, cs->dtype) : o.c->rptr(); }
+  void forward() override {
+    const int64_t T = o.x->shape[0], N = o.x->shape[1], I = o.x->shape[2], H = o.h->shape[1], G = o.w_ih->shape[0];
+    const int dt = o.x->dtype;
+    gemm(ctx, false, true, T * N, G, I, o.x->rptr(), I, o.w_ih->rptr(), I, 0.f, gi->wptr(), dt, NK_F32, o.b_ih->rptr(),
+         o.b_ih->dtype);
+    void* y = out->wptr();
+    for (int64_t t = 0; t < T; ++t) {
+      float* gi_t = reinterpret_cast<float*>(at(gi->rptr(), t * N * G, NK_F32));
+      void* y_t = at(y, t * N * H, dt);
+      if (lstm) {
+        gemm(ctx, false, true, N, G, H, h_prev(t, N * H), H, o.w_hh->rptr(), H, 1.f, gi_t, dt, NK_F32, o.b_hh->rptr(),
+             o.b_hh->dtype);
+        void* c_t = t == T - 1 ? c_last->wptr() : at(cs->wptr(), t * N * H, dt);
+        ck(ctx, nk_lstm_cell_fwd(ctx, c_t, y_t, gi_t, c_prev(t, N * H), N, H, dt));
+      } else {
+        float* gh_t = reinterpret_cast<float*>(at(gh->wptr(), t * N * G, NK_F32));
+        gemm(ctx, false, true, N, G, H, h_prev(t, N * H), H, o.w_hh->rptr(), H, 0.f, gh_t, dt, NK_F32, o.b_hh->rptr(),
+             o.b_hh->dtype);
+        ck(ctx, nk_gru_cell_fwd(ctx, y_t, gi_t, gh_t, h_prev(t, N * H), N, H, dt));
+      }
+    }
+  }
+};
+
+struct RnnSeqBackward : Backward {  // `gradient` is the output's, (T, N, H); c_last_grad the last cell state's (LSTM)
+  std::shared_ptr<RnnSeq> fw;
+  CellGrads d;
+  GradientP c_last_grad;
+  RnnSeqBackward(nk_ctx* c, GradientP g, std::shared_ptr<RnnSeq> f, CellGrads grads)
+      : Backward(c, std::move(g)), fw(std::move(f)), d(std::move(grads)) {
+    if (fw->lstm) c_last_grad = std::make_shared<Gradient>(c, fw->c_last->shape, fw->c_last->dtype);
+  }
+  const char* name() const override { return fw->lstm ? "LSTMBackward" : "GRUBackward"; }
+  void targets(std::vector<Gradient*>& out) override {
+    add_targets(out, {&d.w_hh, &d.w_ih, &d.b_ih, &d.b_hh, &d.x, &d.h, &d.c});
+  }
+  // a weight with a data-parallel reduce-scatter plan is computed locally and reported as not pushed, as the cell does
+  void weight_done(const GradientP& g) {
+    Gradient* r = g->root();
+    if (r->rs_world > 1 && r->rs_hook && r->last_writer == g_bwd_pos) r->rs_hook(r->rs_user, 0);
+    grad_written(g);
+  }
+  void bias(const GradientP& g, const void* dG, int64_t G, int64_t rows, int dt) {
+    if (!g) return;
+    const int64_t ds[1] = {G}, gs[2] = {rows, G};
+    accumulate(ctx, g, [&](void* p, float beta) { ck(ctx, nk_unbroadcast_acc(ctx, p, g->dtype, 1, ds, dG, dt, 2, gs, beta)); });
+    grad_written(g);
+  }
+  // g += the f32 (N, H) state gradient the loop carried, converted into g's element type
+  void state(const GradientP& g, const float* carried, int64_t N, int64_t H) {
+    if (!g) return;
+    const int64_t s[2] = {N, H};
+    accumulate(ctx, g, [&](void* p, float beta) { ck(ctx, nk_unbroadcast_acc(ctx, p, g->dtype, 2, s, carried, NK_F32, 2, s, beta)); });
+    grad_written(g);
+  }
+  void backward() override {
+    const CellOperands& o = fw->o;
+    const bool lstm = fw->lstm;
+    const int64_t T = o.x->shape[0], N = o.x->shape[1], I = o.x->shape[2], H = o.h->shape[1], G = o.w_ih->shape[0];
+    const int64_t NH = N * H, NG = N * G;
+    const int dt = o.x->dtype;
+    const size_t gbytes = size_t(T) * size_t(NG) * esize(dt), sbytes = size_t(NH) * sizeof(float);
+    void *dI = nullptr, *dH = nullptr, *dh_rec = nullptr, *dc = nullptr;
+    auto release = [&] {
+      if (dc) nk_free(ctx, dc);
+      if (dh_rec) nk_free(ctx, dh_rec);
+      if (dH && dH != dI) nk_free(ctx, dH);
+      if (dI) nk_free(ctx, dI);
+    };
+    try {
+      ck(ctx, nk_alloc_uninit(ctx, gbytes, &dI));
+      ck(ctx, nk_alloc_uninit(ctx, sbytes, &dh_rec));
+      const void* dY = grad_or_null(gradient);
+      const float* gi = reinterpret_cast<const float*>(fw->gi->rptr());
+      if (lstm) {
+        dH = dI;   // one gate gradient for both products
+        ck(ctx, nk_alloc_uninit(ctx, sbytes, &dc));
+        if (const void* dcT = grad_or_null(c_last_grad))
+          ck(ctx, nk_cast(ctx, dc, NK_F32, dcT, c_last_grad->dtype, size_t(NH)));
+        else
+          ck(ctx, nk_memset0(ctx, dc, sbytes));
+      } else {
+        ck(ctx, nk_alloc_uninit(ctx, gbytes, &dH));
+        ck(ctx, nk_memset0(ctx, dh_rec, sbytes));
+      }
+      for (int64_t t = T - 1; t >= 0; --t) {
+        const void* dY_t = dY ? at(dY, t * NH, gradient->dtype) : nullptr;
+        const bool send_back = t > 0 || d.h;   // somebody reads the gradient of the state before step t
+        if (lstm) {
+          ck(ctx, nk_lstm_seq_bwd_step(ctx, at(dI, t * NG, dt), dt, static_cast<float*>(dc), gi + t * NG,
+                                       fw->c_prev(t, NH), dY_t, t == T - 1 ? nullptr : static_cast<const float*>(dh_rec),
+                                       N, H, dt));
+          if (send_back) gemm(ctx, false, false, N, H, G, at(dH, t * NG, dt), G, o.w_hh->rptr(), H, 0.f, dh_rec, dt, NK_F32);
+        } else {
+          const float* gh = reinterpret_cast<const float*>(fw->gh->rptr());
+          ck(ctx, nk_gru_seq_bwd_step(ctx, at(dI, t * NG, dt), at(dH, t * NG, dt), dt, static_cast<float*>(dh_rec),
+                                      gi + t * NG, gh + t * NG, fw->h_prev(t, NH), dY_t, N, H, dt));
+          if (send_back) gemm(ctx, false, false, N, H, G, at(dH, t * NG, dt), G, o.w_hh->rptr(), H, 1.f, dh_rec, dt, NK_F32);
+        }
+      }
+      // the parameters first (their data-parallel exchange can then overlap the rest), as the cell does.  Each weight
+      // gradient is written by this node alone, so its hook and its reduce-scatter report fire once, after the last GEMM
+      if (d.w_hh) {   // dW_hh += dG[1:]^T.output[:T-1] + dG[0]^T.hidden (TN)
+        accumulate(ctx, d.w_hh, [&](void* p, float beta) {
+          if (T > 1)
+            gemm(ctx, true, false, G, H, (T - 1) * N, at(dH, NG, dt), G, fw->out->rptr(), H, beta, p, dt, d.w_hh->dtype);
+          gemm(ctx, true, false, G, H, N, dH, G, o.h->rptr(), H, T > 1 ? 1.f : beta, p, dt, d.w_hh->dtype);
+        });
+        weight_done(d.w_hh);
+      }
+      if (d.w_ih) {   // dW_ih += dG^T.X (TN, K = T*N)
+        accumulate(ctx, d.w_ih, [&](void* p, float beta) {
+          gemm(ctx, true, false, G, I, T * N, dI, G, o.x->rptr(), I, beta, p, dt, d.w_ih->dtype);
+        });
+        weight_done(d.w_ih);
+      }
+      bias(d.b_ih, dI, G, T * N, dt);
+      bias(d.b_hh, dH, G, T * N, dt);
+      if (d.x) {      // dX += dG.W_ih (NN over T*N rows)
+        accumulate(ctx, d.x, [&](void* p, float beta) {
+          gemm(ctx, false, false, T * N, I, G, dI, G, o.w_ih->rptr(), I, beta, p, dt, d.x->dtype);
+        });
+        grad_written(d.x);
+      }
+      state(d.h, static_cast<const float*>(dh_rec), N, H);
+      state(d.c, static_cast<const float*>(dc), N, H);
+    } catch (...) {
+      release();
+      throw;
+    }
+    ck(ctx, nk_free(ctx, dc));
+    ck(ctx, nk_free(ctx, dh_rec));
+    if (dH != dI) ck(ctx, nk_free(ctx, dH));
+    ck(ctx, nk_free(ctx, dI));
+  }
+  void no_grad() override {
+    Backward::no_grad();
+    if (c_last_grad) c_last_grad->no_grad();
+  }
+  void with_grad() override {
+    Backward::with_grad();
+    if (c_last_grad) c_last_grad->with_grad();
   }
 };
 
@@ -2095,7 +2271,7 @@ int nkg_convolution_nd(nkg_var* kernel, nkg_var* input, int nsp, const int64_t* 
   });
 }
 
-// ---------------------------------------------------------------- chunks / recurrent cells
+// ---------------------------------------------------------------- chunks / recurrent cells / sequence layers
 int nkg_chunks(nkg_var* a, int ndim, const int64_t* chunk_shape, int capacity, nkg_var** outs, int* count) {
   return guard([&] {
     if (!a || !chunk_shape || !count || (capacity > 0 && !outs)) fail(NK_ERR_INVALID_ARG, "chunks: NULL");
@@ -2202,9 +2378,14 @@ int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out) {
   });
 }
 
-static void cell_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih,
-                      nkg_var* b_hh, nkg_var** new_c, nkg_var** new_h) {
-  const char* who = lstm ? "lstm_cell" : "gru_cell";
+// The operand checks of a cell step (`seq` false: input (N, I)) and of a sequence layer (`seq` true: input (T, N, I),
+// T >= 1).  Returns the operands in History::merge order.
+struct RnnDims {
+  int64_t T, N, I, H;
+};
+static std::vector<nkg_var*> check_rnn_operands(const char* who, bool lstm, bool seq, nkg_var* x, nkg_var* c, nkg_var* h,
+                                                nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih, nkg_var* b_hh,
+                                                bool outputs_given, RnnDims& dims) {
   struct Arg {
     nkg_var* v;
     const char* name;
@@ -2214,7 +2395,7 @@ static void cell_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_
   if (lstm) args.push_back({c, "cell_state"});
   for (const Arg& a : args)
     if (!a.v) fail(NK_ERR_INVALID_ARG, "%s: %s is NULL", who, a.name);
-  if (!new_h || (lstm && !new_c)) fail(NK_ERR_INVALID_ARG, "%s: NULL output", who);
+  if (!outputs_given) fail(NK_ERR_INVALID_ARG, "%s: NULL output", who);
   for (const Arg& a : args) {
     if (a.v->data->dtype != x->data->dtype)
       fail(NK_ERR_INVALID_ARG, "%s: %s has another element type than the input", who, a.name);
@@ -2227,12 +2408,16 @@ static void cell_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_
     return out + (s.size() == 1 ? ",)" : ")");
   };
   const Shape& xs = x->data->shape;
-  if (xs.size() != 2) fail(NK_ERR_INVALID_ARG, "%s: input must be (batch, input_size), got %s", who, shape_str(xs).c_str());
+  if (xs.size() != (seq ? 3u : 2u))
+    fail(NK_ERR_INVALID_ARG, "%s: input must be %s, got %s", who, seq ? "(seq_len, batch, input_size)" : "(batch, input_size)",
+         shape_str(xs).c_str());
+  if (seq && xs[0] < 1) fail(NK_ERR_INVALID_ARG, "%s: input needs at least one time step, got %s", who, shape_str(xs).c_str());
   const Shape& hs = h->data->shape;
-  if (hs.size() != 2 || hs[0] != xs[0])
-    fail(NK_ERR_INVALID_ARG, "%s: hidden must be (batch = %lld, hidden_size), got %s", who, (long long)xs[0],
+  const int64_t N = xs[seq ? 1 : 0], I = xs[seq ? 2 : 1];
+  if (hs.size() != 2 || hs[0] != N)
+    fail(NK_ERR_INVALID_ARG, "%s: hidden must be (batch = %lld, hidden_size), got %s", who, (long long)N,
          shape_str(hs).c_str());
-  const int64_t N = xs[0], I = xs[1], H = hs[1];
+  const int64_t H = hs[1];
   auto expect = [&](nkg_var* v, const char* name, const Shape& want) {
     if (v->data->shape != want)
       fail(NK_ERR_INVALID_ARG, "%s: %s must be %s, got %s", who, name, shape_str(want).c_str(),
@@ -2243,9 +2428,19 @@ static void cell_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_
   expect(w_hh, "weight_hh", {G * H, H});
   expect(b_ih, "bias_ih", {G * H});
   expect(b_hh, "bias_hh", {G * H});
-
+  dims = {seq ? xs[0] : 1, N, I, H};
   std::vector<nkg_var*> operands;   // History::merge over every operand
   for (const Arg& a : args) operands.push_back(a.v);
+  return operands;
+}
+
+static void cell_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih,
+                      nkg_var* b_hh, nkg_var** new_c, nkg_var** new_h) {
+  const char* who = lstm ? "lstm_cell" : "gru_cell";
+  RnnDims dm;
+  const std::vector<nkg_var*> operands =
+      check_rnn_operands(who, lstm, false, x, c, h, w_ih, w_hh, b_ih, b_hh, new_h && (!lstm || new_c), dm);
+  const int64_t N = dm.N, H = dm.H;
   std::shared_ptr<RnnCell> cell;
   std::shared_ptr<RnnCellBackward> cell_bwd;
   nkg_var* vh = record(
@@ -2281,6 +2476,49 @@ int nkg_lstm_cell(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var*
 int nkg_gru_cell(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
                  nkg_var* bias_hh, nkg_var** new_hidden) {
   return guard([&] { cell_impl(false, input, nullptr, hidden, weight_ih, weight_hh, bias_ih, bias_hh, nullptr, new_hidden); });
+}
+
+static void seq_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih,
+                     nkg_var* b_hh, nkg_var** output, nkg_var** last_c) {
+  const char* who = lstm ? "lstm" : "gru";
+  RnnDims dm;
+  const std::vector<nkg_var*> operands =
+      check_rnn_operands(who, lstm, true, x, c, h, w_ih, w_hh, b_ih, b_hh, output && (!lstm || last_c), dm);
+  std::shared_ptr<RnnSeq> seq;
+  std::shared_ptr<RnnSeqBackward> seq_bwd;
+  nkg_var* vy = record(
+      operands, Shape{dm.T, dm.N, dm.H}, x->data->dtype,
+      [&](const TensorP& d) {
+        seq = std::make_shared<RnnSeq>(
+            x->ctx, lstm, CellOperands{x->data, h->data, lstm ? c->data : nullptr, w_ih->data, w_hh->data, b_ih->data, b_hh->data},
+            d);
+        return seq;
+      },
+      [&](const TensorP&, const GradientP& g) {
+        seq_bwd = std::make_shared<RnnSeqBackward>(
+            x->ctx, g, seq,
+            CellGrads{x->grad, h->grad, lstm ? c->grad : nullptr, w_ih->grad, w_hh->grad, b_ih->grad, b_hh->grad});
+        return seq_bwd;
+      });
+  if (lstm) {   // the second output: same tapes, same op id (merging the two histories keeps one node)
+    nkg_var* vc = new nkg_var(*vy);
+    vc->data = seq->c_last;
+    if (seq_bwd) vc->grad = seq_bwd->c_last_grad;
+    *last_c = vc;
+  }
+  *output = vy;
+}
+
+int nkg_lstm(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
+             nkg_var* bias_hh, nkg_var** output, nkg_var** last_cell_state) {
+  return guard([&] {
+    seq_impl(true, input, cell_state, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, last_cell_state);
+  });
+}
+
+int nkg_gru(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih, nkg_var* bias_hh,
+            nkg_var** output) {
+  return guard([&] { seq_impl(false, input, nullptr, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, nullptr); });
 }
 
 // ---------------------------------------------------------------- optimizers on a leaf (neuronika-optim)

@@ -9,6 +9,10 @@
 // those of nk_pointwise.cu (1/(1+expf(-x)), tanhf), so the fused cell and the cell composed from primitives differ only
 // by the composed graph's rounded intermediates.  Saturated or infinite pre-activations give 0 / 1 / +-1, never NaN.
 // The backward recomputes the activations (and c') from the f32 gates instead of keeping them.
+//   sequence steps           nk_lstm_seq_bwd_step / nk_gru_seq_bwd_step: the same gate gradients for one time step of the
+//                            LSTM / GRU sequence node (nk_graph.cpp, RnnSeqBackward).  The gradient carried from step to
+//                            step (dc, and the recurrent part of dh) stays in f32 whatever the element type and is updated
+//                            in place, so a bf16 sequence rounds it once at the end instead of once per step.
 #include "nk_internal.cuh"
 
 // a named namespace: the kernels keep the same symbol names from build to build (profiler traces, torch.profiler)
@@ -142,6 +146,51 @@ __global__ void __launch_bounds__(kThreads) nk_lstm_cell_bwd_kernel(TG* __restri
   }
 }
 
+// One backward time step of the LSTM sequence node.  dh = dh_out (this step's slice of the output gradient, element type
+// T) + dh_rec (f32, what came back through h.W_hh^T from step t+1); either may be NULL = zero.  dc is the running f32
+// cell-state gradient: read as dc_out, overwritten with dc_prev = f*dc_total.
+template <typename T, typename TG, int V>
+__global__ void __launch_bounds__(kThreads) nk_lstm_seq_bwd_step_kernel(TG* __restrict__ dgates, float* __restrict__ dc,
+                                                                        const float* __restrict__ gates,
+                                                                        const T* __restrict__ c_prev,
+                                                                        const T* __restrict__ dh_out,
+                                                                        const float* __restrict__ dh_rec, int64_t n,
+                                                                        int64_t H) {
+  const int64_t per_row = H / V;
+  const size_t units = size_t(n) * size_t(per_row);
+  const size_t stride = size_t(gridDim.x) * blockDim.x;
+  for (size_t u = size_t(blockIdx.x) * blockDim.x + threadIdx.x; u < units; u += stride) {
+    const int64_t row = int64_t(u / size_t(per_row)), j = int64_t(u % size_t(per_row)) * V;
+    const int64_t gs = row * 4 * H + j, ss = row * H + j;
+    float gi[V], gf[V], gg[V], go[V], c[V], dh[V], dr[V], dcr[V];
+    ldv<float, V>(gi, gates + gs);
+    ldv<float, V>(gf, gates + gs + H);
+    ldv<float, V>(gg, gates + gs + 2 * H);
+    ldv<float, V>(go, gates + gs + 3 * H);
+    ldv<T, V>(c, c_prev + ss);
+    ldv<float, V>(dcr, dc + ss);
+    if (dh_out) ldv<T, V>(dh, dh_out + ss);
+    if (dh_rec) ldv<float, V>(dr, dh_rec + ss);
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+      const float i = sigm(gi[k]), f = sigm(gf[k]), g = tanhf(gg[k]), o = sigm(go[k]);
+      const float tc = tanhf(f * c[k] + i * g);
+      const float dhk = (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f);
+      const float dct = dcr[k] + dhk * o * (1.f - tc * tc);
+      gi[k] = dct * g * i * (1.f - i);
+      gf[k] = dct * c[k] * f * (1.f - f);
+      gg[k] = dct * i * (1.f - g * g);
+      go[k] = dhk * tc * o * (1.f - o);
+      dcr[k] = f * dct;
+    }
+    stv<TG, V>(dgates + gs, gi);
+    stv<TG, V>(dgates + gs + H, gf);
+    stv<TG, V>(dgates + gs + 2 * H, gg);
+    stv<TG, V>(dgates + gs + 3 * H, go);
+    stv<float, V>(dc + ss, dcr);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------- GRU
 // igates = x.W_ih^T + b_ih, hgates = h.W_hh^T + b_hh, (n, 3H) f32 each, chunks [r | z | n]
 template <typename T, int V>
@@ -219,6 +268,57 @@ __global__ void __launch_bounds__(kThreads) nk_gru_cell_bwd_kernel(TG* __restric
     stv<TG, V>(dhgates + gs + H, iz);
     stv<TG, V>(dhgates + gs + 2 * H, hn);
     if (dh_prev) stv<T, V>(dh_prev + ss, dhp);
+  }
+}
+
+// One backward time step of the GRU sequence node.  dh = dh_out (element type T, NULL = zero) + dh_rec (f32).  dh_rec is
+// the running hidden-state gradient: read, then overwritten with the pointwise part z*dh of the previous step's gradient
+// (the caller adds dhgates.W_hh to it).  dh_rec may be NULL when nothing is carried (a single step whose hidden state is
+// not differentiable).
+template <typename T, typename TG, int V>
+__global__ void __launch_bounds__(kThreads) nk_gru_seq_bwd_step_kernel(TG* __restrict__ digates, TG* __restrict__ dhgates,
+                                                                       float* __restrict__ dh_rec,
+                                                                       const float* __restrict__ igates,
+                                                                       const float* __restrict__ hgates,
+                                                                       const T* __restrict__ h_prev,
+                                                                       const T* __restrict__ dh_out, int64_t n, int64_t H) {
+  const int64_t per_row = H / V;
+  const size_t units = size_t(n) * size_t(per_row);
+  const size_t stride = size_t(gridDim.x) * blockDim.x;
+  for (size_t u = size_t(blockIdx.x) * blockDim.x + threadIdx.x; u < units; u += stride) {
+    const int64_t row = int64_t(u / size_t(per_row)), j = int64_t(u % size_t(per_row)) * V;
+    const int64_t gs = row * 3 * H + j, ss = row * H + j;
+    float ir[V], iz[V], in[V], hr[V], hz[V], hn[V], h[V], dh[V], dr[V];
+    ldv<float, V>(ir, igates + gs);
+    ldv<float, V>(iz, igates + gs + H);
+    ldv<float, V>(in, igates + gs + 2 * H);
+    ldv<float, V>(hr, hgates + gs);
+    ldv<float, V>(hz, hgates + gs + H);
+    ldv<float, V>(hn, hgates + gs + 2 * H);
+    ldv<T, V>(h, h_prev + ss);
+    if (dh_out) ldv<T, V>(dh, dh_out + ss);
+    if (dh_rec) ldv<float, V>(dr, dh_rec + ss);
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+      const float r = sigm(ir[k] + hr[k]), z = sigm(iz[k] + hz[k]);
+      const float nn = tanhf(in[k] + r * hn[k]);
+      const float dhk = (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f);
+      const float dpn = dhk * (1.f - z) * (1.f - nn * nn);
+      const float dpz = dhk * (h[k] - nn) * z * (1.f - z);
+      const float dpr = dpn * hn[k] * r * (1.f - r);
+      ir[k] = dpr;           // d(i_r) = d(h_r)
+      iz[k] = dpz;           // d(i_z) = d(h_z)
+      in[k] = dpn;           // d(i_n)
+      hn[k] = dpn * r;       // d(h_n)
+      dr[k] = z * dhk;
+    }
+    stv<TG, V>(digates + gs, ir);
+    stv<TG, V>(digates + gs + H, iz);
+    stv<TG, V>(digates + gs + 2 * H, in);
+    stv<TG, V>(dhgates + gs, ir);
+    stv<TG, V>(dhgates + gs + H, iz);
+    stv<TG, V>(dhgates + gs + 2 * H, hn);
+    if (dh_rec) stv<float, V>(dh_rec + ss, dr);
   }
 }
 
@@ -397,6 +497,58 @@ int nk_gru_cell_bwd(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, voi
     });
   });
   NK_LAUNCHED(ctx, "gru_cell_bwd");
+  return NK_OK;
+}
+
+int nk_lstm_seq_bwd_step(nk_ctx* ctx, void* dgates, int dgates_dtype, float* dc, const float* gates, const void* c_prev,
+                         const void* dh_out, const float* dh_rec, int64_t n, int64_t hidden, int dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  if (int rc = cell_args(ctx, "nk_lstm_seq_bwd_step", n, hidden, dtype)) return rc;
+  NK_REQUIRE(ctx, nk_dtype_ok(dgates_dtype), "nk_lstm_seq_bwd_step: bad dgates dtype %d", dgates_dtype);
+  if (n == 0 || hidden == 0) return NK_OK;
+  NK_REQUIRE(ctx, dgates && dc && gates && c_prev, "nk_lstm_seq_bwd_step: NULL pointer");
+  const bool al = aligned16(dgates) && aligned16(dc) && aligned16(gates) && aligned16(c_prev) &&
+                  (!dh_out || aligned16(dh_out)) && (!dh_rec || aligned16(dh_rec));
+  NK_DISPATCH_DTYPE(dtype, T, {
+    NK_DISPATCH_DTYPE(dgates_dtype, TG, {
+      constexpr int V = NkVec<T>::N;
+      const bool vec = al && hidden % V == 0;
+      const int64_t units = n * (vec ? hidden / V : hidden);
+      if (vec)
+        nk_lstm_seq_bwd_step_kernel<T, TG, V><<<rnn_blocks(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)dgates, dc, gates, (const T*)c_prev, (const T*)dh_out, dh_rec, n, hidden);
+      else
+        nk_lstm_seq_bwd_step_kernel<T, TG, 1><<<rnn_blocks(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)dgates, dc, gates, (const T*)c_prev, (const T*)dh_out, dh_rec, n, hidden);
+    });
+  });
+  NK_LAUNCHED(ctx, "lstm_seq_bwd_step");
+  return NK_OK;
+}
+
+int nk_gru_seq_bwd_step(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, float* dh_rec, const float* igates,
+                        const float* hgates, const void* h_prev, const void* dh_out, int64_t n, int64_t hidden, int dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  if (int rc = cell_args(ctx, "nk_gru_seq_bwd_step", n, hidden, dtype)) return rc;
+  NK_REQUIRE(ctx, nk_dtype_ok(dg_dtype), "nk_gru_seq_bwd_step: bad dgates dtype %d", dg_dtype);
+  if (n == 0 || hidden == 0) return NK_OK;
+  NK_REQUIRE(ctx, digates && dhgates && igates && hgates && h_prev, "nk_gru_seq_bwd_step: NULL pointer");
+  const bool al = aligned16(digates) && aligned16(dhgates) && aligned16(igates) && aligned16(hgates) &&
+                  aligned16(h_prev) && (!dh_out || aligned16(dh_out)) && (!dh_rec || aligned16(dh_rec));
+  NK_DISPATCH_DTYPE(dtype, T, {
+    NK_DISPATCH_DTYPE(dg_dtype, TG, {
+      constexpr int V = NkVec<T>::N;
+      const bool vec = al && hidden % V == 0;
+      const int64_t units = n * (vec ? hidden / V : hidden);
+      if (vec)
+        nk_gru_seq_bwd_step_kernel<T, TG, V><<<rnn_blocks(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)digates, (TG*)dhgates, dh_rec, igates, hgates, (const T*)h_prev, (const T*)dh_out, n, hidden);
+      else
+        nk_gru_seq_bwd_step_kernel<T, TG, 1><<<rnn_blocks(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)digates, (TG*)dhgates, dh_rec, igates, hgates, (const T*)h_prev, (const T*)dh_out, n, hidden);
+    });
+  });
+  NK_LAUNCHED(ctx, "gru_seq_bwd_step");
   return NK_OK;
 }
 

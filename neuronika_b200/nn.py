@@ -1,4 +1,5 @@
-"""Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell and Conv2d (neuronika-nn/src/lib.rs:406-626, 724-815)."""
+"""Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell and Conv2d (neuronika-nn/src/lib.rs:406-626, 724-815),
+and the sequence layers LSTM and GRU over them."""
 from __future__ import annotations
 
 import math
@@ -95,6 +96,19 @@ class LSTMCell:
         return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]
 
 
+class LSTM(LSTMCell):
+    """The LSTMCell applied to a whole time-major sequence as one graph node (variable.lstm): same parameters and
+    initialisation as the cell, so a layer built from the same `rng` seed holds the same weights.  One layer, one
+    direction."""
+
+    def forward(self, state, input: V.Var):
+        """`state = (cell_state, hidden)`, both (batch, hidden_size); `input` (seq_len, batch, input_size).  Returns
+        (output, cell_T): every step's hidden state (seq_len, batch, hidden_size), whose last slice is the last hidden
+        state, and the last cell state."""
+        cell_state, hidden = state
+        return V.lstm(input, cell_state, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+
+
 class Dropout:
     """Dropout with probability p and a status of its own: `train()` (the initial mode) draws a new mask on every
     forward() of the graph, `eval()` passes the input through.  The reference's docs name `nn::Dropout`; its crate
@@ -139,3 +153,13 @@ class GRUCell:
 
     def parameters(self):
         return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]
+
+
+class GRU(GRUCell):
+    """The GRUCell applied to a whole time-major sequence as one graph node (variable.gru): same parameters and
+    initialisation as the cell.  One layer, one direction."""
+
+    def forward(self, hidden: V.Var, input: V.Var):
+        """`hidden` (batch, hidden_size), `input` (seq_len, batch, input_size); returns every step's hidden state
+        (seq_len, batch, hidden_size)."""
+        return V.gru(input, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)

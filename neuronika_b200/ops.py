@@ -446,6 +446,32 @@ def gru_cell_bwd(digates: CuArray, dhgates: CuArray, igates: CuArray, hgates: Cu
     return digates, dhgates
 
 
+def lstm_seq_bwd_step(dgates: CuArray, dc: CuArray, gates: CuArray, c_prev: CuArray, dh_out: CuArray | None,
+                      dh_rec: CuArray | None) -> CuArray:
+    """One backward time step of the LSTM sequence node: dgates (overwritten) from dh = dh_out + dh_rec (None = zero;
+    dh_rec f32) and the running f32 cell-state gradient dc, which is replaced by sigmoid(f)*dc_total."""
+    n, hidden = c_prev.shape
+    if dc.dtype != F32 or (dh_rec is not None and dh_rec.dtype != F32):
+        raise ValueError("lstm_seq_bwd_step: dc and dh_rec are f32")
+    _ck(lib.nk_lstm_seq_bwd_step(c_prev.device.ctx, dgates.ptr, dgates.dtype, dc.ptr, gates.ptr, c_prev.ptr, _ptr(dh_out),
+                                 _ptr(dh_rec), n, hidden, c_prev.dtype), c_prev.device)
+    return dgates
+
+
+def gru_seq_bwd_step(digates: CuArray, dhgates: CuArray, dh_rec: CuArray | None, igates: CuArray, hgates: CuArray,
+                     h_prev: CuArray, dh_out: CuArray | None):
+    """One backward time step of the GRU sequence node: digates, dhgates (overwritten) from dh = dh_out + dh_rec (None =
+    zero); the f32 dh_rec is replaced by z*dh.  Returns (digates, dhgates)."""
+    n, hidden = h_prev.shape
+    if digates.dtype != dhgates.dtype:
+        raise ValueError("gru_seq_bwd_step: digates and dhgates must have one element type")
+    if dh_rec is not None and dh_rec.dtype != F32:
+        raise ValueError("gru_seq_bwd_step: dh_rec is f32")
+    _ck(lib.nk_gru_seq_bwd_step(h_prev.device.ctx, digates.ptr, dhgates.ptr, digates.dtype, _ptr(dh_rec), igates.ptr,
+                                hgates.ptr, h_prev.ptr, _ptr(dh_out), n, hidden, h_prev.dtype), h_prev.device)
+    return digates, dhgates
+
+
 def chunk(x: CuArray, chunk_shape, index: int, out: CuArray | None = None) -> CuArray:
     """Block `index` of x's exact_chunks(chunk_shape) (row-major block order), bit exact."""
     cs = tuple(int(c) for c in chunk_shape)

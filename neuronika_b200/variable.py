@@ -81,6 +81,8 @@ _G = {
     "nkg_chunks": (i32, [vp, i32, pi64, i32, pvp, C.POINTER(i32)]),
     "nkg_lstm_cell": (i32, [vp, vp, vp, vp, vp, vp, vp, pvp, pvp]),
     "nkg_gru_cell": (i32, [vp, vp, vp, vp, vp, vp, pvp]),
+    "nkg_lstm": (i32, [vp, vp, vp, vp, vp, vp, vp, pvp, pvp]),
+    "nkg_gru": (i32, [vp, vp, vp, vp, vp, vp, pvp]),
     "nkg_cat": (i32, [pvp, i32, i32, pvp]),
     "nkg_stack": (i32, [pvp, i32, i32, pvp]),
     "nkg_unsqueeze": (i32, [vp, i32, pvp]),
@@ -433,6 +435,25 @@ def gru_cell(input: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: V
     h = vp()
     _ck(lib.nkg_gru_cell(input._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h, C.byref(h)))
     return input._wrap(h)
+
+
+# ---- recurrent sequence layers (one node per sequence; see include/nk_graph.h)
+def lstm(input: Var, cell_state: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: Var, bias_hh: Var):
+    """An LSTM over a whole time-major sequence, as ONE node: `input` (T, N, I), `cell_state` and `hidden` (N, H), the
+    weights as `lstm_cell` takes them.  Returns (output, cell_T): `output` (T, N, H) holds every step's hidden state and
+    `cell_T` (N, H) the last cell state.  The last hidden state is `output[T-1]`; it is not a third result."""
+    y, c = vp(), vp()
+    _ck(lib.nkg_lstm(input._h, cell_state._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h,
+                     C.byref(y), C.byref(c)))
+    return input._wrap(y), input._wrap(c)
+
+
+def gru(input: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: Var, bias_hh: Var):
+    """A GRU over a whole time-major sequence, as ONE node: `input` (T, N, I), `hidden` (N, H), the weights as `gru_cell`
+    takes them.  Returns `output` (T, N, H), every step's hidden state; the last one is `output[T-1]`."""
+    y = vp()
+    _ck(lib.nkg_gru(input._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h, C.byref(y)))
+    return input._wrap(y)
 
 
 # ---- constructors (neuronika-variable/src/lib.rs:51-240), on a device

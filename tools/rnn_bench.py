@@ -1,9 +1,11 @@
 #!/usr/bin/env python
 """LSTM / GRU training-step benchmark (development tool; bench.py measures the flagship workload).
 
-Workload: an unrolled sequence of T = 32 steps, bf16 parameters with f32 gradients, the input a `Var`, h0 = c0 = 0, the
-loss the mse of h_T against a seeded target.  One step is zero_grad -> forward -> backward -> SGD, captured once with
-Device.capture and replayed.  Shapes (N, I, H) = (256, 1024, 1024) and (1024, 2048, 2048), LSTM and GRU.
+Workload: a sequence of T = 32 steps, bf16 parameters with f32 gradients, the input a `Var`, h0 = c0 = 0, the loss the
+mse of h_T against a seeded target.  One step is zero_grad -> forward -> backward -> SGD, captured once with
+Device.capture and replayed.  Shapes (N, I, H) = (256, 1024, 1024) and (1024, 2048, 2048), LSTM and GRU.  Three variants
+of the same computation: "fused" unrolls nn.LSTMCell / nn.GRUCell (one node per time step), "composed" unrolls the cell
+written with primitives, "sequence" is nn.LSTM / nn.GRU (one node for the whole sequence).
 
 Reported per configuration, in one JSON line each:
   - ms per sequence and per time step, and kernel launches per time step (the captured graph's kernel count / T);
@@ -13,7 +15,11 @@ Reported per configuration, in one JSON line each:
     each must move (f32 gates, bf16 states / gradients) counted from the shapes;
   - in the same process and alternating with it: the same cell composed from primitives through the graph API
     (chunks + sigmoid / tanh + mul / add, intended gate assignment), also captured and replayed, and
-    torch.nn.LSTMCell / GRUCell in bf16 on the same GPU in an eager loop ("torch_eager_bf16").
+    torch.nn.LSTMCell / GRUCell in bf16 on the same GPU in an eager loop ("torch_eager_bf16") and torch.nn.LSTM / GRU
+    (cuDNN) in bf16 on the whole sequence ("torch_cudnn_bf16");
+  - the sequence layer's GEMMs alone, in two groups: the products that run once over all T*N rows (x.W_ih^T + b, dW_ih,
+    dW_hh) and the 2T sequential ones that stay N rows tall (h.W_hh^T + b forward, dG.W_hh backward), as ms per sequence
+    and as shares of the sequence layer's step.
 Card name, power limit and the median SM clock during the timed windows (NVML) are printed beside the numbers.
 
     python tools/rnn_bench.py [--reps 5] [--window-ms 200]
@@ -77,11 +83,15 @@ def composed_cell(kind, cell, state, x, n, hidden):
     return (state - nn) * z + nn
 
 
-def graph_step(nk, dev, kind, n, n_in, hidden, composed):
-    """(captured step, kernels per replay)"""
+def graph_step(nk, dev, kind, n, n_in, hidden, variant):
+    """the captured step of one variant ("fused", "composed" or "sequence")"""
     from neuronika_b200 import optim
     rng = np.random.default_rng(0)
-    cls = nk.nn.LSTMCell if kind == "lstm" else nk.nn.GRUCell
+    composed, sequence = variant == "composed", variant == "sequence"
+    if sequence:
+        cls = nk.nn.LSTM if kind == "lstm" else nk.nn.GRU
+    else:
+        cls = nk.nn.LSTMCell if kind == "lstm" else nk.nn.GRUCell
     cell = cls(dev, n_in, hidden, nk.BF16, grad_dtype=nk.F32, rng=rng)
     opt = optim.StochasticGD.new(1e-3)
     for p in cell.parameters():
@@ -89,13 +99,21 @@ def graph_step(nk, dev, kind, n, n_in, hidden, composed):
     xs = [nk.from_ndarray(dev, rng.uniform(-1, 1, (n, n_in)).astype(np.float32), nk.BF16) for _ in range(T)]
     zero = nk.zeros(dev, (n, hidden), nk.BF16)
     tgt = nk.from_ndarray(dev, rng.uniform(-0.5, 0.5, (n, hidden)).astype(np.float32), nk.BF16)
+    if sequence:
+        x_seq = nk.from_ndarray(dev, np.stack([x.data() for x in xs]), nk.BF16)
+        tgt_seq = nk.from_ndarray(dev, tgt.data().reshape(1, n, hidden), nk.BF16)
 
     def step():
         opt.zero_grad()
         state = (zero, zero) if kind == "lstm" else zero
-        for x in xs:
-            state = composed_cell(kind, cell, state, x, n, hidden) if composed else cell.forward(state, x)
-        loss = (state[1] if kind == "lstm" else state).mse_loss(tgt)
+        if sequence:
+            out = cell.forward(state, x_seq)
+            h_last = (out[0] if kind == "lstm" else out).chunks((1, n, hidden))[T - 1]      # output[T-1] is h_T
+            loss = h_last.mse_loss(tgt_seq)
+        else:
+            for x in xs:
+                state = composed_cell(kind, cell, state, x, n, hidden) if composed else cell.forward(state, x)
+            loss = (state[1] if kind == "lstm" else state).mse_loss(tgt)
         loss.forward()
         loss.backward(1.0)
         opt.step()
@@ -125,6 +143,46 @@ def torch_step(torch, kind, n, n_in, hidden):
         torch.nn.functional.mse_loss(h, tgt).backward()
         opt.step()
     return step
+
+
+def torch_cudnn_step(torch, kind, n, n_in, hidden):
+    g = torch.Generator(device="cuda").manual_seed(0)
+    layer = (torch.nn.LSTM if kind == "lstm" else torch.nn.GRU)(n_in, hidden).cuda().to(torch.bfloat16)
+    opt = torch.optim.SGD(layer.parameters(), lr=1e-3)
+    x = (torch.rand(T, n, n_in, device="cuda", generator=g) * 2 - 1).to(torch.bfloat16)
+    tgt = (torch.rand(n, hidden, device="cuda", generator=g) - 0.5).to(torch.bfloat16)
+    zero = torch.zeros(1, n, hidden, device="cuda", dtype=torch.bfloat16)
+
+    def step():
+        opt.zero_grad(set_to_none=False)
+        out, _ = layer(x, (zero, zero) if kind == "lstm" else zero)
+        torch.nn.functional.mse_loss(out[-1], tgt).backward()
+        opt.step()
+    return step
+
+
+def sequence_gemms(nk, dev, kind, n, n_in, hidden):
+    """the sequence layer's products of one training step in two groups: (whole-sequence fn, sequential fn)"""
+    from neuronika_b200 import ops
+    G = (4 if kind == "lstm" else 3) * hidden
+    r = lambda *s: dev.from_ndarray(np.random.default_rng(1).uniform(-1, 1, s).astype(np.float32), nk.BF16)
+    x, hs, h, w_ih, w_hh, b = r(T * n, n_in), r((T - 1) * n, hidden), r(n, hidden), r(G, n_in), r(G, hidden), r(G)
+    gates, dg = dev.zeros((T * n, G), nk.F32), r(T * n, G)
+    gates_t, dg_t, dg_rest = gates.slice_flat(0, (n, G)), dg.slice_flat(0, (n, G)), dg.slice_flat(n * G, ((T - 1) * n, G))
+    dw_ih, dw_hh, dh = dev.zeros((G, n_in), nk.F32), dev.zeros((G, hidden), nk.F32), dev.zeros((n, hidden), nk.F32)
+
+    def whole():
+        ops.gemm(x, w_ih, gates, trans_b=True, bias=b)
+        ops.gemm(dg_rest, hs, dw_hh, trans_a=True)
+        ops.gemm(dg_t, h, dw_hh, trans_a=True, beta=1.0)
+        ops.gemm(dg, x, dw_ih, trans_a=True)
+
+    def sequential():
+        for _ in range(T):
+            ops.gemm(h, w_hh, gates_t, trans_b=True, bias=b, beta=1.0)
+        for _ in range(T):
+            ops.gemm(dg_t, w_hh, dh)
+    return whole, sequential
 
 
 def gemm_only(nk, dev, torch, kind, n, n_in, hidden):
@@ -188,18 +246,24 @@ def main():
     print(json.dumps({"card": card, "sm_count": dev.sm_count, "T": T}), flush=True)
     for kind in ("lstm", "gru"):
         for n, n_in, hidden in SHAPES:
-            fused = graph_step(nk, dev, kind, n, n_in, hidden, composed=False)
-            comp = graph_step(nk, dev, kind, n, n_in, hidden, composed=True)
+            fused = graph_step(nk, dev, kind, n, n_in, hidden, "fused")
+            comp = graph_step(nk, dev, kind, n, n_in, hidden, "composed")
+            seq = graph_step(nk, dev, kind, n, n_in, hidden, "sequence")
             teager = torch_step(torch, kind, n, n_in, hidden)
-            res = {"fused": [], "composed": [], "torch_eager_bf16": []}
+            tcudnn = torch_cudnn_step(torch, kind, n, n_in, hidden)
+            res = {"fused": [], "composed": [], "sequence": [], "torch_eager_bf16": [], "torch_cudnn_bf16": []}
             mhz = []
             for _ in range(args.reps):      # alternating, one window each
-                for name, fn in (("fused", fused.launch), ("composed", comp.launch), ("torch_eager_bf16", teager)):
+                for name, fn in (("fused", fused.launch), ("composed", comp.launch), ("sequence", seq.launch),
+                                 ("torch_eager_bf16", teager), ("torch_cudnn_bf16", tcudnn)):
                     ms, m = timed(torch, fn, clock, args.window_ms, 1)
                     res[name].append(ms)
                     mhz.append(m)
             gem, flops = gemm_only(nk, dev, torch, kind, n, n_in, hidden)
             gms, _ = timed(torch, gem, clock, args.window_ms / 4, args.reps)
+            whole, sequential = sequence_gemms(nk, dev, kind, n, n_in, hidden)
+            wms, _ = timed(torch, whole, clock, args.window_ms / 4, args.reps)
+            sms, _ = timed(torch, sequential, clock, args.window_ms / 4, args.reps)
             fwd, fb, bwd, bb = gate_kernels(nk, dev, kind, n, hidden)
             fms, _ = timed(torch, fwd, clock, args.window_ms / 4, args.reps)
             bms, _ = timed(torch, bwd, clock, args.window_ms / 4, args.reps)
@@ -209,9 +273,15 @@ def main():
                 "ms_per_sequence": {k: round(v, 3) for k, v in med.items()},
                 "ms_per_time_step": {k: round(v / T, 4) for k, v in med.items()},
                 "launches_per_time_step": {"fused": round(fused.kernel_count / T, 2),
-                                           "composed": round(comp.kernel_count / T, 2)},
+                                           "composed": round(comp.kernel_count / T, 2),
+                                           "sequence": round(seq.kernel_count / T, 2)},
                 "speedup_fused_vs_composed": round(med["composed"] / med["fused"], 2),
                 "speedup_fused_vs_torch_eager_bf16": round(med["torch_eager_bf16"] / med["fused"], 2),
+                "speedup_sequence_vs_fused": round(med["fused"] / med["sequence"], 2),
+                "speedup_sequence_vs_torch_cudnn_bf16": round(med["torch_cudnn_bf16"] / med["sequence"], 2),
+                "sequence_whole_gemms_ms": round(wms, 3), "sequence_sequential_gemms_ms": round(sms, 3),
+                "sequential_gemm_share_of_sequence_step": round(sms / med["sequence"], 3),
+                "whole_gemm_share_of_sequence_step": round(wms / med["sequence"], 3),
                 "gemm_only_ms_per_time_step": round(gms, 4),
                 "gemm_tflops": round(flops / gms / 1e9, 1),
                 "gemm_share_of_fused_step": round(gms * T / med["fused"], 3),
@@ -221,6 +291,7 @@ def main():
             }), flush=True)
             fused.close()
             comp.close()
+            seq.close()
     clock.halt.set()
 
 
