@@ -118,6 +118,14 @@ int nk_gemm_bias_act(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, 
                      float beta, void* C, int64_t ldc, int ab_dtype, int c_dtype,
                      const void* bias /* N elements, c_dtype or f32 */, int bias_dtype,
                      int relu);
+/* `batch` independent products C_b = alpha * op(A_b).op(B_b) + beta*C_b + bias_b, where X_b = X + b*strideX elements and
+ * bias_b (N elements, column-indexed, or NULL) = bias + b*bias_stride.  bf16 operands that TMA can address (16-byte
+ * aligned bases, leading dimensions and operand strides multiples of 8 elements, strides >= 0, every C_b 16-byte
+ * aligned; not TT) run as ONE launch of the batched wgmma kernel; anything else as one nk_gemm_bias_act per product. */
+int nk_gemm_strided_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha,
+                            const void* A, int64_t lda, int64_t strideA, const void* B, int64_t ldb, int64_t strideB,
+                            float beta, void* C, int64_t ldc, int64_t strideC, int64_t batch, int ab_dtype, int c_dtype,
+                            const void* bias, int64_t bias_stride, int bias_dtype);
 
 /* C = beta*C + relu'(relu_operand) (.) (op(A).op(B)): the input gradient of a matmul whose left operand is the output
  * of a ReLU, with that ReLU's backward (relu/mod.rs:71-78: dx += (x > 0) * g) applied in the GEMM epilogue instead of a
@@ -363,6 +371,27 @@ int nk_lstm_seq_bwd_step(nk_ctx* ctx, void* dgates, int dgates_dtype, float* dc,
                          const void* dh_out, const float* dh_rec, int64_t n, int64_t hidden, int dtype);
 int nk_gru_seq_bwd_step(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, float* dh_rec, const float* igates,
                         const float* hgates, const void* h_prev, const void* dh_out, int64_t n, int64_t hidden, int dtype);
+/* One time step of BOTH directions of a bidirectional sequence layer (nk_graph.h, nkg_lstm_layer / nkg_gru_layer) in one
+ * launch, with the gate maths above.  Every per-direction operand X is passed as direction 0's pointer plus X_dstride,
+ * the distance in elements (any sign) to direction 1's.  Rows of y, dh_out and the GRU backward's h_prev are ld* apart
+ * (2H for the layer's (T, N, 2H) output); every other (n, H) operand is dense.  h_next (forward), dc and dh_rec
+ * (backward, f32) are (2, n, H) buffers with direction stride n*H.
+ *   forward:  writes h' into y and h_next (and, LSTM, c' into c_out);
+ *   backward: as nk_lstm_seq_bwd_step / nk_gru_seq_bwd_step per direction; dgates / digates / dhgates share the gates'
+ *             layout (gates_dstride); dh_out and dh_rec may be NULL. */
+int nk_lstm_bidir_fwd_step(nk_ctx* ctx, void* y, int64_t y_dstride, int64_t ldy, void* h_next, void* c_out,
+                           int64_t c_out_dstride, const float* gates, int64_t gates_dstride, const void* c_prev,
+                           int64_t c_prev_dstride, int64_t n, int64_t hidden, int dtype);
+int nk_gru_bidir_fwd_step(nk_ctx* ctx, void* y, int64_t y_dstride, int64_t ldy, void* h_next, const float* igates,
+                          const float* hgates, int64_t gates_dstride, const void* h_prev, int64_t h_prev_dstride, int64_t n,
+                          int64_t hidden, int dtype);
+int nk_lstm_bidir_bwd_step(nk_ctx* ctx, void* dgates, int dgates_dtype, int64_t gates_dstride, float* dc, const float* gates,
+                           const void* c_prev, int64_t c_prev_dstride, const void* dh_out, int64_t dh_out_dstride,
+                           int64_t ld_dh_out, const float* dh_rec, int64_t n, int64_t hidden, int dtype);
+int nk_gru_bidir_bwd_step(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, int64_t gates_dstride, float* dh_rec,
+                          const float* igates, const float* hgates, const void* h_prev, int64_t h_prev_dstride,
+                          int64_t ld_h_prev, const void* dh_out, int64_t dh_out_dstride, int64_t ld_dh_out, int64_t n,
+                          int64_t hidden, int dtype);
 /* chunks (chunk/mod.rs): y = block `index` of x in row-major block order (ndarray's exact_chunks: trailing partial blocks
  * are dropped); a bit-exact copy.  Backward: dx[block] = beta*dx[block] + g, nothing else of dx is touched. */
 int nk_chunk_fwd(nk_ctx* ctx, void* y, const void* x, int ndim, const int64_t* x_shape, const int64_t* chunk_shape,

@@ -144,6 +144,18 @@ int nkg_lstm(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weig
              nkg_var* bias_hh, nkg_var** output, nkg_var** last_cell_state);
 int nkg_gru(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih, nkg_var* bias_hh,
             nkg_var** output);
+/* nkg_lstm_layer / nkg_gru_layer: one layer of torch.nn.LSTM / GRU, one or two directions (D = hidden's first dimension).
+ * input (T, N, I); hidden and cell_state (D, N, H); parameters stacked over the directions, weight_ih (D, G*H, I),
+ * weight_hh (D, G*H, H), biases (D, G*H), direction 1 = torch's `_reverse` parameters.  `output` (T, N, D*H) holds every
+ * time step's hidden state, the reverse direction's (which runs from time T-1 down to 0) in columns [H, 2H);
+ * `last_hidden` / `last_cell_state` (D, N, H) are each direction's state after its last step (time T-1 forward, time 0
+ * reverse).  ONE forward and ONE backward node.  D = 1 issues the calls of nkg_lstm / nkg_gru plus one N*H copy into
+ * last_hidden.  D = 2 runs both directions' step t in one nk_gemm_strided_batched and one nk_*_bidir_*_step launch
+ * (2 + 2T launches forward, 2T + the whole-sequence products backward) and keeps D times what one direction keeps. */
+int nkg_lstm_layer(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh,
+                   nkg_var* bias_ih, nkg_var* bias_hh, nkg_var** output, nkg_var** last_hidden, nkg_var** last_cell_state);
+int nkg_gru_layer(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
+                  nkg_var* bias_hh, nkg_var** output, nkg_var** last_hidden);
 
 /* ---- concatenation (var.rs:564-645, vardiff.rs:627-; multi_concatenate/mod.rs, multi_stack/mod.rs) ----
  * nkg_cat: the `count` operands side by side along `axis` (0 <= axis < ndim; equal shapes on every other axis, any length

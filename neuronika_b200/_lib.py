@@ -80,6 +80,8 @@ _PROTOS = {
     "nk_gemm": (i32, [vp, i32, i32, i64, i64, i64, f32, vp, i64, vp, i64, f32, vp, i64, i32, i32]),
     "nk_gemm_bias_act": (i32, [vp, i32, i32, i64, i64, i64, f32, vp, i64, vp, i64, f32, vp, i64, i32, i32,
                                vp, i32, i32]),
+    "nk_gemm_strided_batched": (i32, [vp, i32, i32, i64, i64, i64, f32, vp, i64, i64, vp, i64, i64, f32, vp, i64, i64,
+                                      i64, i32, i32, vp, i64, i32]),
     "nk_gemm_relu_bwd": (i32, [vp, i32, i32, i64, i64, i64, vp, i64, vp, i64, f32, vp, i64, i32, i32, vp]),
     "nk_gemm_relu_bwd_colsum": (i32, [vp, i32, i32, i64, i64, i64, vp, i64, vp, i64, f32, vp, i64, i32, i32, vp, vp]),
     "nk_add_bcast_fwd": (i32, [vp, vp, vp, vp, i32, i32, pi64, i32, pi64, i32, pi64]),
@@ -143,6 +145,10 @@ _PROTOS = {
     "nk_gru_cell_bwd": (i32, [vp, vp, vp, i32, vp, f32, vp, vp, vp, vp, i64, i64, i32]),
     "nk_lstm_seq_bwd_step": (i32, [vp, vp, i32, vp, vp, vp, vp, vp, i64, i64, i32]),
     "nk_gru_seq_bwd_step": (i32, [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, i64, i32]),
+    "nk_lstm_bidir_fwd_step": (i32, [vp, vp, i64, i64, vp, vp, i64, vp, i64, vp, i64, i64, i64, i32]),
+    "nk_gru_bidir_fwd_step": (i32, [vp, vp, i64, i64, vp, vp, vp, i64, vp, i64, i64, i64, i32]),
+    "nk_lstm_bidir_bwd_step": (i32, [vp, vp, i32, i64, vp, vp, vp, i64, vp, i64, i64, vp, i64, i64, i32]),
+    "nk_gru_bidir_bwd_step": (i32, [vp, vp, vp, i32, i64, vp, vp, vp, vp, i64, i64, vp, i64, i64, i64, i64, i32]),
     "nk_chunk_fwd": (i32, [vp, vp, vp, i32, pi64, pi64, i64, i32]),
     "nk_chunk_bwd": (i32, [vp, vp, i32, vp, i32, i32, pi64, pi64, i64, f32]),
     "nk_cat_fwd": (i32, [vp, vp, pvp, pi64, i32, i64, i64, i32]),

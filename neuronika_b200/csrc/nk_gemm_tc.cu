@@ -65,6 +65,7 @@ struct GemmParams {
   int batch, a_batched, b_batched, batch_reduce, splits;
   int64_t c_batch_stride;
   int tma_store;   // the epilogue writes C through the C tensor map (see the header); the host checks the conditions
+  int64_t bias_batch_stride;   // the bias of product b starts this many elements further (nk_gemm_strided_batched)
 };
 
 __device__ __forceinline__ int tile_m_block(const GemmParams& p, int tile) {
@@ -108,20 +109,21 @@ struct Cfg {
 // v[j] = alpha * acc[j] + bias (row- or column-indexed) for one 32-column chunk of one output row.  The product is
 // rounded before the bias is added (__fmul_rn: never contracted into an FMA), in every epilogue, so that all of them
 // store the same bits
-__device__ __forceinline__ void scale_and_bias(const GemmParams& p, int64_t row, int64_t col0, const uint32_t* r, bool full,
-                                               float* v) {
+// `bias` is p.bias, or the bias of the batch being drained
+__device__ __forceinline__ void scale_and_bias(const GemmParams& p, const void* bias, int64_t row, int64_t col0,
+                                               const uint32_t* r, bool full, float* v) {
 #pragma unroll
   for (int j = 0; j < 32; ++j) v[j] = __fmul_rn(p.alpha, __uint_as_float(r[j]));
-  if (p.bias && p.bias_per_row) {
-    const float b = p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[row]) : static_cast<const float*>(p.bias)[row];
+  if (bias && p.bias_per_row) {
+    const float b = p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(bias)[row]) : static_cast<const float*>(bias)[row];
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] += b;
-  } else if (p.bias) {
+  } else if (bias) {
     // 32 scalar loads here serialise on L1 latency and made the epilogue slower than a K = 1024 main loop:
     // fetch the 32 bias values of a full chunk with 16-byte loads
-    if (full && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0) {
+    if (full && (reinterpret_cast<uintptr_t>(bias) & 15) == 0) {
       if (p.bias_bf16) {
-        const uint4* bp = reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(p.bias) + col0);
+        const uint4* bp = reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(bias) + col0);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const uint4 w = __ldg(bp + q);
@@ -133,7 +135,7 @@ __device__ __forceinline__ void scale_and_bias(const GemmParams& p, int64_t row,
           }
         }
       } else {
-        const float4* bp = reinterpret_cast<const float4*>(static_cast<const float*>(p.bias) + col0);
+        const float4* bp = reinterpret_cast<const float4*>(static_cast<const float*>(bias) + col0);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
           const float4 w = __ldg(bp + q);
@@ -144,8 +146,8 @@ __device__ __forceinline__ void scale_and_bias(const GemmParams& p, int64_t row,
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (col0 + j < p.N)
-          v[j] += p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[col0 + j])
-                              : static_cast<const float*>(p.bias)[col0 + j];
+          v[j] += p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(bias)[col0 + j])
+                              : static_cast<const float*>(bias)[col0 + j];
     }
   }
 }
@@ -195,9 +197,19 @@ __device__ __forceinline__ void epilogue_colsum_chunk32(const GemmParams& p, int
   if (col0 + lane < p.N) atomicAdd(p.colsum + col0 + lane, v[0]);
 }
 
-template <typename TC>
+// The bias of the product whose C starts c_off elements into p.C (kernels instantiated with BATCH_BIAS, for
+// nk_gemm_strided_batched: biases bias_batch_stride apart).  Derived from c_off where it is used rather than kept as a
+// pointer across the drain: one more 64-bit value live in the 256-wide kernels, which run at the register cap, costs
+// spills.  The other kernels (the convolution's batched ones among them) read p.bias as before.
+template <bool BATCH_BIAS>
+__device__ __forceinline__ const void* batch_bias(const GemmParams& p, int64_t c_off) {
+  if (!BATCH_BIAS || !c_off) return p.bias;
+  return static_cast<const char*>(p.bias) + (c_off / p.c_batch_stride) * p.bias_batch_stride * (p.bias_bf16 ? 2 : 4);
+}
+
+template <typename TC, bool BATCH_BIAS>
 __device__ __forceinline__ void epilogue_store_chunk32(const GemmParams& p, int64_t row, int64_t col0, const uint32_t* r,
-                                                       int ncols, bool vec_ok, int64_t c_off = 0, bool atomic = false) {
+                                                       int ncols, bool vec_ok, int64_t c_off, bool atomic) {
   TC* crow = static_cast<TC*>(p.C) + c_off + row * p.ldc + col0;
   if (atomic) {  // partial sum of a split reduction: f32 atomics (alpha applied, beta handled by the host)
     if constexpr (sizeof(TC) == 4) {
@@ -213,7 +225,7 @@ __device__ __forceinline__ void epilogue_store_chunk32(const GemmParams& p, int6
   }
   float v[32];
   const bool full = (col0 + 32 <= p.N) && ncols == 32;
-  scale_and_bias(p, row, col0, r, full, v);
+  scale_and_bias(p, batch_bias<BATCH_BIAS>(p, c_off), row, col0, r, full, v);
   const TC* mrow = p.mask ? static_cast<const TC*>(p.mask) + row * p.ldc + col0 : nullptr;
   if (full && vec_ok) {
     constexpr int V = 16 / sizeof(TC);
@@ -279,7 +291,7 @@ __device__ __forceinline__ float epi_value(const GemmParams& p, float acc, float
   return p.relu ? (v > 0.f ? v : 0.f) : v;
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false>
+template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false, bool BATCH_BIAS = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
@@ -512,9 +524,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           const int srow = warp * 16 + rr;
           const int64_t grow = int64_t(m_blk) * BLOCK_M + cw * 64 + srow;
           if (grow >= p.M) break;
+          const void* bias = p.bias;
+          if constexpr (BATCH_BIAS) bias = batch_bias<true>(p, c_off);
           float rb = 0.f;
-          if (p.bias && p.bias_per_row)
-            rb = p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[grow]) : static_cast<const float*>(p.bias)[grow];
+          if (bias && p.bias_per_row)
+            rb = p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(bias)[grow]) : static_cast<const float*>(bias)[grow];
           for (int c = lane; c < chunk_cols; c += 32) {
             const int64_t col = col_base + c;
             if (col >= p.N) break;
@@ -524,10 +538,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
               if constexpr (sizeof(TC) == 4) atomicAdd(reinterpret_cast<float*>(cp), v);
               continue;
             }
-            if (p.bias) {
+            if (bias) {
               v += p.bias_per_row ? rb
-                                  : (p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[col])
-                                                 : static_cast<const float*>(p.bias)[col]);
+                                  : (p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(bias)[col])
+                                                 : static_cast<const float*>(bias)[col]);
             }
             if (p.beta != 0.f) v += p.beta * nk_to_f32<TC>(*cp);
             if (p.relu) v = v > 0.f ? v : 0.f;
@@ -548,7 +562,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
         const int64_t col0 = int64_t(n_blk) * BLOCK_N + ch * kEpiCols + half * 32;
         if (p.colsum && col0 < p.N) epilogue_colsum_chunk32<TC>(p, row, col0, r, lane, vec_ok);
-        if (row < p.M && col0 < p.N) epilogue_store_chunk32<TC>(p, row, col0, r, ncols, vec_ok, c_off, atomic);
+        if (row < p.M && col0 < p.N) epilogue_store_chunk32<TC, BATCH_BIAS>(p, row, col0, r, ncols, vec_ok, c_off, atomic);
       }
     }
   }
@@ -579,10 +593,10 @@ int make_tmap_2d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t rows, i
   return NK_OK;
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false>
+template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false, bool BATCH_BIAS = false>
 int launch_cfg(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, GemmParams& p) {
   using C_ = Cfg<BLOCK_N>;
-  auto kern = gemm_tc_kernel<BLOCK_N, A_MN, B_MN, TC, BATCH>;
+  auto kern = gemm_tc_kernel<BLOCK_N, A_MN, B_MN, TC, BATCH, BATCH_BIAS>;
   static bool attr_done[64] = {};  // per template instantiation and device (the attribute is per device)
   if (!attr_done[ctx->device & 63]) {
     static_assert(C_::SMEM_BYTES <= kSmemLimit, "shared memory budget");
@@ -683,7 +697,7 @@ int nk_gemm_wgmma(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int
   p.relu = relu;
   p.mask = mask;
   p.colsum = colsum;
-  p.batch = 1, p.a_batched = p.b_batched = p.batch_reduce = 0, p.splits = 1, p.c_batch_stride = 0;
+  p.batch = 1, p.a_batched = p.b_batched = p.batch_reduce = 0, p.splits = 1, p.c_batch_stride = 0, p.bias_batch_stride = 0;
   p.num_m_blocks = int((M + BLOCK_M - 1) / BLOCK_M);
   p.num_n_blocks = 0;
   p.num_k_blocks = int((K + BLOCK_K - 1) / BLOCK_K);
@@ -771,14 +785,14 @@ static int make_tmap_3d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t 
   return NK_OK;
 }
 
-// `batch` products C_b = alpha * op(A_b).op(B_b) (+ row bias, ReLU) with operands batch_stride elements apart (stride 0 = the
-// same operand for every batch), or -- reduce != 0 -- ONE product C += alpha * sum_b op(A_b).op(B_b) (C f32, accumulated
-// with atomics: the caller zeroes / scales C first).  The engine behind the im2col convolution path (nk_conv_gemm.cu).
-// Returns NK_ERR_UNSUPPORTED (last_error untouched) when the operands are not TMA-addressable.
-int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
-                            int64_t lda, int64_t strideA, const void* B, int64_t ldb, int64_t strideB, void* C, int64_t ldc,
-                            int64_t strideC, int64_t batch, int c_dtype, const void* row_bias, int bias_dtype, int relu,
-                            int reduce) {
+// `batch` products C_b = alpha * op(A_b).op(B_b) + beta*C_b (+ bias, ReLU) with operands batch_stride elements apart
+// (stride 0 = the same operand for every batch), or -- reduce != 0 -- ONE product C += alpha * sum_b op(A_b).op(B_b) (C
+// f32, accumulated with atomics: the caller zeroes / scales C first; beta is ignored).  The bias is indexed by the output
+// row (bias_per_row) or column; that of product b starts bias_stride elements further.
+static int gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
+                              int64_t lda, int64_t strideA, const void* B, int64_t ldb, int64_t strideB, float beta, void* C,
+                              int64_t ldc, int64_t strideC, int64_t batch, int c_dtype, const void* bias, int bias_dtype,
+                              int bias_per_row, int64_t bias_stride, int relu, int reduce) {
   if (!nk_gemm_wgmma_supported(transA, transB, M, N, K, A, lda, B, ldb)) return NK_ERR_UNSUPPORTED;
   if (batch < 1 || batch > (int64_t(1) << 30) || (strideA * 2) % 16 != 0 || (strideB * 2) % 16 != 0) return NK_ERR_UNSUPPORTED;
   if (reduce && c_dtype != NK_F32) return NK_ERR_UNSUPPORTED;
@@ -786,8 +800,9 @@ int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_
   int block_n = N <= 64 ? 64 : (N <= 128 ? 128 : 256);
   GemmParams p;
   p.M = M, p.N = N, p.K = K, p.ldc = ldc, p.C = C;
-  p.bias = row_bias, p.bias_bf16 = bias_dtype == NK_BF16, p.bias_per_row = 1;
-  p.alpha = alpha, p.beta = 0.f, p.relu = relu, p.mask = nullptr, p.colsum = nullptr;
+  p.bias = bias, p.bias_bf16 = bias_dtype == NK_BF16, p.bias_per_row = bias_per_row;
+  p.bias_batch_stride = bias ? bias_stride : 0;   // the drain finds a product's bias from its C offset (batch_bias)
+  p.alpha = alpha, p.beta = reduce ? 0.f : beta, p.relu = relu, p.mask = nullptr, p.colsum = nullptr;
   p.num_m_blocks = int((M + BLOCK_M - 1) / BLOCK_M);
   p.num_n_blocks = 0;
   p.num_k_blocks = int((K + BLOCK_K - 1) / BLOCK_K);
@@ -815,9 +830,13 @@ int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_
   CUtensorMap tc;
   memset(&tc, 0, sizeof(tc));
   ctx->last_gemm_kernel = "wgmma_batched";
-#define NK_TCB(BN, AM, BM_)                                                                          \
-  (c_dtype == NK_BF16 ? launch_cfg<BN, AM, BM_, __nv_bfloat16, true>(ctx, ta, tb, tc, p)              \
-                      : launch_cfg<BN, AM, BM_, float, true>(ctx, ta, tb, tc, p))
+  // products with biases of their own get the kernels that find each product's bias (batch_bias)
+  const bool per_batch_bias = p.bias && p.bias_batch_stride && !reduce;
+#define NK_TCB(BN, AM, BM_)                                                                                      \
+  (per_batch_bias ? (c_dtype == NK_BF16 ? launch_cfg<BN, AM, BM_, __nv_bfloat16, true, true>(ctx, ta, tb, tc, p) \
+                                        : launch_cfg<BN, AM, BM_, float, true, true>(ctx, ta, tb, tc, p))        \
+                  : (c_dtype == NK_BF16 ? launch_cfg<BN, AM, BM_, __nv_bfloat16, true>(ctx, ta, tb, tc, p)       \
+                                        : launch_cfg<BN, AM, BM_, float, true>(ctx, ta, tb, tc, p)))
 #define NK_TCB_BN(AM, BM_) (block_n == 256 ? NK_TCB(256, AM, BM_) : block_n == 128 ? NK_TCB(128, AM, BM_) : NK_TCB(64, AM, BM_))
   if (!a_mn && !b_mn) return NK_TCB_BN(false, false);
   if (!a_mn && b_mn) return NK_TCB_BN(false, true);
@@ -825,6 +844,16 @@ int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_
   return nk_set_error(ctx, NK_ERR_UNSUPPORTED, "batched gemm: the TT form is not instantiated");
 #undef NK_TCB_BN
 #undef NK_TCB
+}
+
+// The engine behind the im2col convolution path (nk_conv_gemm.cu): beta 0, row-indexed bias shared by the batches.
+// Returns NK_ERR_UNSUPPORTED (last_error untouched) when the operands are not TMA-addressable.
+int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
+                            int64_t lda, int64_t strideA, const void* B, int64_t ldb, int64_t strideB, void* C, int64_t ldc,
+                            int64_t strideC, int64_t batch, int c_dtype, const void* row_bias, int bias_dtype, int relu,
+                            int reduce) {
+  return gemm_wgmma_batched(ctx, transA, transB, M, N, K, alpha, A, lda, strideA, B, ldb, strideB, 0.f, C, ldc, strideC, batch,
+                            c_dtype, row_bias, bias_dtype, 1, 0, relu, reduce);
 }
 
 extern "C" {
@@ -855,6 +884,41 @@ int nk_gemm_bias_act(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, 
   }
   return nk_gemm_simt(ctx, transA, transB, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, ab_dtype, c_dtype, bias,
                       bias_dtype, relu);
+}
+
+int nk_gemm_strided_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
+                            int64_t lda, int64_t strideA, const void* B, int64_t ldb, int64_t strideB, float beta, void* C,
+                            int64_t ldc, int64_t strideC, int64_t batch, int ab_dtype, int c_dtype, const void* bias,
+                            int64_t bias_stride, int bias_dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, nk_dtype_ok(ab_dtype) && nk_dtype_ok(c_dtype), "nk_gemm_strided_batched: bad dtype");
+  NK_REQUIRE(ctx, M >= 0 && N >= 0 && K >= 0 && batch >= 0, "nk_gemm_strided_batched: negative dimension");
+  NK_REQUIRE(ctx, !bias || nk_dtype_ok(bias_dtype), "nk_gemm_strided_batched: bad bias dtype");
+  if (M == 0 || N == 0 || batch == 0) return NK_OK;
+  // one launch of the batched wgmma kernel (TMA needs non-negative operand strides); its drain epilogue decides on 16-byte
+  // stores from the first product's C, so every product's C must sit on a 16-byte boundary like the first one's
+  const size_t cs = nk_dtype_size(c_dtype), bs = bias ? nk_dtype_size(bias_dtype) : 0;
+  const bool tc = ab_dtype == NK_BF16 && ctx->gemm_engine != NK_GEMM_SIMT && K > 0 && !(transA && transB) &&
+                  strideA >= 0 && strideB >= 0 && strideC >= 0 && bias_stride >= 0 && (strideC * int64_t(cs)) % 16 == 0 &&
+                  (!bias || !bias_stride || batch == 1 || strideC > 0) &&
+                  lda >= (transA ? M : K) && ldb >= (transB ? K : N) && ldc >= N;
+  if (tc) {
+    NK_REQUIRE(ctx, A && B && C, "nk_gemm_strided_batched: NULL pointer");
+    const int rc = gemm_wgmma_batched(ctx, transA, transB, M, N, K, alpha, A, lda, strideA, B, ldb, strideB, beta, C, ldc,
+                                      strideC, batch, c_dtype, bias, bias_dtype, 0, bias_stride, 0, 0);
+    if (rc != NK_ERR_UNSUPPORTED) return rc;
+  }
+  // everything else: one GEMM per product (which checks the arguments)
+  const size_t as = nk_dtype_size(ab_dtype);
+  for (int64_t b = 0; b < batch; ++b) {
+    const int rc = nk_gemm_bias_act(
+        ctx, transA, transB, M, N, K, alpha, A ? static_cast<const char*>(A) + b * strideA * int64_t(as) : nullptr, lda,
+        B ? static_cast<const char*>(B) + b * strideB * int64_t(as) : nullptr, ldb, beta,
+        C ? static_cast<char*>(C) + b * strideC * int64_t(cs) : nullptr, ldc, ab_dtype, c_dtype,
+        bias ? static_cast<const char*>(bias) + b * bias_stride * int64_t(bs) : nullptr, bias_dtype, 0);
+    if (rc) return rc;
+  }
+  return NK_OK;
 }
 
 int nk_gemm_relu_bwd_colsum(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, const void* A, int64_t lda,

@@ -1339,37 +1339,57 @@ struct RnnCellBackward : Backward {  // `gradient` is the new hidden state's; c_
 };
 
 // ------------------------------------------------------------------------------- recurrent sequence layers
-// nn.LSTM / nn.GRU (one layer, one direction, time-major) as ONE forward and ONE backward node whatever T is.  Of a
-// cell's products only h_{t-1}.W_hh^T (forward) and dG_t.W_hh (backward) depend on the recurrence; the others run once
-// over all T*N rows: X.W_ih^T + b_ih, dW_ih, dW_hh, dX and the bias column sums.  The node keeps the f32 gate
-// pre-activations of every step (what T cell nodes keep) and, for the LSTM, the cell states.  The backward carries the
-// state gradients (dc, and the part of dh that comes back through W_hh) in f32 from step T-1 down to step 0
-// (nk_lstm_seq_bwd_step / nk_gru_seq_bwd_step) and converts them once, into the gradients of the initial states.
+// nn.LSTM / nn.GRU (time-major) as ONE forward and ONE backward node per layer whatever T is.  Of a cell's products only
+// h_{t-1}.W_hh^T (forward) and dG_t.W_hh (backward) depend on the recurrence; the others run once over all T*N rows:
+// X.W_ih^T + b_ih, dW_ih, dW_hh, dX and the bias column sums.  The node keeps the f32 gate pre-activations of every step
+// (what T cell nodes keep) and, for the LSTM, the cell states.  The backward carries the state gradients (dc, and the
+// part of dh that comes back through W_hh) in f32 from the last step down to step 0 (nk_lstm_seq_bwd_step /
+// nk_gru_seq_bwd_step) and converts them once, into the gradients of the initial states.
+// A bidirectional layer (D = 2) runs both directions in the same node: step s is time s of the forward direction and
+// time T-1-s of the reverse one, and each step is ONE nk_gemm_strided_batched (the two directions' recurrent products)
+// and ONE two-direction step kernel (nk_*_bidir_*_step), so it launches per step what a one-direction layer launches.
+// The parameters are stacked over directions, (D, G, *), and the gates and gate gradients are (D, T*N, G) in time
+// order, so the step-s operands of the two directions are a constant distance apart: (2T-1-2s)*N*G elements of the
+// gates, G*H of W_hh, N*H of the (2, N, H) state buffers.
 static inline char* at(void* p, int64_t elems, int dt) { return static_cast<char*>(p) + size_t(elems) * esize(dt); }
 static inline const char* at(const void* p, int64_t elems, int dt) {
   return static_cast<const char*>(p) + size_t(elems) * esize(dt);
 }
+struct RnnDims {
+  int64_t T, N, I, H, D;
+};
 struct RnnSeq : Forward {
   bool lstm;
-  CellOperands o;      // x is (T, N, I)
-  TensorP gi, gh;      // f32 gate pre-activations of every step: LSTM (T*N, 4H) in gi; GRU (T*N, 3H) in gi and gh
-  TensorP out;         // (T, N, H): every step's hidden state
-  TensorP cs, c_last;  // LSTM: the cell states of steps 0 .. T-2, (T-1, N, H), and the last one, (N, H)
-  RnnSeq(nk_ctx* c, bool l, CellOperands ops, TensorP output) : Forward(c), lstm(l), o(std::move(ops)), out(std::move(output)) {
-    const int64_t T = o.x->shape[0], N = o.x->shape[1], H = o.h->shape[1], G = o.w_ih->shape[0];
-    gi = std::make_shared<Tensor>(c, Shape{T * N, G}, NK_F32);
-    if (!lstm) gh = std::make_shared<Tensor>(c, Shape{T * N, G}, NK_F32);
+  int64_t T, N, I, H, G, D;
+  CellOperands o;      // x is (T, N, I); a layer's states are (D, N, H) and its parameters (D, G, *)
+  TensorP gi, gh;      // f32 gate pre-activations of every step: LSTM (D, T*N, 4H) in gi; GRU (D, T*N, 3H) in gi and gh
+  TensorP out;         // (T, N, D*H): every step's hidden state, the reverse direction in columns [H, 2H)
+  TensorP cs, c_last;  // LSTM: the cell states of steps 0 .. T-2, (D, T-1, N, H), and the last one, (D, N, H) ((N, H) for
+                       // nkg_lstm)
+  TensorP h_n;         // layers (nkg_lstm_layer / nkg_gru_layer): the last hidden state of each direction, (D, N, H)
+  RnnSeq(nk_ctx* c, bool l, bool layer, const RnnDims& dm, CellOperands ops, TensorP output)
+      : Forward(c), lstm(l), T(dm.T), N(dm.N), I(dm.I), H(dm.H), G((l ? 4 : 3) * dm.H), D(dm.D), o(std::move(ops)),
+        out(std::move(output)) {
+    gi = std::make_shared<Tensor>(c, Shape{D, T * N, G}, NK_F32);
+    if (!lstm) gh = std::make_shared<Tensor>(c, Shape{D, T * N, G}, NK_F32);
+    const Shape state = layer ? Shape{D, N, H} : Shape{N, H};
     if (lstm) {
-      cs = std::make_shared<Tensor>(c, Shape{T - 1, N, H}, out->dtype);
-      c_last = std::make_shared<Tensor>(c, Shape{N, H}, out->dtype);
+      cs = std::make_shared<Tensor>(c, Shape{D, T - 1, N, H}, out->dtype);
+      c_last = std::make_shared<Tensor>(c, state, out->dtype);
     }
+    if (layer) h_n = std::make_shared<Tensor>(c, state, out->dtype);
   }
   const char* name() const override { return lstm ? "LSTM" : "GRU"; }
-  // the state before step t: the initial one, or what step t-1 wrote
+  // D = 1: the state before step t, the initial one or what step t-1 wrote
   const void* h_prev(int64_t t, int64_t NH) const { return t ? at(out->rptr(), (t - 1) * NH, out->dtype) : o.h->rptr(); }
   const void* c_prev(int64_t t, int64_t NH) const { return t ? at(cs->rptr(), (t - 1) * NH, cs->dtype) : o.c->rptr(); }
+  // D = 2: the cell state before step s of direction 0, and the distance to direction 1's
+  const void* c_prev2(int64_t s, int64_t& dstride) const {
+    dstride = s ? (T - 1) * N * H : N * H;
+    return s ? at(cs->rptr(), (s - 1) * N * H, cs->dtype) : o.c->rptr();
+  }
   void forward() override {
-    const int64_t T = o.x->shape[0], N = o.x->shape[1], I = o.x->shape[2], H = o.h->shape[1], G = o.w_ih->shape[0];
+    if (D == 2) return forward_bidir();
     const int dt = o.x->dtype;
     gemm(ctx, false, true, T * N, G, I, o.x->rptr(), I, o.w_ih->rptr(), I, 0.f, gi->wptr(), dt, NK_F32, o.b_ih->rptr(),
          o.b_ih->dtype);
@@ -1389,16 +1409,61 @@ struct RnnSeq : Forward {
         ck(ctx, nk_gru_cell_fwd(ctx, y_t, gi_t, gh_t, h_prev(t, N * H), N, H, dt));
       }
     }
+    if (h_n) ck(ctx, nk_cast(ctx, h_n->wptr(), dt, at(y, (T - 1) * N * H, dt), dt, size_t(N * H)));
+  }
+  void forward_bidir() {
+    const int dt = o.x->dtype;
+    const int64_t NH = N * H, NG = N * G;
+    float* g = static_cast<float*>(gi->wptr());
+    for (int64_t d = 0; d < 2; ++d)
+      gemm(ctx, false, true, T * N, G, I, o.x->rptr(), I, at(o.w_ih->rptr(), d * G * I, dt), I, 0.f, g + d * T * NG, dt,
+           NK_F32, at(o.b_ih->rptr(), d * G, o.b_ih->dtype), o.b_ih->dtype);
+    float* gH = lstm ? g : static_cast<float*>(gh->wptr());   // the recurrent products: added to the LSTM's gates
+    void* y = out->wptr();
+    // (2, 2, N, H) ping-pong of the (2, N, H) hidden states that the next step's GEMM reads, for this pass only (the
+    // backward reads the states from the output)
+    void* hs = nullptr;
+    if (T > 1) ck(ctx, nk_alloc_uninit(ctx, size_t(4 * NH) * esize(dt), &hs));
+    try {
+      steps_bidir(g, gH, y, hs);
+    } catch (...) {
+      if (hs) nk_free(ctx, hs);
+      throw;
+    }
+    if (hs) ck(ctx, nk_free(ctx, hs));
+  }
+  void steps_bidir(float* g, float* gH, void* y, void* hs) {
+    const int dt = o.x->dtype;
+    const int64_t NH = N * H, NG = N * G;
+    for (int64_t s = 0; s < T; ++s) {
+      const void* hp = s ? at(hs, ((s - 1) & 1) * 2 * NH, dt) : o.h->rptr();
+      void* hn = s == T - 1 ? h_n->wptr() : at(hs, (s & 1) * 2 * NH, dt);
+      const int64_t gds = (2 * T - 1 - 2 * s) * NG;               // gates: time s of direction 0 -> time T-1-s of direction 1
+      void* y_s = at(y, s * N * 2 * H, dt);
+      const int64_t yds = (T - 1 - 2 * s) * N * 2 * H + H;         // output: row T-1-s, columns [H, 2H)
+      ck(ctx, nk_gemm_strided_batched(ctx, 0, 1, N, G, H, 1.f, hp, H, NH, o.w_hh->rptr(), H, G * H, lstm ? 1.f : 0.f,
+                                      gH + s * NG, G, gds, 2, dt, NK_F32, o.b_hh->rptr(), G, o.b_hh->dtype));
+      if (lstm) {
+        int64_t cpds;
+        const void* cp = c_prev2(s, cpds);
+        void* co = s == T - 1 ? c_last->wptr() : at(cs->wptr(), s * NH, dt);
+        ck(ctx, nk_lstm_bidir_fwd_step(ctx, y_s, yds, 2 * H, hn, co, s == T - 1 ? NH : (T - 1) * NH, g + s * NG, gds, cp,
+                                       cpds, N, H, dt));
+      } else {
+        ck(ctx, nk_gru_bidir_fwd_step(ctx, y_s, yds, 2 * H, hn, g + s * NG, gH + s * NG, gds, hp, NH, N, H, dt));
+      }
+    }
   }
 };
 
-struct RnnSeqBackward : Backward {  // `gradient` is the output's, (T, N, H); c_last_grad the last cell state's (LSTM)
+struct RnnSeqBackward : Backward {  // `gradient` is the output's, (T, N, D*H); c_last_grad / h_n_grad the last states'
   std::shared_ptr<RnnSeq> fw;
   CellGrads d;
-  GradientP c_last_grad;
+  GradientP c_last_grad, h_n_grad;
   RnnSeqBackward(nk_ctx* c, GradientP g, std::shared_ptr<RnnSeq> f, CellGrads grads)
       : Backward(c, std::move(g)), fw(std::move(f)), d(std::move(grads)) {
     if (fw->lstm) c_last_grad = std::make_shared<Gradient>(c, fw->c_last->shape, fw->c_last->dtype);
+    if (fw->h_n) h_n_grad = std::make_shared<Gradient>(c, fw->h_n->shape, fw->h_n->dtype);
   }
   const char* name() const override { return fw->lstm ? "LSTMBackward" : "GRUBackward"; }
   void targets(std::vector<Gradient*>& out) override {
@@ -1410,26 +1475,36 @@ struct RnnSeqBackward : Backward {  // `gradient` is the output's, (T, N, H); c_
     if (r->rs_world > 1 && r->rs_hook && r->last_writer == g_bwd_pos) r->rs_hook(r->rs_user, 0);
     grad_written(g);
   }
-  void bias(const GradientP& g, const void* dG, int64_t G, int64_t rows, int dt) {
+  // the column sums of each direction's (rows, G) slice of dG, into that direction's row of g
+  void bias(const GradientP& g, const void* dG, int64_t G, int64_t rows, int dt, int64_t D = 1) {
     if (!g) return;
     const int64_t ds[1] = {G}, gs[2] = {rows, G};
-    accumulate(ctx, g, [&](void* p, float beta) { ck(ctx, nk_unbroadcast_acc(ctx, p, g->dtype, 1, ds, dG, dt, 2, gs, beta)); });
+    accumulate(ctx, g, [&](void* p, float beta) {
+      for (int64_t k = 0; k < D; ++k)
+        ck(ctx, nk_unbroadcast_acc(ctx, at(p, k * G, g->dtype), g->dtype, 1, ds, at(dG, k * rows * G, dt), dt, 2, gs, beta));
+    });
     grad_written(g);
   }
-  // g += the f32 (N, H) state gradient the loop carried, converted into g's element type
-  void state(const GradientP& g, const float* carried, int64_t N, int64_t H) {
+  // g += the f32 (rows, H) state gradient the loop carried, converted into g's element type
+  void state(const GradientP& g, const float* carried, int64_t rows, int64_t H) {
     if (!g) return;
-    const int64_t s[2] = {N, H};
+    const int64_t s[2] = {rows, H};
     accumulate(ctx, g, [&](void* p, float beta) { ck(ctx, nk_unbroadcast_acc(ctx, p, g->dtype, 2, s, carried, NK_F32, 2, s, beta)); });
     grad_written(g);
+  }
+  // the carried f32 state gradient starts as the gradient of the last state (false: nobody wrote one)
+  bool seed(void* carried, const GradientP& last, int64_t n) {
+    const void* g = grad_or_null(last);
+    if (g) ck(ctx, nk_cast(ctx, carried, NK_F32, g, last->dtype, size_t(n)));
+    return g != nullptr;
   }
   void backward() override {
     const CellOperands& o = fw->o;
     const bool lstm = fw->lstm;
-    const int64_t T = o.x->shape[0], N = o.x->shape[1], I = o.x->shape[2], H = o.h->shape[1], G = o.w_ih->shape[0];
+    const int64_t T = fw->T, N = fw->N, I = fw->I, H = fw->H, G = fw->G, D = fw->D;
     const int64_t NH = N * H, NG = N * G;
     const int dt = o.x->dtype;
-    const size_t gbytes = size_t(T) * size_t(NG) * esize(dt), sbytes = size_t(NH) * sizeof(float);
+    const size_t gbytes = size_t(D * T) * size_t(NG) * esize(dt), sbytes = size_t(D * NH) * sizeof(float);
     void *dI = nullptr, *dH = nullptr, *dh_rec = nullptr, *dc = nullptr;
     auto release = [&] {
       if (dc) nk_free(ctx, dc);
@@ -1442,58 +1517,98 @@ struct RnnSeqBackward : Backward {  // `gradient` is the output's, (T, N, H); c_
       ck(ctx, nk_alloc_uninit(ctx, sbytes, &dh_rec));
       const void* dY = grad_or_null(gradient);
       const float* gi = reinterpret_cast<const float*>(fw->gi->rptr());
+      const float* gh = lstm ? nullptr : reinterpret_cast<const float*>(fw->gh->rptr());
+      bool dh_seeded = false;   // dh_rec holds the last hidden state's gradient before the last step
       if (lstm) {
         dH = dI;   // one gate gradient for both products
         ck(ctx, nk_alloc_uninit(ctx, sbytes, &dc));
-        if (const void* dcT = grad_or_null(c_last_grad))
-          ck(ctx, nk_cast(ctx, dc, NK_F32, dcT, c_last_grad->dtype, size_t(NH)));
-        else
-          ck(ctx, nk_memset0(ctx, dc, sbytes));
+        if (!seed(dc, c_last_grad, D * NH)) ck(ctx, nk_memset0(ctx, dc, sbytes));
+        dh_seeded = seed(dh_rec, h_n_grad, D * NH);
       } else {
         ck(ctx, nk_alloc_uninit(ctx, gbytes, &dH));
-        ck(ctx, nk_memset0(ctx, dh_rec, sbytes));
+        if (!seed(dh_rec, h_n_grad, D * NH)) ck(ctx, nk_memset0(ctx, dh_rec, sbytes));
       }
-      for (int64_t t = T - 1; t >= 0; --t) {
-        const void* dY_t = dY ? at(dY, t * NH, gradient->dtype) : nullptr;
-        const bool send_back = t > 0 || d.h;   // somebody reads the gradient of the state before step t
-        if (lstm) {
-          ck(ctx, nk_lstm_seq_bwd_step(ctx, at(dI, t * NG, dt), dt, static_cast<float*>(dc), gi + t * NG,
-                                       fw->c_prev(t, NH), dY_t, t == T - 1 ? nullptr : static_cast<const float*>(dh_rec),
-                                       N, H, dt));
-          if (send_back) gemm(ctx, false, false, N, H, G, at(dH, t * NG, dt), G, o.w_hh->rptr(), H, 0.f, dh_rec, dt, NK_F32);
-        } else {
-          const float* gh = reinterpret_cast<const float*>(fw->gh->rptr());
-          ck(ctx, nk_gru_seq_bwd_step(ctx, at(dI, t * NG, dt), at(dH, t * NG, dt), dt, static_cast<float*>(dh_rec),
-                                      gi + t * NG, gh + t * NG, fw->h_prev(t, NH), dY_t, N, H, dt));
-          if (send_back) gemm(ctx, false, false, N, H, G, at(dH, t * NG, dt), G, o.w_hh->rptr(), H, 1.f, dh_rec, dt, NK_F32);
+      const float* dh_last = dh_seeded ? static_cast<const float*>(dh_rec) : nullptr;
+      if (D == 1) {
+        for (int64_t t = T - 1; t >= 0; --t) {
+          const void* dY_t = dY ? at(dY, t * NH, gradient->dtype) : nullptr;
+          const bool send_back = t > 0 || d.h;   // somebody reads the gradient of the state before step t
+          if (lstm) {
+            ck(ctx, nk_lstm_seq_bwd_step(ctx, at(dI, t * NG, dt), dt, static_cast<float*>(dc), gi + t * NG,
+                                         fw->c_prev(t, NH), dY_t, t == T - 1 ? dh_last : static_cast<const float*>(dh_rec),
+                                         N, H, dt));
+            if (send_back) gemm(ctx, false, false, N, H, G, at(dH, t * NG, dt), G, o.w_hh->rptr(), H, 0.f, dh_rec, dt, NK_F32);
+          } else {
+            ck(ctx, nk_gru_seq_bwd_step(ctx, at(dI, t * NG, dt), at(dH, t * NG, dt), dt, static_cast<float*>(dh_rec),
+                                        gi + t * NG, gh + t * NG, fw->h_prev(t, NH), dY_t, N, H, dt));
+            if (send_back) gemm(ctx, false, false, N, H, G, at(dH, t * NG, dt), G, o.w_hh->rptr(), H, 1.f, dh_rec, dt, NK_F32);
+          }
+        }
+      } else {
+        const void* y = fw->out->rptr();
+        for (int64_t s = T - 1; s >= 0; --s) {
+          const int64_t gds = (2 * T - 1 - 2 * s) * NG;
+          const void* dY_s = dY ? at(dY, s * N * 2 * H, gradient->dtype) : nullptr;
+          const int64_t yds = (T - 1 - 2 * s) * N * 2 * H + H;
+          const bool send_back = s > 0 || d.h;
+          if (lstm) {
+            int64_t cpds;
+            const void* cp = fw->c_prev2(s, cpds);
+            ck(ctx, nk_lstm_bidir_bwd_step(ctx, at(dI, s * NG, dt), dt, gds, static_cast<float*>(dc), gi + s * NG, cp, cpds,
+                                           dY_s, yds, 2 * H, s == T - 1 ? dh_last : static_cast<const float*>(dh_rec), N,
+                                           H, dt));
+          } else {
+            // the hidden state before step s: the initial one, or output rows s-1 (direction 0) and T-s (direction 1)
+            const void* hp = s ? at(y, (s - 1) * N * 2 * H, dt) : o.h->rptr();
+            const int64_t hpds = s ? (T - 2 * s + 1) * N * 2 * H + H : NH;
+            ck(ctx, nk_gru_bidir_bwd_step(ctx, at(dI, s * NG, dt), at(dH, s * NG, dt), dt, gds, static_cast<float*>(dh_rec),
+                                          gi + s * NG, gh + s * NG, hp, hpds, s ? 2 * H : H, dY_s, yds, 2 * H, N, H, dt));
+          }
+          if (send_back)
+            ck(ctx, nk_gemm_strided_batched(ctx, 0, 0, N, H, G, 1.f, at(dH, s * NG, dt), G, gds, o.w_hh->rptr(), H, G * H,
+                                            lstm ? 0.f : 1.f, dh_rec, H, NH, 2, dt, NK_F32, nullptr, 0, NK_F32));
         }
       }
       // the parameters first (their data-parallel exchange can then overlap the rest), as the cell does.  Each weight
       // gradient is written by this node alone, so its hook and its reduce-scatter report fire once, after the last GEMM
-      if (d.w_hh) {   // dW_hh += dG[1:]^T.output[:T-1] + dG[0]^T.hidden (TN)
+      if (d.w_hh) {   // dW_hh += dG[later steps]^T.output[earlier steps] + dG[first step]^T.hidden (TN), per direction
+        const void* y = fw->out->rptr();
+        const int64_t ldy = D * H;
         accumulate(ctx, d.w_hh, [&](void* p, float beta) {
-          if (T > 1)
-            gemm(ctx, true, false, G, H, (T - 1) * N, at(dH, NG, dt), G, fw->out->rptr(), H, beta, p, dt, d.w_hh->dtype);
-          gemm(ctx, true, false, G, H, N, dH, G, o.h->rptr(), H, T > 1 ? 1.f : beta, p, dt, d.w_hh->dtype);
+          for (int64_t k = 0; k < D; ++k) {
+            void* pk = at(p, k * G * H, d.w_hh->dtype);
+            const void* dG = at(dH, k * T * NG, dt);
+            // direction 0 runs forward: step t >= 1 follows output row t-1; direction 1 runs backward: step t <= T-2
+            // follows output row t+1, columns [H, 2H); the first step of each follows its initial state
+            if (T > 1)
+              gemm(ctx, true, false, G, H, (T - 1) * N, k ? dG : at(dG, NG, dt), G, k ? at(y, N * ldy + H, dt) : y, ldy,
+                   beta, pk, dt, d.w_hh->dtype);
+            gemm(ctx, true, false, G, H, N, k ? at(dG, (T - 1) * NG, dt) : dG, G, at(o.h->rptr(), k * NH, dt), H,
+                 T > 1 ? 1.f : beta, pk, dt, d.w_hh->dtype);
+          }
         });
         weight_done(d.w_hh);
       }
-      if (d.w_ih) {   // dW_ih += dG^T.X (TN, K = T*N)
+      if (d.w_ih) {   // dW_ih += dG^T.X (TN, K = T*N), per direction
         accumulate(ctx, d.w_ih, [&](void* p, float beta) {
-          gemm(ctx, true, false, G, I, T * N, dI, G, o.x->rptr(), I, beta, p, dt, d.w_ih->dtype);
+          for (int64_t k = 0; k < D; ++k)
+            gemm(ctx, true, false, G, I, T * N, at(dI, k * T * NG, dt), G, o.x->rptr(), I, beta, at(p, k * G * I, d.w_ih->dtype),
+                 dt, d.w_ih->dtype);
         });
         weight_done(d.w_ih);
       }
-      bias(d.b_ih, dI, G, T * N, dt);
-      bias(d.b_hh, dH, G, T * N, dt);
-      if (d.x) {      // dX += dG.W_ih (NN over T*N rows)
+      bias(d.b_ih, dI, G, T * N, dt, D);
+      bias(d.b_hh, dH, G, T * N, dt, D);
+      if (d.x) {      // dX += sum over directions of dG.W_ih (NN over T*N rows)
         accumulate(ctx, d.x, [&](void* p, float beta) {
-          gemm(ctx, false, false, T * N, I, G, dI, G, o.w_ih->rptr(), I, beta, p, dt, d.x->dtype);
+          for (int64_t k = 0; k < D; ++k)
+            gemm(ctx, false, false, T * N, I, G, at(dI, k * T * NG, dt), G, at(o.w_ih->rptr(), k * G * I, dt), I,
+                 k ? 1.f : beta, p, dt, d.x->dtype);
         });
         grad_written(d.x);
       }
-      state(d.h, static_cast<const float*>(dh_rec), N, H);
-      state(d.c, static_cast<const float*>(dc), N, H);
+      state(d.h, static_cast<const float*>(dh_rec), D * N, H);
+      state(d.c, static_cast<const float*>(dc), D * N, H);
     } catch (...) {
       release();
       throw;
@@ -1506,10 +1621,12 @@ struct RnnSeqBackward : Backward {  // `gradient` is the output's, (T, N, H); c_
   void no_grad() override {
     Backward::no_grad();
     if (c_last_grad) c_last_grad->no_grad();
+    if (h_n_grad) h_n_grad->no_grad();
   }
   void with_grad() override {
     Backward::with_grad();
     if (c_last_grad) c_last_grad->with_grad();
+    if (h_n_grad) h_n_grad->with_grad();
   }
 };
 
@@ -2379,13 +2496,11 @@ int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out) {
 }
 
 // The operand checks of a cell step (`seq` false: input (N, I)) and of a sequence layer (`seq` true: input (T, N, I),
-// T >= 1).  Returns the operands in History::merge order.
-struct RnnDims {
-  int64_t T, N, I, H;
-};
+// T >= 1; `layer`: states (D, N, H) and parameters stacked over D = 1 or 2 directions).  Returns the operands in
+// History::merge order.
 static std::vector<nkg_var*> check_rnn_operands(const char* who, bool lstm, bool seq, nkg_var* x, nkg_var* c, nkg_var* h,
                                                 nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih, nkg_var* b_hh,
-                                                bool outputs_given, RnnDims& dims) {
+                                                bool outputs_given, RnnDims& dims, bool layer = false) {
   struct Arg {
     nkg_var* v;
     const char* name;
@@ -2414,11 +2529,17 @@ static std::vector<nkg_var*> check_rnn_operands(const char* who, bool lstm, bool
   if (seq && xs[0] < 1) fail(NK_ERR_INVALID_ARG, "%s: input needs at least one time step, got %s", who, shape_str(xs).c_str());
   const Shape& hs = h->data->shape;
   const int64_t N = xs[seq ? 1 : 0], I = xs[seq ? 2 : 1];
-  if (hs.size() != 2 || hs[0] != N)
+  if (layer) {
+    if (hs.size() != 3 || (hs[0] != 1 && hs[0] != 2) || hs[1] != N)
+      fail(NK_ERR_INVALID_ARG, "%s: hidden must be (num_directions = 1 or 2, batch = %lld, hidden_size), got %s", who,
+           (long long)N, shape_str(hs).c_str());
+  } else if (hs.size() != 2 || hs[0] != N) {
     fail(NK_ERR_INVALID_ARG, "%s: hidden must be (batch = %lld, hidden_size), got %s", who, (long long)N,
          shape_str(hs).c_str());
-  const int64_t H = hs[1];
-  auto expect = [&](nkg_var* v, const char* name, const Shape& want) {
+  }
+  const int64_t D = layer ? hs[0] : 1, H = hs.back();
+  auto expect = [&](nkg_var* v, const char* name, Shape want) {
+    if (layer) want.insert(want.begin(), D);
     if (v->data->shape != want)
       fail(NK_ERR_INVALID_ARG, "%s: %s must be %s, got %s", who, name, shape_str(want).c_str(),
            shape_str(v->data->shape).c_str());
@@ -2428,7 +2549,7 @@ static std::vector<nkg_var*> check_rnn_operands(const char* who, bool lstm, bool
   expect(w_hh, "weight_hh", {G * H, H});
   expect(b_ih, "bias_ih", {G * H});
   expect(b_hh, "bias_hh", {G * H});
-  dims = {seq ? xs[0] : 1, N, I, H};
+  dims = {seq ? xs[0] : 1, N, I, H, D};
   std::vector<nkg_var*> operands;   // History::merge over every operand
   for (const Arg& a : args) operands.push_back(a.v);
   return operands;
@@ -2478,20 +2599,21 @@ int nkg_gru_cell(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* w
   return guard([&] { cell_impl(false, input, nullptr, hidden, weight_ih, weight_hh, bias_ih, bias_hh, nullptr, new_hidden); });
 }
 
-static void seq_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih,
-                     nkg_var* b_hh, nkg_var** output, nkg_var** last_c) {
-  const char* who = lstm ? "lstm" : "gru";
+// `layer` (nkg_lstm_layer / nkg_gru_layer): states (D, N, H), stacked parameters, and the last hidden state as an output
+static void seq_impl(bool lstm, bool layer, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_ih, nkg_var* w_hh, nkg_var* b_ih,
+                     nkg_var* b_hh, nkg_var** output, nkg_var** last_h, nkg_var** last_c) {
+  const char* who = layer ? (lstm ? "lstm_layer" : "gru_layer") : (lstm ? "lstm" : "gru");
   RnnDims dm;
-  const std::vector<nkg_var*> operands =
-      check_rnn_operands(who, lstm, true, x, c, h, w_ih, w_hh, b_ih, b_hh, output && (!lstm || last_c), dm);
+  const std::vector<nkg_var*> operands = check_rnn_operands(
+      who, lstm, true, x, c, h, w_ih, w_hh, b_ih, b_hh, output && (!layer || last_h) && (!lstm || last_c), dm, layer);
   std::shared_ptr<RnnSeq> seq;
   std::shared_ptr<RnnSeqBackward> seq_bwd;
   nkg_var* vy = record(
-      operands, Shape{dm.T, dm.N, dm.H}, x->data->dtype,
+      operands, Shape{dm.T, dm.N, dm.D * dm.H}, x->data->dtype,
       [&](const TensorP& d) {
         seq = std::make_shared<RnnSeq>(
-            x->ctx, lstm, CellOperands{x->data, h->data, lstm ? c->data : nullptr, w_ih->data, w_hh->data, b_ih->data, b_hh->data},
-            d);
+            x->ctx, lstm, layer, dm,
+            CellOperands{x->data, h->data, lstm ? c->data : nullptr, w_ih->data, w_hh->data, b_ih->data, b_hh->data}, d);
         return seq;
       },
       [&](const TensorP&, const GradientP& g) {
@@ -2506,19 +2628,43 @@ static void seq_impl(bool lstm, nkg_var* x, nkg_var* c, nkg_var* h, nkg_var* w_i
     if (seq_bwd) vc->grad = seq_bwd->c_last_grad;
     *last_c = vc;
   }
+  if (layer) {
+    nkg_var* vh = new nkg_var(*vy);
+    vh->data = seq->h_n;
+    if (seq_bwd) vh->grad = seq_bwd->h_n_grad;
+    *last_h = vh;
+  }
   *output = vy;
 }
 
 int nkg_lstm(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
              nkg_var* bias_hh, nkg_var** output, nkg_var** last_cell_state) {
   return guard([&] {
-    seq_impl(true, input, cell_state, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, last_cell_state);
+    seq_impl(true, false, input, cell_state, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, nullptr,
+             last_cell_state);
   });
 }
 
 int nkg_gru(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih, nkg_var* bias_hh,
             nkg_var** output) {
-  return guard([&] { seq_impl(false, input, nullptr, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, nullptr); });
+  return guard([&] {
+    seq_impl(false, false, input, nullptr, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, nullptr, nullptr);
+  });
+}
+
+int nkg_lstm_layer(nkg_var* input, nkg_var* cell_state, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh,
+                   nkg_var* bias_ih, nkg_var* bias_hh, nkg_var** output, nkg_var** last_hidden, nkg_var** last_cell_state) {
+  return guard([&] {
+    seq_impl(true, true, input, cell_state, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, last_hidden,
+             last_cell_state);
+  });
+}
+
+int nkg_gru_layer(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* weight_hh, nkg_var* bias_ih,
+                  nkg_var* bias_hh, nkg_var** output, nkg_var** last_hidden) {
+  return guard([&] {
+    seq_impl(false, true, input, nullptr, hidden, weight_ih, weight_hh, bias_ih, bias_hh, output, last_hidden, nullptr);
+  });
 }
 
 // ---------------------------------------------------------------- optimizers on a leaf (neuronika-optim)

@@ -13,6 +13,9 @@
 //                            LSTM / GRU sequence node (nk_graph.cpp, RnnSeqBackward).  The gradient carried from step to
 //                            step (dc, and the recurrent part of dh) stays in f32 whatever the element type and is updated
 //                            in place, so a bf16 sequence rounds it once at the end instead of once per step.
+//   two directions           nk_{lstm,gru}_bidir_{fwd,bwd}_step: one time step of both directions of a bidirectional
+//                            layer in one launch (blockIdx.y = direction), each direction's operands a given distance apart.
+// All of them share the per-unit gate maths below (lstm_fwd_unit, lstm_bwd_unit, gru_fwd_unit, gru_bwd_unit).
 #include "nk_internal.cuh"
 
 // a named namespace: the kernels keep the same symbol names from build to build (profiler traces, torch.profiler)
@@ -30,6 +33,46 @@ static inline int rnn_blocks(nk_ctx* ctx, size_t work_items) {
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
+
+// The gate maths of one hidden unit, shared by the cell, sequence-step and two-direction step kernels.
+// LSTM forward: the new cell state cn and hidden state hn from the gate pre-activations and the previous cell state c.
+__device__ __forceinline__ void lstm_fwd_unit(float gi, float gf, float gg, float go, float c, float& cn, float& hn) {
+  cn = sigm(gf) * c + sigm(gi) * tanhf(gg);
+  hn = sigm(go) * tanhf(cn);
+}
+// LSTM backward: the gate pre-activations are replaced by their gradients, given the hidden-state gradient dh and the
+// cell-state gradient dc that reach this step; returns sigmoid(f)*dc_total, the part of the previous cell state's gradient
+__device__ __forceinline__ float lstm_bwd_unit(float& gi, float& gf, float& gg, float& go, float c, float dh, float dc) {
+  const float i = sigm(gi), f = sigm(gf), g = tanhf(gg), o = sigm(go);
+  const float tc = tanhf(f * c + i * g);
+  const float dct = dc + dh * o * (1.f - tc * tc);
+  gi = dct * g * i * (1.f - i);
+  gf = dct * c * f * (1.f - f);
+  gg = dct * i * (1.f - g * g);
+  go = dh * tc * o * (1.f - o);
+  return f * dct;
+}
+// GRU forward: the new hidden state from both gate pre-activations and the previous hidden state h
+__device__ __forceinline__ float gru_fwd_unit(float ir, float iz, float in, float hr, float hz, float hn, float h) {
+  const float r = sigm(ir + hr), z = sigm(iz + hz);
+  const float nn = tanhf(in + r * hn);
+  return (h - nn) * z + nn;
+}
+// GRU backward: ir, iz, in become d(i_r) = d(h_r), d(i_z) = d(h_z), d(i_n) and hn becomes d(h_n); returns z*dh, the
+// pointwise part of the previous hidden state's gradient
+__device__ __forceinline__ float gru_bwd_unit(float& ir, float& iz, float& in, float hr, float hz, float& hn, float h,
+                                              float dh) {
+  const float r = sigm(ir + hr), z = sigm(iz + hz);
+  const float nn = tanhf(in + r * hn);
+  const float dpn = dh * (1.f - z) * (1.f - nn * nn);
+  const float dpz = dh * (h - nn) * z * (1.f - z);
+  const float dpr = dpn * hn * r * (1.f - r);
+  ir = dpr;
+  iz = dpz;
+  in = dpn;
+  hn = dpn * r;
+  return z * dh;
+}
 
 // V elements of T at p (16 / 8 byte vector accesses when V * sizeof(T) allows it; the caller guarantees alignment)
 template <typename T, int V>
@@ -91,11 +134,7 @@ __global__ void __launch_bounds__(kThreads) nk_lstm_cell_fwd_kernel(T* __restric
     ldv<float, V>(go, g + 3 * H);
     ldv<T, V>(c, c_prev + row * H + j);
 #pragma unroll
-    for (int k = 0; k < V; ++k) {
-      const float cn = sigm(gf[k]) * c[k] + sigm(gi[k]) * tanhf(gg[k]);
-      co[k] = cn;
-      ho[k] = sigm(go[k]) * tanhf(cn);
-    }
+    for (int k = 0; k < V; ++k) lstm_fwd_unit(gi[k], gf[k], gg[k], go[k], c[k], co[k], ho[k]);
     stv<T, V>(c_out + row * H + j, co);
     stv<T, V>(h_out + row * H + j, ho);
   }
@@ -126,15 +165,7 @@ __global__ void __launch_bounds__(kThreads) nk_lstm_cell_bwd_kernel(TG* __restri
     if (dc_prev && beta_dc != 0.f) ldv<T, V>(dcp, dc_prev + ss);
 #pragma unroll
     for (int k = 0; k < V; ++k) {
-      const float i = sigm(gi[k]), f = sigm(gf[k]), g = tanhf(gg[k]), o = sigm(go[k]);
-      const float tc = tanhf(f * c[k] + i * g);
-      const float dhk = dh_out ? dh[k] : 0.f;
-      const float dct = (dc_out ? dc[k] : 0.f) + dhk * o * (1.f - tc * tc);
-      gi[k] = dct * g * i * (1.f - i);
-      gf[k] = dct * c[k] * f * (1.f - f);
-      gg[k] = dct * i * (1.f - g * g);
-      go[k] = dhk * tc * o * (1.f - o);
-      float r = f * dct;
+      float r = lstm_bwd_unit(gi[k], gf[k], gg[k], go[k], c[k], dh_out ? dh[k] : 0.f, dc_out ? dc[k] : 0.f);
       if (dc_prev && beta_dc != 0.f) r += beta_dc * dcp[k];
       dcp[k] = r;
     }
@@ -172,17 +203,8 @@ __global__ void __launch_bounds__(kThreads) nk_lstm_seq_bwd_step_kernel(TG* __re
     if (dh_out) ldv<T, V>(dh, dh_out + ss);
     if (dh_rec) ldv<float, V>(dr, dh_rec + ss);
 #pragma unroll
-    for (int k = 0; k < V; ++k) {
-      const float i = sigm(gi[k]), f = sigm(gf[k]), g = tanhf(gg[k]), o = sigm(go[k]);
-      const float tc = tanhf(f * c[k] + i * g);
-      const float dhk = (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f);
-      const float dct = dcr[k] + dhk * o * (1.f - tc * tc);
-      gi[k] = dct * g * i * (1.f - i);
-      gf[k] = dct * c[k] * f * (1.f - f);
-      gg[k] = dct * i * (1.f - g * g);
-      go[k] = dhk * tc * o * (1.f - o);
-      dcr[k] = f * dct;
-    }
+    for (int k = 0; k < V; ++k)
+      dcr[k] = lstm_bwd_unit(gi[k], gf[k], gg[k], go[k], c[k], (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f), dcr[k]);
     stv<TG, V>(dgates + gs, gi);
     stv<TG, V>(dgates + gs + H, gf);
     stv<TG, V>(dgates + gs + 2 * H, gg);
@@ -212,11 +234,7 @@ __global__ void __launch_bounds__(kThreads) nk_gru_cell_fwd_kernel(T* __restrict
     ldv<float, V>(hn, hgates + gs + 2 * H);
     ldv<T, V>(h, h_prev + ss);
 #pragma unroll
-    for (int k = 0; k < V; ++k) {
-      const float r = sigm(ir[k] + hr[k]), z = sigm(iz[k] + hz[k]);
-      const float nn = tanhf(in[k] + r * hn[k]);
-      ho[k] = (h[k] - nn) * z + nn;
-    }
+    for (int k = 0; k < V; ++k) ho[k] = gru_fwd_unit(ir[k], iz[k], in[k], hr[k], hz[k], hn[k], h[k]);
     stv<T, V>(h_out + ss, ho);
   }
 }
@@ -248,16 +266,7 @@ __global__ void __launch_bounds__(kThreads) nk_gru_cell_bwd_kernel(TG* __restric
     if (dh_prev && beta_dh != 0.f) ldv<T, V>(dhp, dh_prev + ss);
 #pragma unroll
     for (int k = 0; k < V; ++k) {
-      const float r = sigm(ir[k] + hr[k]), z = sigm(iz[k] + hz[k]);
-      const float nn = tanhf(in[k] + r * hn[k]);
-      const float dpn = dh[k] * (1.f - z) * (1.f - nn * nn);
-      const float dpz = dh[k] * (h[k] - nn) * z * (1.f - z);
-      const float dpr = dpn * hn[k] * r * (1.f - r);
-      ir[k] = dpr;           // d(i_r) = d(h_r)
-      iz[k] = dpz;           // d(i_z) = d(h_z)
-      in[k] = dpn;           // d(i_n)
-      hn[k] = dpn * r;       // d(h_n)
-      float v = z * dh[k];
+      float v = gru_bwd_unit(ir[k], iz[k], in[k], hr[k], hz[k], hn[k], h[k], dh[k]);
       if (dh_prev && beta_dh != 0.f) v += beta_dh * dhp[k];
       dhp[k] = v;
     }
@@ -299,19 +308,153 @@ __global__ void __launch_bounds__(kThreads) nk_gru_seq_bwd_step_kernel(TG* __res
     if (dh_out) ldv<T, V>(dh, dh_out + ss);
     if (dh_rec) ldv<float, V>(dr, dh_rec + ss);
 #pragma unroll
-    for (int k = 0; k < V; ++k) {
-      const float r = sigm(ir[k] + hr[k]), z = sigm(iz[k] + hz[k]);
-      const float nn = tanhf(in[k] + r * hn[k]);
-      const float dhk = (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f);
-      const float dpn = dhk * (1.f - z) * (1.f - nn * nn);
-      const float dpz = dhk * (h[k] - nn) * z * (1.f - z);
-      const float dpr = dpn * hn[k] * r * (1.f - r);
-      ir[k] = dpr;           // d(i_r) = d(h_r)
-      iz[k] = dpz;           // d(i_z) = d(h_z)
-      in[k] = dpn;           // d(i_n)
-      hn[k] = dpn * r;       // d(h_n)
-      dr[k] = z * dhk;
-    }
+    for (int k = 0; k < V; ++k)
+      dr[k] = gru_bwd_unit(ir[k], iz[k], in[k], hr[k], hz[k], hn[k], h[k], (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f));
+    stv<TG, V>(digates + gs, ir);
+    stv<TG, V>(digates + gs + H, iz);
+    stv<TG, V>(digates + gs + 2 * H, in);
+    stv<TG, V>(dhgates + gs, ir);
+    stv<TG, V>(dhgates + gs + H, iz);
+    stv<TG, V>(dhgates + gs + 2 * H, hn);
+    if (dh_rec) stv<float, V>(dh_rec + ss, dr);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------- two directions
+// One time step of both directions of a bidirectional layer (nk_graph.cpp, RnnSeq with D = 2) in one launch:
+// blockIdx.y = d is the direction, and every per-direction operand of direction d starts d * <its _ds> elements after the
+// pointer passed (the graph passes the step's forward-direction slices and the distance to the reverse direction's).
+// The state buffers h_next, dc and dh_rec are (2, n, H), direction stride n*H.  Rows of y / dh_out / h_prev are ld apart.
+template <typename T, int V>
+__global__ void __launch_bounds__(kThreads) nk_lstm_bidir_fwd_step_kernel(T* __restrict__ y, int64_t y_ds, int64_t ldy,
+                                                                          T* __restrict__ h_next, T* __restrict__ c_out,
+                                                                          int64_t c_out_ds, const float* __restrict__ gates,
+                                                                          int64_t g_ds, const T* __restrict__ c_prev,
+                                                                          int64_t c_prev_ds, int64_t n, int64_t H) {
+  const int64_t d = blockIdx.y;
+  y += d * y_ds, h_next += d * n * H, c_out += d * c_out_ds, gates += d * g_ds, c_prev += d * c_prev_ds;
+  const int64_t per_row = H / V;
+  const size_t units = size_t(n) * size_t(per_row);
+  const size_t stride = size_t(gridDim.x) * blockDim.x;
+  for (size_t u = size_t(blockIdx.x) * blockDim.x + threadIdx.x; u < units; u += stride) {
+    const int64_t row = int64_t(u / size_t(per_row)), j = int64_t(u % size_t(per_row)) * V;
+    const float* g = gates + row * 4 * H + j;
+    float gi[V], gf[V], gg[V], go[V], c[V], co[V], ho[V];
+    ldv<float, V>(gi, g);
+    ldv<float, V>(gf, g + H);
+    ldv<float, V>(gg, g + 2 * H);
+    ldv<float, V>(go, g + 3 * H);
+    ldv<T, V>(c, c_prev + row * H + j);
+#pragma unroll
+    for (int k = 0; k < V; ++k) lstm_fwd_unit(gi[k], gf[k], gg[k], go[k], c[k], co[k], ho[k]);
+    stv<T, V>(c_out + row * H + j, co);
+    stv<T, V>(y + row * ldy + j, ho);
+    stv<T, V>(h_next + row * H + j, ho);
+  }
+}
+
+template <typename T, int V>
+__global__ void __launch_bounds__(kThreads) nk_gru_bidir_fwd_step_kernel(T* __restrict__ y, int64_t y_ds, int64_t ldy,
+                                                                         T* __restrict__ h_next,
+                                                                         const float* __restrict__ igates,
+                                                                         const float* __restrict__ hgates, int64_t g_ds,
+                                                                         const T* __restrict__ h_prev, int64_t h_prev_ds,
+                                                                         int64_t n, int64_t H) {
+  const int64_t d = blockIdx.y;
+  y += d * y_ds, h_next += d * n * H, igates += d * g_ds, hgates += d * g_ds, h_prev += d * h_prev_ds;
+  const int64_t per_row = H / V;
+  const size_t units = size_t(n) * size_t(per_row);
+  const size_t stride = size_t(gridDim.x) * blockDim.x;
+  for (size_t u = size_t(blockIdx.x) * blockDim.x + threadIdx.x; u < units; u += stride) {
+    const int64_t row = int64_t(u / size_t(per_row)), j = int64_t(u % size_t(per_row)) * V;
+    const int64_t gs = row * 3 * H + j;
+    float ir[V], iz[V], in[V], hr[V], hz[V], hn[V], h[V], ho[V];
+    ldv<float, V>(ir, igates + gs);
+    ldv<float, V>(iz, igates + gs + H);
+    ldv<float, V>(in, igates + gs + 2 * H);
+    ldv<float, V>(hr, hgates + gs);
+    ldv<float, V>(hz, hgates + gs + H);
+    ldv<float, V>(hn, hgates + gs + 2 * H);
+    ldv<T, V>(h, h_prev + row * H + j);
+#pragma unroll
+    for (int k = 0; k < V; ++k) ho[k] = gru_fwd_unit(ir[k], iz[k], in[k], hr[k], hz[k], hn[k], h[k]);
+    stv<T, V>(y + row * ldy + j, ho);
+    stv<T, V>(h_next + row * H + j, ho);
+  }
+}
+
+// dgates share the gates' layout (direction distance g_ds); dc (f32) is read as dc_out and overwritten with dc_prev
+template <typename T, typename TG, int V>
+__global__ void __launch_bounds__(kThreads) nk_lstm_bidir_bwd_step_kernel(TG* __restrict__ dgates, int64_t g_ds,
+                                                                          float* __restrict__ dc,
+                                                                          const float* __restrict__ gates,
+                                                                          const T* __restrict__ c_prev, int64_t c_prev_ds,
+                                                                          const T* __restrict__ dh_out, int64_t dh_ds,
+                                                                          int64_t ld_dh, const float* __restrict__ dh_rec,
+                                                                          int64_t n, int64_t H) {
+  const int64_t d = blockIdx.y;
+  dgates += d * g_ds, gates += d * g_ds, dc += d * n * H, c_prev += d * c_prev_ds;
+  if (dh_out) dh_out += d * dh_ds;
+  if (dh_rec) dh_rec += d * n * H;
+  const int64_t per_row = H / V;
+  const size_t units = size_t(n) * size_t(per_row);
+  const size_t stride = size_t(gridDim.x) * blockDim.x;
+  for (size_t u = size_t(blockIdx.x) * blockDim.x + threadIdx.x; u < units; u += stride) {
+    const int64_t row = int64_t(u / size_t(per_row)), j = int64_t(u % size_t(per_row)) * V;
+    const int64_t gs = row * 4 * H + j, ss = row * H + j;
+    float gi[V], gf[V], gg[V], go[V], c[V], dh[V], dr[V], dcr[V];
+    ldv<float, V>(gi, gates + gs);
+    ldv<float, V>(gf, gates + gs + H);
+    ldv<float, V>(gg, gates + gs + 2 * H);
+    ldv<float, V>(go, gates + gs + 3 * H);
+    ldv<T, V>(c, c_prev + ss);
+    ldv<float, V>(dcr, dc + ss);
+    if (dh_out) ldv<T, V>(dh, dh_out + row * ld_dh + j);
+    if (dh_rec) ldv<float, V>(dr, dh_rec + ss);
+#pragma unroll
+    for (int k = 0; k < V; ++k)
+      dcr[k] = lstm_bwd_unit(gi[k], gf[k], gg[k], go[k], c[k], (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f), dcr[k]);
+    stv<TG, V>(dgates + gs, gi);
+    stv<TG, V>(dgates + gs + H, gf);
+    stv<TG, V>(dgates + gs + 2 * H, gg);
+    stv<TG, V>(dgates + gs + 3 * H, go);
+    stv<float, V>(dc + ss, dcr);
+  }
+}
+
+// dh_rec (f32) is read and overwritten with z*dh (the caller adds dhgates.W_hh)
+template <typename T, typename TG, int V>
+__global__ void __launch_bounds__(kThreads) nk_gru_bidir_bwd_step_kernel(TG* __restrict__ digates, TG* __restrict__ dhgates,
+                                                                         int64_t g_ds, float* __restrict__ dh_rec,
+                                                                         const float* __restrict__ igates,
+                                                                         const float* __restrict__ hgates,
+                                                                         const T* __restrict__ h_prev, int64_t h_prev_ds,
+                                                                         int64_t ld_h, const T* __restrict__ dh_out,
+                                                                         int64_t dh_ds, int64_t ld_dh, int64_t n,
+                                                                         int64_t H) {
+  const int64_t d = blockIdx.y;
+  digates += d * g_ds, dhgates += d * g_ds, igates += d * g_ds, hgates += d * g_ds, h_prev += d * h_prev_ds;
+  if (dh_out) dh_out += d * dh_ds;
+  if (dh_rec) dh_rec += d * n * H;
+  const int64_t per_row = H / V;
+  const size_t units = size_t(n) * size_t(per_row);
+  const size_t stride = size_t(gridDim.x) * blockDim.x;
+  for (size_t u = size_t(blockIdx.x) * blockDim.x + threadIdx.x; u < units; u += stride) {
+    const int64_t row = int64_t(u / size_t(per_row)), j = int64_t(u % size_t(per_row)) * V;
+    const int64_t gs = row * 3 * H + j, ss = row * H + j;
+    float ir[V], iz[V], in[V], hr[V], hz[V], hn[V], h[V], dh[V], dr[V];
+    ldv<float, V>(ir, igates + gs);
+    ldv<float, V>(iz, igates + gs + H);
+    ldv<float, V>(in, igates + gs + 2 * H);
+    ldv<float, V>(hr, hgates + gs);
+    ldv<float, V>(hz, hgates + gs + H);
+    ldv<float, V>(hn, hgates + gs + 2 * H);
+    ldv<T, V>(h, h_prev + row * ld_h + j);
+    if (dh_out) ldv<T, V>(dh, dh_out + row * ld_dh + j);
+    if (dh_rec) ldv<float, V>(dr, dh_rec + ss);
+#pragma unroll
+    for (int k = 0; k < V; ++k)
+      dr[k] = gru_bwd_unit(ir[k], iz[k], in[k], hr[k], hz[k], hn[k], h[k], (dh_out ? dh[k] : 0.f) + (dh_rec ? dr[k] : 0.f));
     stv<TG, V>(digates + gs, ir);
     stv<TG, V>(digates + gs + H, iz);
     stv<TG, V>(digates + gs + 2 * H, in);
@@ -390,6 +533,10 @@ static int chunk_dims(nk_ctx* ctx, ChunkDims& d, int ndim, const int64_t* x_shap
   for (int k = ndim; k < NK_MAX_DIMS; ++k) d.cshape[k] = 1, d.xstride[k] = 0;
   return NK_OK;
 }
+
+// the vector bodies need 16-byte aligned bases and every stride (ld, direction distance) a multiple of 16 bytes
+static inline bool bytes16(int64_t elems, size_t esize) { return (elems * int64_t(esize)) % 16 == 0; }
+static inline dim3 bidir_grid(nk_ctx* ctx, size_t units) { return dim3(unsigned(rnn_blocks(ctx, units)), 2u); }
 
 static int cell_args(nk_ctx* ctx, const char* who, int64_t n, int64_t hidden, int dtype) {
   NK_REQUIRE(ctx, n >= 0 && hidden >= 0, "%s: negative size", who);
@@ -549,6 +696,127 @@ int nk_gru_seq_bwd_step(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype,
     });
   });
   NK_LAUNCHED(ctx, "gru_seq_bwd_step");
+  return NK_OK;
+}
+
+int nk_lstm_bidir_fwd_step(nk_ctx* ctx, void* y, int64_t y_dstride, int64_t ldy, void* h_next, void* c_out,
+                           int64_t c_out_dstride, const float* gates, int64_t gates_dstride, const void* c_prev,
+                           int64_t c_prev_dstride, int64_t n, int64_t hidden, int dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  if (int rc = cell_args(ctx, "nk_lstm_bidir_fwd_step", n, hidden, dtype)) return rc;
+  NK_REQUIRE(ctx, ldy >= hidden, "nk_lstm_bidir_fwd_step: ldy %lld < hidden %lld", (long long)ldy, (long long)hidden);
+  if (n == 0 || hidden == 0) return NK_OK;
+  NK_REQUIRE(ctx, y && h_next && c_out && gates && c_prev, "nk_lstm_bidir_fwd_step: NULL pointer");
+  NK_DISPATCH_DTYPE(dtype, T, {
+    constexpr int V = NkVec<T>::N;
+    const size_t es = sizeof(T);
+    const bool vec = hidden % V == 0 && aligned16(y) && aligned16(h_next) && aligned16(c_out) && aligned16(gates) &&
+                     aligned16(c_prev) && bytes16(y_dstride, es) && bytes16(ldy, es) && bytes16(c_out_dstride, es) &&
+                     bytes16(gates_dstride, 4) && bytes16(c_prev_dstride, es);
+    const int64_t units = n * (vec ? hidden / V : hidden);
+    if (vec)
+      nk_lstm_bidir_fwd_step_kernel<T, V><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+          (T*)y, y_dstride, ldy, (T*)h_next, (T*)c_out, c_out_dstride, gates, gates_dstride, (const T*)c_prev,
+          c_prev_dstride, n, hidden);
+    else
+      nk_lstm_bidir_fwd_step_kernel<T, 1><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+          (T*)y, y_dstride, ldy, (T*)h_next, (T*)c_out, c_out_dstride, gates, gates_dstride, (const T*)c_prev,
+          c_prev_dstride, n, hidden);
+  });
+  NK_LAUNCHED(ctx, "lstm_bidir_fwd_step");
+  return NK_OK;
+}
+
+int nk_gru_bidir_fwd_step(nk_ctx* ctx, void* y, int64_t y_dstride, int64_t ldy, void* h_next, const float* igates,
+                          const float* hgates, int64_t gates_dstride, const void* h_prev, int64_t h_prev_dstride, int64_t n,
+                          int64_t hidden, int dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  if (int rc = cell_args(ctx, "nk_gru_bidir_fwd_step", n, hidden, dtype)) return rc;
+  NK_REQUIRE(ctx, ldy >= hidden, "nk_gru_bidir_fwd_step: ldy %lld < hidden %lld", (long long)ldy, (long long)hidden);
+  if (n == 0 || hidden == 0) return NK_OK;
+  NK_REQUIRE(ctx, y && h_next && igates && hgates && h_prev, "nk_gru_bidir_fwd_step: NULL pointer");
+  NK_DISPATCH_DTYPE(dtype, T, {
+    constexpr int V = NkVec<T>::N;
+    const size_t es = sizeof(T);
+    const bool vec = hidden % V == 0 && aligned16(y) && aligned16(h_next) && aligned16(igates) && aligned16(hgates) &&
+                     aligned16(h_prev) && bytes16(y_dstride, es) && bytes16(ldy, es) && bytes16(gates_dstride, 4) &&
+                     bytes16(h_prev_dstride, es);
+    const int64_t units = n * (vec ? hidden / V : hidden);
+    if (vec)
+      nk_gru_bidir_fwd_step_kernel<T, V><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+          (T*)y, y_dstride, ldy, (T*)h_next, igates, hgates, gates_dstride, (const T*)h_prev, h_prev_dstride, n, hidden);
+    else
+      nk_gru_bidir_fwd_step_kernel<T, 1><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+          (T*)y, y_dstride, ldy, (T*)h_next, igates, hgates, gates_dstride, (const T*)h_prev, h_prev_dstride, n, hidden);
+  });
+  NK_LAUNCHED(ctx, "gru_bidir_fwd_step");
+  return NK_OK;
+}
+
+int nk_lstm_bidir_bwd_step(nk_ctx* ctx, void* dgates, int dgates_dtype, int64_t gates_dstride, float* dc, const float* gates,
+                           const void* c_prev, int64_t c_prev_dstride, const void* dh_out, int64_t dh_out_dstride,
+                           int64_t ld_dh_out, const float* dh_rec, int64_t n, int64_t hidden, int dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  if (int rc = cell_args(ctx, "nk_lstm_bidir_bwd_step", n, hidden, dtype)) return rc;
+  NK_REQUIRE(ctx, nk_dtype_ok(dgates_dtype), "nk_lstm_bidir_bwd_step: bad dgates dtype %d", dgates_dtype);
+  NK_REQUIRE(ctx, !dh_out || ld_dh_out >= hidden, "nk_lstm_bidir_bwd_step: ld_dh_out %lld < hidden %lld",
+             (long long)ld_dh_out, (long long)hidden);
+  if (n == 0 || hidden == 0) return NK_OK;
+  NK_REQUIRE(ctx, dgates && dc && gates && c_prev, "nk_lstm_bidir_bwd_step: NULL pointer");
+  NK_DISPATCH_DTYPE(dtype, T, {
+    NK_DISPATCH_DTYPE(dgates_dtype, TG, {
+      constexpr int V = NkVec<T>::N;
+      const size_t es = sizeof(T);
+      const bool vec = hidden % V == 0 && aligned16(dgates) && aligned16(dc) && aligned16(gates) && aligned16(c_prev) &&
+                       bytes16(gates_dstride, sizeof(TG)) && bytes16(gates_dstride, 4) && bytes16(c_prev_dstride, es) &&
+                       (!dh_out || (aligned16(dh_out) && bytes16(dh_out_dstride, es) && bytes16(ld_dh_out, es))) &&
+                       (!dh_rec || aligned16(dh_rec));
+      const int64_t units = n * (vec ? hidden / V : hidden);
+      if (vec)
+        nk_lstm_bidir_bwd_step_kernel<T, TG, V><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)dgates, gates_dstride, dc, gates, (const T*)c_prev, c_prev_dstride, (const T*)dh_out, dh_out_dstride,
+            ld_dh_out, dh_rec, n, hidden);
+      else
+        nk_lstm_bidir_bwd_step_kernel<T, TG, 1><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)dgates, gates_dstride, dc, gates, (const T*)c_prev, c_prev_dstride, (const T*)dh_out, dh_out_dstride,
+            ld_dh_out, dh_rec, n, hidden);
+    });
+  });
+  NK_LAUNCHED(ctx, "lstm_bidir_bwd_step");
+  return NK_OK;
+}
+
+int nk_gru_bidir_bwd_step(nk_ctx* ctx, void* digates, void* dhgates, int dg_dtype, int64_t gates_dstride, float* dh_rec,
+                          const float* igates, const float* hgates, const void* h_prev, int64_t h_prev_dstride, int64_t ld_h_prev,
+                          const void* dh_out, int64_t dh_out_dstride, int64_t ld_dh_out, int64_t n, int64_t hidden,
+                          int dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  if (int rc = cell_args(ctx, "nk_gru_bidir_bwd_step", n, hidden, dtype)) return rc;
+  NK_REQUIRE(ctx, nk_dtype_ok(dg_dtype), "nk_gru_bidir_bwd_step: bad dgates dtype %d", dg_dtype);
+  NK_REQUIRE(ctx, ld_h_prev >= hidden && (!dh_out || ld_dh_out >= hidden), "nk_gru_bidir_bwd_step: leading dimension too small");
+  if (n == 0 || hidden == 0) return NK_OK;
+  NK_REQUIRE(ctx, digates && dhgates && igates && hgates && h_prev, "nk_gru_bidir_bwd_step: NULL pointer");
+  NK_DISPATCH_DTYPE(dtype, T, {
+    NK_DISPATCH_DTYPE(dg_dtype, TG, {
+      constexpr int V = NkVec<T>::N;
+      const size_t es = sizeof(T);
+      const bool vec = hidden % V == 0 && aligned16(digates) && aligned16(dhgates) && aligned16(igates) &&
+                       aligned16(hgates) && aligned16(h_prev) && bytes16(gates_dstride, sizeof(TG)) &&
+                       bytes16(gates_dstride, 4) && bytes16(h_prev_dstride, es) && bytes16(ld_h_prev, es) &&
+                       (!dh_out || (aligned16(dh_out) && bytes16(dh_out_dstride, es) && bytes16(ld_dh_out, es))) &&
+                       (!dh_rec || aligned16(dh_rec));
+      const int64_t units = n * (vec ? hidden / V : hidden);
+      if (vec)
+        nk_gru_bidir_bwd_step_kernel<T, TG, V><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)digates, (TG*)dhgates, gates_dstride, dh_rec, igates, hgates, (const T*)h_prev, h_prev_dstride, ld_h_prev,
+            (const T*)dh_out, dh_out_dstride, ld_dh_out, n, hidden);
+      else
+        nk_gru_bidir_bwd_step_kernel<T, TG, 1><<<bidir_grid(ctx, units), kThreads, 0, ctx->stream>>>(
+            (TG*)digates, (TG*)dhgates, gates_dstride, dh_rec, igates, hgates, (const T*)h_prev, h_prev_dstride, ld_h_prev,
+            (const T*)dh_out, dh_out_dstride, ld_dh_out, n, hidden);
+    });
+  });
+  NK_LAUNCHED(ctx, "gru_bidir_bwd_step");
   return NK_OK;
 }
 

@@ -1,5 +1,5 @@
 """Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell and Conv2d (neuronika-nn/src/lib.rs:406-626, 724-815),
-and the sequence layers LSTM and GRU over them."""
+and the sequence layers LSTM and GRU over them (stacked and bidirectional like torch.nn.LSTM / GRU)."""
 from __future__ import annotations
 
 import math
@@ -96,17 +96,110 @@ class LSTMCell:
         return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]
 
 
-class LSTM(LSTMCell):
-    """The LSTMCell applied to a whole time-major sequence as one graph node (variable.lstm): same parameters and
-    initialisation as the cell, so a layer built from the same `rng` seed holds the same weights.  One layer, one
-    direction."""
+class _Stacked:
+    """`num_layers` layers of one or two directions, one graph node per layer (variable.lstm_layer / gru_layer).
+
+    Layer k holds weight_ih_l{k} (D, G, I_k), weight_hh_l{k} (D, G, H), bias_ih_l{k} and bias_hh_l{k} (D, G), stacked
+    over the D directions (index 1 = torch's `_reverse` parameters); I_0 = input_size and I_k = D*H above.  All are
+    ~ U(-k, k), k = 1/sqrt(hidden_size), drawn from `rng` layer by layer, direction by direction, in the order weight_ih,
+    weight_hh, bias_ih, bias_hh.  Torch weights port as `np.stack([w_l0, w_l0_reverse])` (or `w_l0[None]` for one
+    direction): e.g. `weight_ih_l0 = np.stack([m.weight_ih_l0, m.weight_ih_l0_reverse])`.
+    `dropout` > 0 applies Var.dropout to every layer's output but the last, while the module is in training mode
+    (`train()`, the initial mode; `eval()` turns it off)."""
+
+    num_layers, bidirectional, dropout = 1, False, 0.0
+    _stacked = False   # the default configuration keeps the cell's parameters and results
+
+    def _init_stacked(self, device, input_size, hidden_size, gates, dtype, grad_dtype, rng, num_layers, bidirectional,
+                      dropout):
+        if num_layers < 1:
+            raise ValueError(f"num_layers must be at least 1, got {num_layers}")
+        if not 0.0 <= dropout <= 1.0:
+            raise ValueError(f"Wrong probability received: {dropout}.")
+        self._stacked = True
+        self.num_layers, self.bidirectional, self.dropout = int(num_layers), bool(bidirectional), float(dropout)
+        self.hidden_size = int(hidden_size)
+        self.status = V.Status(True)
+        rng = rng or np.random.default_rng()
+        k = 1.0 / math.sqrt(hidden_size)
+        g, dirs = gates * hidden_size, 2 if bidirectional else 1
+        for layer in range(self.num_layers):
+            isz = input_size if layer == 0 else dirs * hidden_size
+            drawn = [[], [], [], []]
+            for _ in range(dirs):
+                for i, shape in enumerate(((g, isz), (g, hidden_size), (g,), (g,))):
+                    drawn[i].append(uniform(rng, shape, -k, k))
+            for name, arrays in zip(self._names, drawn):
+                setattr(self, f"{name}_l{layer}",
+                        V.from_ndarray(device, np.stack(arrays), dtype).requires_grad(grad_dtype))
+
+    _names = ("weight_ih", "weight_hh", "bias_ih", "bias_hh")
+
+    def _layer_params(self, layer):
+        return [getattr(self, f"{name}_l{layer}") for name in self._names]
+
+    def _run_stacked(self, layer_fn, states, input: V.Var):
+        """`states`: the (num_layers*D, N, H) initial states, split per layer with one chunks node; returns (output,
+        *last states), the last states of all layers joined with one cat node each."""
+        dirs = 2 if self.bidirectional else 1
+        if self.num_layers > 1:
+            per_layer = [s.chunks((dirs,) + tuple(s.shape[1:])) for s in states]
+        else:
+            per_layer = [[s] for s in states]
+        x, lasts = input, []
+        for layer in range(self.num_layers):
+            y, *last = layer_fn(x, [p[layer] for p in per_layer], self._layer_params(layer))
+            if self.dropout > 0.0 and layer < self.num_layers - 1:
+                y = y.dropout(self.dropout, self.status)
+            x = y
+            lasts.append(last)
+        joined = [ls[0] if len(ls) == 1 else ls[0].cat(ls[1:], 0) for ls in zip(*lasts)]
+        return (x, *joined)
+
+    def _stacked_parameters(self):
+        return [p for layer in range(self.num_layers) for p in self._layer_params(layer)]
+
+    def train(self) -> None:
+        """Dropout between the layers on (the initial mode)."""
+        if self._stacked:
+            self.status.train()
+
+    def eval(self) -> None:
+        """Dropout between the layers off."""
+        if self._stacked:
+            self.status.eval()
+
+
+class LSTM(_Stacked, LSTMCell):
+    """torch.nn.LSTM over a whole time-major sequence, one graph node per layer.
+
+    With the defaults (one layer, one direction, no dropout) it is the LSTMCell applied to every step (variable.lstm):
+    the cell's parameters weight_ih (4H, I), weight_hh, bias_ih, bias_hh and initialisation, so a layer built from the
+    same `rng` seed holds the same weights.  With `num_layers` > 1 or `bidirectional` it holds the stacked parameters of
+    `_Stacked` (weight_ih_l0 (D, 4H, I), ...) and takes and returns states shaped like torch's, (num_layers*D, N, H)."""
+
+    def __init__(self, device: Device, input_size: int, hidden_size: int, dtype=F32, grad_dtype=None,
+                 rng: np.random.Generator | None = None, num_layers: int = 1, bidirectional: bool = False,
+                 dropout: float = 0.0):
+        if num_layers == 1 and not bidirectional and dropout == 0.0:
+            super().__init__(device, input_size, hidden_size, dtype, grad_dtype, rng)
+        else:
+            self._init_stacked(device, input_size, hidden_size, 4, dtype, grad_dtype, rng, num_layers, bidirectional,
+                               dropout)
 
     def forward(self, state, input: V.Var):
-        """`state = (cell_state, hidden)`, both (batch, hidden_size); `input` (seq_len, batch, input_size).  Returns
-        (output, cell_T): every step's hidden state (seq_len, batch, hidden_size), whose last slice is the last hidden
-        state, and the last cell state."""
+        """`state = (cell_state, hidden)`; `input` (seq_len, batch, input_size).  With the defaults the states are
+        (batch, hidden_size) and the result is (output, cell_T): every step's hidden state (seq_len, batch,
+        hidden_size), whose last slice is the last hidden state, and the last cell state.  Otherwise the states are
+        (num_layers*D, batch, hidden_size) and the result is (output, h_n, c_n) as torch.nn.LSTM returns it: output
+        (seq_len, batch, D*hidden_size) of the last layer, and every layer's and direction's last states."""
         cell_state, hidden = state
-        return V.lstm(input, cell_state, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+        if not self._stacked:
+            return V.lstm(input, cell_state, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+        return self._run_stacked(lambda x, st, p: V.lstm_layer(x, st[0], st[1], *p), [cell_state, hidden], input)
+
+    def parameters(self):
+        return self._stacked_parameters() if self._stacked else super().parameters()
 
 
 class Dropout:
@@ -155,11 +248,27 @@ class GRUCell:
         return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]
 
 
-class GRU(GRUCell):
-    """The GRUCell applied to a whole time-major sequence as one graph node (variable.gru): same parameters and
-    initialisation as the cell.  One layer, one direction."""
+class GRU(_Stacked, GRUCell):
+    """torch.nn.GRU over a whole time-major sequence, one graph node per layer.  With the defaults it is the GRUCell
+    applied to every step (variable.gru), with the cell's parameters and initialisation; otherwise it holds the stacked
+    parameters of `_Stacked` (weight_ih_l0 (D, 3H, I), ...)."""
+
+    def __init__(self, device: Device, input_size: int, hidden_size: int, dtype=F32, grad_dtype=None,
+                 rng: np.random.Generator | None = None, num_layers: int = 1, bidirectional: bool = False,
+                 dropout: float = 0.0):
+        if num_layers == 1 and not bidirectional and dropout == 0.0:
+            super().__init__(device, input_size, hidden_size, dtype, grad_dtype, rng)
+        else:
+            self._init_stacked(device, input_size, hidden_size, 3, dtype, grad_dtype, rng, num_layers, bidirectional,
+                               dropout)
 
     def forward(self, hidden: V.Var, input: V.Var):
-        """`hidden` (batch, hidden_size), `input` (seq_len, batch, input_size); returns every step's hidden state
-        (seq_len, batch, hidden_size)."""
-        return V.gru(input, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+        """`input` (seq_len, batch, input_size).  With the defaults `hidden` is (batch, hidden_size) and the result is
+        every step's hidden state (seq_len, batch, hidden_size).  Otherwise `hidden` is (num_layers*D, batch,
+        hidden_size) and the result is (output, h_n) as torch.nn.GRU returns it."""
+        if not self._stacked:
+            return V.gru(input, hidden, self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+        return self._run_stacked(lambda x, st, p: V.gru_layer(x, st[0], *p), [hidden], input)
+
+    def parameters(self):
+        return self._stacked_parameters() if self._stacked else super().parameters()

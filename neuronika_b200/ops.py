@@ -35,6 +35,21 @@ def gemm(a: CuArray, b: CuArray, c: CuArray, trans_a=False, trans_b=False, alpha
     return c
 
 
+def gemm_strided_batched(a: CuArray, b: CuArray, c: CuArray, m: int, n: int, k: int, batch: int, lda: int, ldb: int,
+                         ldc: int, stride_a: int, stride_b: int, stride_c: int, trans_a=False, trans_b=False, alpha=1.0,
+                         beta=0.0, bias: CuArray | None = None, bias_stride: int = 0) -> CuArray:
+    """`batch` products c_i = alpha*op(a_i).op(b_i) + beta*c_i + bias_i, where x_i starts stride_x elements after x_{i-1}
+    (the arrays' first elements are the first product's) and bias_i (n elements) bias_stride after bias_{i-1}."""
+    dev = a.device
+    if a.dtype != b.dtype:
+        raise ValueError("gemm_strided_batched: operand dtypes differ")
+    _ck(lib.nk_gemm_strided_batched(dev.ctx, int(trans_a), int(trans_b), m, n, k, float(alpha), a.ptr, lda, stride_a,
+                                    b.ptr, ldb, stride_b, float(beta), c.ptr, ldc, stride_c, batch, a.dtype, c.dtype,
+                                    bias.ptr if bias is not None else None, bias_stride,
+                                    bias.dtype if bias is not None else F32), dev)
+    return c
+
+
 def mm(a, b, out=None, out_dtype=None):
     out = out or CuArray(a.device, (a.shape[0], b.shape[1]), out_dtype if out_dtype is not None else a.dtype)
     return gemm(a, b, out)

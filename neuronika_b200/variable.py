@@ -83,6 +83,8 @@ _G = {
     "nkg_gru_cell": (i32, [vp, vp, vp, vp, vp, vp, pvp]),
     "nkg_lstm": (i32, [vp, vp, vp, vp, vp, vp, vp, pvp, pvp]),
     "nkg_gru": (i32, [vp, vp, vp, vp, vp, vp, pvp]),
+    "nkg_lstm_layer": (i32, [vp, vp, vp, vp, vp, vp, vp, pvp, pvp, pvp]),
+    "nkg_gru_layer": (i32, [vp, vp, vp, vp, vp, vp, pvp, pvp]),
     "nkg_cat": (i32, [pvp, i32, i32, pvp]),
     "nkg_stack": (i32, [pvp, i32, i32, pvp]),
     "nkg_unsqueeze": (i32, [vp, i32, pvp]),
@@ -454,6 +456,26 @@ def gru(input: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: Var, b
     y = vp()
     _ck(lib.nkg_gru(input._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h, C.byref(y)))
     return input._wrap(y)
+
+
+def lstm_layer(input: Var, cell_state: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: Var, bias_hh: Var):
+    """One layer of torch.nn.LSTM with D = 1 or 2 directions (D = hidden.shape[0]), as ONE node: `input` (T, N, I),
+    `cell_state` and `hidden` (D, N, H), the parameters stacked over the directions: weight_ih (D, 4H, I), weight_hh
+    (D, 4H, H), biases (D, 4H).  Returns (output, h_n, c_n): `output` (T, N, D*H), the reverse direction in columns
+    [H, 2H), and each direction's last hidden and cell state, (D, N, H)."""
+    y, h, c = vp(), vp(), vp()
+    _ck(lib.nkg_lstm_layer(input._h, cell_state._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h,
+                           C.byref(y), C.byref(h), C.byref(c)))
+    return input._wrap(y), input._wrap(h), input._wrap(c)
+
+
+def gru_layer(input: Var, hidden: Var, weight_ih: Var, weight_hh: Var, bias_ih: Var, bias_hh: Var):
+    """One layer of torch.nn.GRU with D = 1 or 2 directions, as ONE node; the operands as `lstm_layer` takes them (gates
+    3H).  Returns (output, h_n): `output` (T, N, D*H) and each direction's last hidden state (D, N, H)."""
+    y, h = vp(), vp()
+    _ck(lib.nkg_gru_layer(input._h, hidden._h, weight_ih._h, weight_hh._h, bias_ih._h, bias_hh._h, C.byref(y),
+                          C.byref(h)))
+    return input._wrap(y), input._wrap(h)
 
 
 # ---- constructors (neuronika-variable/src/lib.rs:51-240), on a device

@@ -20,9 +20,15 @@ Reported per configuration, in one JSON line each:
   - the sequence layer's GEMMs alone, in two groups: the products that run once over all T*N rows (x.W_ih^T + b, dW_ih,
     dW_hh) and the 2T sequential ones that stay N rows tall (h.W_hh^T + b forward, dG.W_hh backward), as ms per sequence
     and as shares of the sequence layer's step.
+Then one more JSON line per configuration ("stacked"): nn.LSTM / nn.GRU unidirectional, bidirectional and 2 layers x
+bidirectional on the same sequence (the loss on the last time step of the last layer's output), each beside
+torch.nn.LSTM / GRU(num_layers, bidirectional) in bf16 (cuDNN); the ratio bidirectional / (2 x unidirectional) (below 1:
+the two directions' batched step GEMM and step kernel cost less than two layers' worth) and the launches per time step.
+Each of these three captured steps reserves a 12 GiB capture arena (what the GRU's 2 layers x 2 directions at N = 1024
+need), 36 GiB of device memory in all while a row is measured: run it on a card that has that much free.
 Card name, power limit and the median SM clock during the timed windows (NVML) are printed beside the numbers.
 
-    python tools/rnn_bench.py [--reps 5] [--window-ms 200]
+    python tools/rnn_bench.py [--reps 5] [--window-ms 200] [--stacked-only]
 """
 from __future__ import annotations
 
@@ -145,13 +151,15 @@ def torch_step(torch, kind, n, n_in, hidden):
     return step
 
 
-def torch_cudnn_step(torch, kind, n, n_in, hidden):
+def torch_cudnn_step(torch, kind, n, n_in, hidden, layers=1, bidirectional=False):
     g = torch.Generator(device="cuda").manual_seed(0)
-    layer = (torch.nn.LSTM if kind == "lstm" else torch.nn.GRU)(n_in, hidden).cuda().to(torch.bfloat16)
+    dirs = 2 if bidirectional else 1
+    layer = (torch.nn.LSTM if kind == "lstm" else torch.nn.GRU)(n_in, hidden, num_layers=layers,
+                                                                bidirectional=bidirectional).cuda().to(torch.bfloat16)
     opt = torch.optim.SGD(layer.parameters(), lr=1e-3)
     x = (torch.rand(T, n, n_in, device="cuda", generator=g) * 2 - 1).to(torch.bfloat16)
-    tgt = (torch.rand(n, hidden, device="cuda", generator=g) - 0.5).to(torch.bfloat16)
-    zero = torch.zeros(1, n, hidden, device="cuda", dtype=torch.bfloat16)
+    tgt = (torch.rand(n, dirs * hidden, device="cuda", generator=g) - 0.5).to(torch.bfloat16)
+    zero = torch.zeros(layers * dirs, n, hidden, device="cuda", dtype=torch.bfloat16)
 
     def step():
         opt.zero_grad(set_to_none=False)
@@ -159,6 +167,65 @@ def torch_cudnn_step(torch, kind, n, n_in, hidden):
         torch.nn.functional.mse_loss(out[-1], tgt).backward()
         opt.step()
     return step
+
+
+STACKED = [("unidirectional", 1, False), ("bidirectional", 1, True), ("2_layers_bidirectional", 2, True)]
+
+
+def stacked_step(nk, dev, kind, n, n_in, hidden, layers, bidirectional):
+    """the captured step of nn.LSTM / nn.GRU(num_layers, bidirectional); the loss on the last layer's output[T-1]"""
+    from neuronika_b200 import optim
+    rng = np.random.default_rng(0)
+    dirs = 2 if bidirectional else 1
+    stacked = layers > 1 or bidirectional
+    m = (nk.nn.LSTM if kind == "lstm" else nk.nn.GRU)(dev, n_in, hidden, nk.BF16, grad_dtype=nk.F32, rng=rng,
+                                                       num_layers=layers, bidirectional=bidirectional)
+    opt = optim.StochasticGD.new(1e-3)
+    for p in m.parameters():
+        opt.register(p)
+    x = nk.from_ndarray(dev, rng.uniform(-1, 1, (T, n, n_in)).astype(np.float32), nk.BF16)
+    zero = nk.zeros(dev, (layers * dirs, n, hidden) if stacked else (n, hidden), nk.BF16)
+    tgt = nk.from_ndarray(dev, rng.uniform(-0.5, 0.5, (1, n, dirs * hidden)).astype(np.float32), nk.BF16)
+
+    def step():
+        opt.zero_grad()
+        out = m.forward((zero, zero), x) if kind == "lstm" else m.forward(zero, x)
+        y = out[0] if (kind == "lstm" or stacked) else out
+        loss = y.chunks((1, n, dirs * hidden))[T - 1].mse_loss(tgt)
+        loss.forward()
+        loss.backward(1.0)
+        opt.step()
+
+    step()
+    step()
+    dev.synchronize()
+    with dev.capture(12 << 30) as cap:   # the GRU's 2 layers x 2 directions at N = 1024, H = 2048 take ~9 GiB
+        step()
+    return cap.graph
+
+
+def stacked_row(nk, dev, torch, clock, args, card, kind, n, n_in, hidden):
+    graphs = {name: stacked_step(nk, dev, kind, n, n_in, hidden, layers, bi) for name, layers, bi in STACKED}
+    cudnn = {name: torch_cudnn_step(torch, kind, n, n_in, hidden, layers, bi) for name, layers, bi in STACKED}
+    res, mhz = {}, []
+    for _ in range(args.reps):      # alternating, one window each
+        for name, _, _ in STACKED:
+            for key, fn in ((name, graphs[name].launch), (name + "_torch_cudnn_bf16", cudnn[name])):
+                ms, m = timed(torch, fn, clock, args.window_ms, 1)
+                res.setdefault(key, []).append(ms)
+                mhz.append(m)
+    med = {k: float(np.median(v)) for k, v in res.items()}
+    print(json.dumps({
+        "cell": kind, "variant": "stacked", "N": n, "I": n_in, "H": hidden, "T": T,
+        "ms_per_sequence": {k: round(v, 3) for k, v in med.items()},
+        "launches_per_time_step": {name: round(graphs[name].kernel_count / T, 2) for name, _, _ in STACKED},
+        "bidirectional_over_2x_unidirectional": round(med["bidirectional"] / (2 * med["unidirectional"]), 3),
+        "speedup_vs_torch_cudnn_bf16": {name: round(med[name + "_torch_cudnn_bf16"] / med[name], 2)
+                                        for name, _, _ in STACKED},
+        "median_sm_mhz": float(np.median(mhz)), "card": card["name"], "power_limit_w": card["power_limit_w"],
+    }), flush=True)
+    for g in graphs.values():
+        g.close()
 
 
 def sequence_gemms(nk, dev, kind, n, n_in, hidden):
@@ -231,6 +298,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--window-ms", type=float, default=200.0)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--stacked-only", action="store_true", help="only the stacked / bidirectional rows")
     args = ap.parse_args()
     import torch
 
@@ -246,6 +314,9 @@ def main():
     print(json.dumps({"card": card, "sm_count": dev.sm_count, "T": T}), flush=True)
     for kind in ("lstm", "gru"):
         for n, n_in, hidden in SHAPES:
+            if args.stacked_only:
+                stacked_row(nk, dev, torch, clock, args, card, kind, n, n_in, hidden)
+                continue
             fused = graph_step(nk, dev, kind, n, n_in, hidden, "fused")
             comp = graph_step(nk, dev, kind, n, n_in, hidden, "composed")
             seq = graph_step(nk, dev, kind, n, n_in, hidden, "sequence")
@@ -292,6 +363,7 @@ def main():
             fused.close()
             comp.close()
             seq.close()
+            stacked_row(nk, dev, torch, clock, args, card, kind, n, n_in, hidden)
     clock.halt.set()
 
 
