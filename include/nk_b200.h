@@ -467,7 +467,10 @@ int nk_allreduce_sum(nk_ctx* ctx, void* ptr, size_t n, int dtype);
  * is fused into the kernels around it (neuronika_b200/csrc/nk_peer.cu):
  *   nk_gemm_rs       the wgmma GEMM whose epilogue stores row shard o of the (M,N) f32 product
  *                    into rank o's slot buffer `slots[o]` (world*M/world*N floats, slot index = the
- *                    calling rank) over NVLink, tile by tile while the MMAs run (reduce-scatter);
+ *                    calling rank) over NVLink, tile by tile while the MMAs run (reduce-scatter).
+ *                    Needs 2 <= world <= 8, bf16 operands that TMA can address, M % (world*128) == 0,
+ *                    N > 128, N % 4 == 0 and 16-byte aligned slots; K = 0 (an empty local batch) stores
+ *                    zero shards.  An error launches nothing and leaves the slots untouched;
  *   nk_peer_barrier  flag exchange through peer memory: returns (on the stream) once every rank has
  *                    reached the same `epoch`; `flags[r]` is rank r's flag array (>= world words);
  *   nk_reduce_bcast  the owner sums its `world` slots in rank order and stores the result into every

@@ -379,9 +379,31 @@ int nk_gemm_rs(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_
   NK_REQUIRE(ctx, slots && world >= 2 && world <= kMaxWorld && rank >= 0 && rank < world,
              "nk_gemm_rs: bad world %d / rank %d", world, rank);
   NK_REQUIRE(ctx, ab_dtype == NK_BF16, "nk_gemm_rs: the fused exchange runs on the tensor-core engine (bf16 operands)");
+  NK_REQUIRE(ctx, M >= 0 && N >= 0 && K >= 0, "nk_gemm_rs: negative dimension");
   NK_REQUIRE(ctx, M % (int64_t(world) * 128) == 0, "nk_gemm_rs: M = %lld is not a multiple of world * 128",
              (long long)M);
+  // the epilogue's conditions (launch_cfg), checked here so that the error names them: nk_gemm_bias_act would report
+  // any refusal of the forced tensor-core engine as operands that TMA cannot address
+  NK_REQUIRE(ctx, N > 128 && N % 4 == 0,
+             "nk_gemm_rs: N = %lld: the reduce-scatter epilogue runs 128x256 tiles (N > 128) with 16-byte row stores "
+             "(N %% 4 == 0)", (long long)N);
+  for (int o = 0; o < world; ++o)
+    NK_REQUIRE(ctx, slots[o] && (reinterpret_cast<uintptr_t>(slots[o]) & 15) == 0,
+               "nk_gemm_rs: slot buffer %d is NULL or not 16-byte aligned", o);
   const int64_t shard = (M / world) * N;  // elements per (owner, source) slot
+  if (M == 0) return NK_OK;
+  if (K == 0) {
+    // an empty local batch: the product is zero, and every owner still receives this rank's (zero) shard, so that all
+    // ranks go on to the same exchange
+    for (int o = 0; o < world; ++o) {
+      const int rc = nk_memset0(ctx, static_cast<float*>(slots[o]) + int64_t(rank) * shard, size_t(shard) * sizeof(float));
+      if (rc) return rc;
+    }
+    return NK_OK;
+  }
+  NK_REQUIRE(ctx, nk_gemm_wgmma_supported(transA, transB, M, N, K, A, lda, B, ldb),
+             "nk_gemm_rs: operands are not TMA-addressable (16-byte aligned base, leading dimension multiple of 8 "
+             "elements)");
   ctx->rs_world = world;
   ctx->rs_rank = rank;
   for (int o = 0; o < world; ++o) ctx->rs_dst[o] = static_cast<float*>(slots[o]) + int64_t(rank) * shard;
