@@ -334,6 +334,26 @@ int nk_convnd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, co
                          int64_t n, int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k,
                          const int64_t* stride, const int64_t* dilation, int64_t groups, int dtype,
                          float beta);
+/* 1-D / 3-D convolution LAYERS (nn.Conv1d / nn.Conv3d, neuronika-nn/src/lib.rs:630-916): y = conv(pad(x), w) + bias,
+ * x (N, Cin, s[0..nsp)), w (Cout, Cin, k[0..nsp)), nsp = 1 or 3, groups = 1, pad[a] on both sides of axis a with an
+ * nk_pad_mode (pad_value: the constant mode's fill), bias (Cout) or NULL.  bf16 shapes of the im2col engine run on the
+ * tensor cores with the padding applied inside the column gather ("wgmma_im2col_nd_*"); f32, the other shapes and
+ * nk_conv_config(DIRECT) pad into a stream-ordered temporary and run the CUDA-core kernels of nk_convnd_* ("direct_nd_*"),
+ * bit-identical to nk_padnd_fwd -> nk_convnd_* -> nk_add_bcast_fwd.  dx gets the interior slice of the padded input's
+ * gradient for every mode (the reference's pad backward, pad/mod.rs:157-182; torch instead folds the border gradient of
+ * reflect / replicate padding back onto the input).  bwd_kernel also accumulates dbias[Cout] (dw_dtype) when non-NULL.
+ * With N = 0 nothing is computed and dW (and dbias) become beta * dW; g and x may then be NULL.  Reflective padding must
+ * be smaller than the input extent. */
+int nk_conv_layer_nd_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int nsp, int64_t n,
+                         int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* stride,
+                         const int64_t* dilation, const int64_t* pad, int pad_mode, float pad_value, int dtype);
+int nk_conv_layer_nd_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int nsp, int64_t n, int64_t cin,
+                               const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* stride,
+                               const int64_t* dilation, const int64_t* pad, int pad_mode, int dtype, float beta);
+int nk_conv_layer_nd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbias, const void* g, const void* x, int nsp,
+                                int64_t n, int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k,
+                                const int64_t* stride, const int64_t* dilation, const int64_t* pad, int pad_mode,
+                                float pad_value, int dtype, float beta);
 /* name of the kernel variant the last conv call used */
 const char* nk_last_conv_kernel(nk_ctx* ctx);
 

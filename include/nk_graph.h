@@ -114,6 +114,13 @@ int nkg_vv(nkg_var* a, nkg_var* b, nkg_var** out);             /* vector_vector_
 /* 1-d (N,C,L) / 3-d (N,C,D,H,W) convolution; the receiver is the kernel, as in nkg_convolution */
 int nkg_convolution_nd(nkg_var* kernel, nkg_var* input, int nsp, const int64_t* stride, const int64_t* dilation,
                        int64_t groups, nkg_var** out);
+/* The 1-d / 3-d convolution LAYER (nn.Conv1d / nn.Conv3d) as ONE node: out = conv(pad(input), weight) + bias, input
+ * (N, Cin, s...) with nsp = 1 or 3 sample dims, weight (Cout, Cin, k...), bias (Cout, 1, ..) with nsp ones, or NULL;
+ * `padding` per sample dim with an nk_pad_mode (`value`: the constant mode's fill).  The same results as the nodes
+ * pad_mode -> convolution_nd -> add, without the padded copy of the input or its gradient: forward and backward are
+ * nk_conv_layer_nd_* (tensor cores for bf16).  The backward writes only the gradients of differentiable operands. */
+int nkg_conv_layer(nkg_var* input, nkg_var* weight, nkg_var* bias, int nsp, const int64_t* padding, int mode, float value,
+                   const int64_t* stride, const int64_t* dilation, nkg_var** out);
 
 /* ---- chunks and recurrent cells (SURVEY.md 8-f rank 4) ----
  * nkg_chunks (var.rs:401-417): every block of ndarray's exact_chunks(chunk_shape) in row-major block order, one lazy

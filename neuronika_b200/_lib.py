@@ -129,6 +129,10 @@ _PROTOS = {
     "nk_convnd_fwd": (i32, [vp, vp, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, i64, i32]),
     "nk_convnd_bwd_input": (i32, [vp, vp, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, i64, i32, f32]),
     "nk_convnd_bwd_kernel": (i32, [vp, vp, i32, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, i64, i32, f32]),
+    "nk_conv_layer_nd_fwd": (i32, [vp, vp, vp, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, pi64, i32, f32, i32]),
+    "nk_conv_layer_nd_bwd_input": (i32, [vp, vp, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, pi64, i32, i32, f32]),
+    "nk_conv_layer_nd_bwd_kernel": (i32, [vp, vp, i32, vp, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, pi64, i32,
+                                          f32, i32, f32]),
     "nk_adam_step": (i32, [vp, vp, i32, vp, i32, vp, vp, vp, vp, sz, i64, f32, f32, f32, f32, f32, f32, f32, i32]),
     "nk_rmsprop_step": (i32, [vp, vp, i32, vp, i32, vp, vp, vp, vp, sz, f32, f32, f32, f32, f32, f32, f32, i32]),
     "nk_adagrad_step": (i32, [vp, vp, i32, vp, i32, vp, vp, sz, i64, f32, f32, f32, f32, f32, f32, i32]),

@@ -11,6 +11,13 @@
 //   runs) and is the MN-major wgmma operand as it lies; the buffer lives in HBM for the duration of the call (sample
 //   chunks of <= 4 GB).  The (Cout, K) kernel is copied once into rows of Kp = ceil8(K) elements (TMA row pitch).
 // Compute bound for Cin >= 16 (K >= 144); the column buffer adds 2 x |cols| of HBM traffic.
+//
+// The same three GEMMs serve the 1-D / 3-D convolution LAYERS (nk_conv_layer_nd_*, nk_conv_nd.cu): x (N, Cin, s0[, s1,
+// s2]), k = (c, i0, i1, i2), l = output position in row-major order, and the layer's padding applied inside the gather
+// instead of through a padded copy of x: column element (c, i, p) reads padded coordinate u' = p*s + i*d along each axis,
+// mapped to a source index by the padding mode exactly as nk_padnd_fwd maps it (a bit-exact copy or the fill value).
+// col2im writes only the interior dx positions, each the f32 sum of the taps that read padded coordinate u + pad: the
+// reference's pad backward, the interior slice for every mode (pad/mod.rs:157-182).
 #include "nk_internal.cuh"
 
 int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
@@ -26,6 +33,30 @@ constexpr int64_t kChunkBytes = int64_t(4) << 30;
 struct CgDims {
   int64_t n, cin, h, w, cout, kh, kw, sh, sw, dh, dw, ho, wo, K, Kp, L, Lp;
 };
+
+// the 1-D / 3-D layer: sample dims padded to three with leading extents of 1 (kernel 1, stride 1, dilation 1, pad 0)
+struct CgNdDims {
+  int64_t n, cin, cout, K, Kp, L, Lp;
+  int64_t in[3], k[3], s[3], d[3], pad[3], out[3];
+  int mode;        // nk_pad_mode
+  float value;     // fill of the constant mode
+};
+
+// eight consecutive bf16 source elements x[off .. off+7] (2-byte aligned): aligned 4-byte loads + a funnel shift when the
+// run starts on an odd element
+__device__ __forceinline__ uint4 load_run8(const __nv_bfloat16* __restrict__ x, int64_t off, int64_t x_elems) {
+  const uint32_t* xw = reinterpret_cast<const uint32_t*>(x);
+  if ((off & 1) == 0) {
+    const uint32_t* s = xw + (off >> 1);
+    return make_uint4(__ldg(s), __ldg(s + 1), __ldg(s + 2), __ldg(s + 3));
+  }
+  const uint32_t* s = xw + ((off - 1) >> 1);
+  const uint32_t w0 = __ldg(s), w1 = __ldg(s + 1), w2 = __ldg(s + 2), w3 = __ldg(s + 3);
+  // the fifth word holds source element off+7 in its low half; its high half may lie past the end of x
+  const uint32_t w4 = (off + 9 <= x_elems) ? __ldg(s + 4) : uint32_t(reinterpret_cast<const unsigned short*>(x)[off + 7]);
+  return make_uint4(__funnelshift_r(w0, w1, 16), __funnelshift_r(w1, w2, 16), __funnelshift_r(w2, w3, 16),
+                    __funnelshift_r(w3, w4, 16));
+}
 
 // colsT[ns][k][l0 .. l0+7]: one thread per 16-byte vector of eight consecutive output pixels of one im2col row (rows Lp
 // apart; the pixels l >= L of the last vector are written as zeros)
@@ -48,20 +79,8 @@ __global__ void __launch_bounds__(kThreads) im2col_kernel(__nv_bfloat16* __restr
     const int64_t plane = ((n0 + ns) * d.cin + c) * d.h;
     uint4 out;
     if (d.sw == 1 && q + 8 <= wo && l0 + 8 <= L) {
-      const int64_t off = (plane + p * d.sh + i * d.dh) * d.w + q + j * d.dw;   // first of 8 consecutive source elements
-      const uint32_t* xw = reinterpret_cast<const uint32_t*>(x);
-      if ((off & 1) == 0) {
-        const uint32_t* s = xw + (off >> 1);
-        out = make_uint4(__ldg(s), __ldg(s + 1), __ldg(s + 2), __ldg(s + 3));
-      } else {
-        const uint32_t* s = xw + ((off - 1) >> 1);
-        const uint32_t w0 = __ldg(s), w1 = __ldg(s + 1), w2 = __ldg(s + 2), w3 = __ldg(s + 3);
-        // the fifth word holds source element off+7 in its low half; its high half may lie past the end of x
-        const uint32_t w4 = (off + 9 <= x_elems) ? __ldg(s + 4)
-                                                 : uint32_t(reinterpret_cast<const unsigned short*>(x)[off + 7]);
-        out = make_uint4(__funnelshift_r(w0, w1, 16), __funnelshift_r(w1, w2, 16), __funnelshift_r(w2, w3, 16),
-                         __funnelshift_r(w3, w4, 16));
-      }
+      // first of 8 consecutive source elements
+      out = load_run8(x, (plane + p * d.sh + i * d.dh) * d.w + q + j * d.dw, x_elems);
     } else {
       __align__(16) unsigned short e[8];
       const unsigned short* xs = reinterpret_cast<const unsigned short*>(x);
@@ -173,6 +192,133 @@ __global__ void __launch_bounds__(kThreads) finalize_dw_padded(T* __restrict__ d
   dw[idx] = nk_from_f32<T>(v);
 }
 
+// ---- 1-D / 3-D layers with the padding folded into the gather
+// source index of padded coordinate u along an axis of length len padded by p on both sides, or -1 for the fill value:
+// the map of nk_padnd_fwd (nk_pointwise.cu pad_src; reflective/mod.rs:22-31, replicative/mod.rs:22-31)
+__device__ __forceinline__ int pad_src_index(int u, int len, int p, int mode) {
+  if (u >= p && u < len + p) return u - p;
+  if (mode == NK_PAD_REFLECTIVE) return (u < p ? 2 * p - u : 2 * (len + p - 1) - u) - p;
+  if (mode == NK_PAD_REPLICATIVE) return u < p ? 0 : len - 1;
+  return -1;
+}
+
+// colsT[ns][(c, i0, i1, i2)][l0 .. l0+7] as im2col_kernel, through the padding map.  A vector of eight outputs along one
+// output row (unit stride on the last axis) reads one source row: the fill value when the padding puts that row outside x
+// (constant mode), else a contiguous run (load_run8) when the eight columns are interior; only runs that touch the border
+// along the last axis, non-unit last-axis strides and vectors that wrap a row are gathered element by element.
+__global__ void __launch_bounds__(kThreads) im2col_nd_kernel(__nv_bfloat16* __restrict__ cols, const __nv_bfloat16* __restrict__ x,
+                                                             CgNdDims d, int64_t n0, int64_t nn) {
+  const uint32_t lv_n = uint32_t(d.Lp / 8), L = uint32_t(d.L), K = uint32_t(d.K);
+  const int in0 = int(d.in[0]), in1 = int(d.in[1]), in2 = int(d.in[2]), k1 = int(d.k[1]), k2 = int(d.k[2]);
+  const int o1 = int(d.out[1]), o2 = int(d.out[2]), ksz = int(d.k[0]) * k1 * k2;
+  const int s0 = int(d.s[0]), s1 = int(d.s[1]), s2 = int(d.s[2]), d0 = int(d.d[0]), d1 = int(d.d[1]), d2 = int(d.d[2]);
+  const int p0 = int(d.pad[0]), p1 = int(d.pad[1]), p2 = int(d.pad[2]), mode = d.mode;
+  const int64_t isz = int64_t(in0) * in1 * in2;
+  const int64_t total = nn * int64_t(K) * lv_n;
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  const int64_t x_elems = d.n * d.cin * isz;
+  const unsigned short fill = __bfloat16_as_ushort(__float2bfloat16_rn(d.value));
+  const unsigned short* xs = reinterpret_cast<const unsigned short*>(x);
+  for (int64_t idx = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; idx < total; idx += stride) {
+    const uint32_t row = uint32_t(idx / lv_n);          // (ns, k)
+    const uint32_t lv = uint32_t(idx - int64_t(row) * lv_n);
+    const uint32_t ns = row / K, k = row - ns * K;
+    const int c = int(k) / ksz;
+    int t = int(k) - c * ksz;
+    const int i2 = t % k2;
+    t /= k2;
+    const int i1 = t % k1, i0 = t / k1;
+    const int64_t plane = ((n0 + ns) * d.cin + c) * isz;
+    const uint32_t l0 = lv * 8;
+    const int q = int(l0 % uint32_t(o2)), r = int(l0 / uint32_t(o2));
+    uint4 out;
+    if (s2 == 1 && q + 8 <= o2 && l0 + 8 <= L) {
+      const int r0 = pad_src_index((r / o1) * s0 + i0 * d0, in0, p0, mode);
+      const int r1 = pad_src_index((r % o1) * s1 + i1 * d1, in1, p1, mode);
+      const int u2 = q + i2 * d2 - p2;                  // source column of the first output
+      if (r0 < 0 || r1 < 0) {
+        const uint32_t f = uint32_t(fill) * 0x10001u;
+        out = make_uint4(f, f, f, f);
+      } else if (u2 >= 0 && u2 + 8 <= in2) {
+        out = load_run8(x, plane + (int64_t(r0) * in1 + r1) * in2 + u2, x_elems);
+      } else {
+        __align__(16) unsigned short e[8];
+        const unsigned short* src = xs + plane + (int64_t(r0) * in1 + r1) * in2;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int u = pad_src_index(q + j + i2 * d2, in2, p2, mode);
+          e[j] = u < 0 ? fill : __ldg(src + u);
+        }
+        out = *reinterpret_cast<const uint4*>(e);
+      }
+    } else {
+      __align__(16) unsigned short e[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t l = l0 + j;
+        unsigned short v = 0;
+        if (l < L) {
+          const int c2 = int(l % uint32_t(o2)), rr = int(l / uint32_t(o2));
+          const int u0 = pad_src_index((rr / o1) * s0 + i0 * d0, in0, p0, mode);
+          const int u1 = pad_src_index((rr % o1) * s1 + i1 * d1, in1, p1, mode);
+          const int u2 = pad_src_index(c2 * s2 + i2 * d2, in2, p2, mode);
+          v = (u0 < 0 || u1 < 0 || u2 < 0) ? fill : __ldg(xs + plane + (int64_t(u0) * in1 + u1) * in2 + u2);
+        }
+        e[j] = v;
+      }
+      out = *reinterpret_cast<const uint4*>(e);
+    }
+    reinterpret_cast<uint4*>(cols)[idx] = out;
+  }
+}
+
+// dx[n,c,u] = beta*dx + sum over the taps i and output positions p with p*s + i*d = u + pad (per axis) of
+// dcolsT[ns][(c,i)][p]: only the interior positions of the padded input, whatever the mode; one thread per dx element,
+// the taps summed in f32 and rounded once
+__global__ void __launch_bounds__(kThreads) col2im_nd_kernel(__nv_bfloat16* __restrict__ dx, const float* __restrict__ dcols,
+                                                             CgNdDims d, int64_t n0, int64_t nn, float beta) {
+  const int in0 = int(d.in[0]), in1 = int(d.in[1]), in2 = int(d.in[2]);
+  const int k0 = int(d.k[0]), k1 = int(d.k[1]), k2 = int(d.k[2]);
+  const int o0 = int(d.out[0]), o1 = int(d.out[1]), o2 = int(d.out[2]);
+  const int s0 = int(d.s[0]), s1 = int(d.s[1]), s2 = int(d.s[2]), d0 = int(d.d[0]), d1 = int(d.d[1]), d2 = int(d.d[2]);
+  const int cin = int(d.cin), ksz = k0 * k1 * k2;
+  const uint32_t isz = uint32_t(in0) * uint32_t(in1) * uint32_t(in2);
+  const int64_t total = nn * d.cin * int64_t(isz);
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  for (int64_t idx = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; idx < total; idx += stride) {
+    const uint32_t pl = uint32_t(idx / isz);            // (ns, c)
+    const uint32_t uv = uint32_t(idx - int64_t(pl) * isz);
+    const int U2 = int(uv % uint32_t(in2)) + int(d.pad[2]);
+    const int t = int(uv / uint32_t(in2));
+    const int U1 = t % in1 + int(d.pad[1]), U0 = t / in1 + int(d.pad[0]);
+    const uint32_t ns = pl / uint32_t(cin), c = pl - ns * uint32_t(cin);
+    const float* dc = dcols + (int64_t(ns) * d.K + int64_t(c) * ksz) * d.Lp;
+    float acc = 0.f;
+    for (int i0 = 0; i0 < k0; ++i0) {
+      const int pu0 = U0 - i0 * d0;
+      if (pu0 < 0) break;
+      const int q0 = pu0 / s0;
+      if (q0 * s0 != pu0 || q0 >= o0) continue;
+      for (int i1 = 0; i1 < k1; ++i1) {
+        const int pu1 = U1 - i1 * d1;
+        if (pu1 < 0) break;
+        const int q1 = pu1 / s1;
+        if (q1 * s1 != pu1 || q1 >= o1) continue;
+        for (int i2 = 0; i2 < k2; ++i2) {
+          const int pu2 = U2 - i2 * d2;
+          if (pu2 < 0) break;
+          const int q2 = pu2 / s2;
+          if (q2 * s2 != pu2 || q2 >= o2) continue;
+          acc += dc[int64_t((i0 * k1 + i1) * k2 + i2) * d.Lp + (int64_t(q0) * o1 + q1) * o2 + q2];
+        }
+      }
+    }
+    __nv_bfloat16* o = dx + n0 * d.cin * int64_t(isz) + idx;
+    if (beta != 0.f) acc += beta * __bfloat162float(*o);
+    *o = __float2bfloat16_rn(acc);
+  }
+}
+
 inline int cg_blocks(nk_ctx* ctx, int64_t items) {
   int64_t b = (items + kThreads - 1) / kThreads;
   const int64_t cap = int64_t(ctx->sm_count) * 16;
@@ -226,7 +372,22 @@ int launch_col2im(nk_ctx* ctx, __nv_bfloat16* dx, const float* dcols, const CgDi
   return NK_OK;
 }
 
-int64_t chunk_samples(const CgDims& d, int64_t elem_bytes = 2) {
+// the 1-D / 3-D layer's gather / scatter (one launch per sample chunk)
+int launch_im2col(nk_ctx* ctx, __nv_bfloat16* cols, const __nv_bfloat16* x, const CgNdDims& d, int64_t n0, int64_t nn) {
+  im2col_nd_kernel<<<cg_blocks(ctx, nn * d.K * (d.Lp / 8)), kThreads, 0, ctx->stream>>>(cols, x, d, n0, nn);
+  NK_LAUNCHED(ctx, "im2col_nd");
+  return NK_OK;
+}
+int launch_col2im(nk_ctx* ctx, __nv_bfloat16* dx, const float* dcols, const CgNdDims& d, int64_t n0, int64_t nn, float beta) {
+  col2im_nd_kernel<<<cg_blocks(ctx, nn * d.cin * d.in[0] * d.in[1] * d.in[2]), kThreads, 0, ctx->stream>>>(dx, dcols, d, n0,
+                                                                                                          nn, beta);
+  NK_LAUNCHED(ctx, "col2im_nd");
+  return NK_OK;
+}
+
+// the helpers and drivers below read only the GEMM geometry (n, cout, K, Kp, L, Lp) of CgDims / CgNdDims
+template <class D>
+int64_t chunk_samples(const D& d, int64_t elem_bytes = 2) {
   int64_t per = d.Lp * d.Kp * elem_bytes;
   int64_t c = kChunkBytes / per;
   if (c < 1) c = 1;
@@ -235,12 +396,14 @@ int64_t chunk_samples(const CgDims& d, int64_t elem_bytes = 2) {
 
 // The output gradient as a GEMM operand: TMA needs its rows of L pixels 16-byte aligned, i.e. L % 8 == 0 and an aligned
 // base.  Otherwise each sample chunk is first copied into rows Lp apart (slot `slot` of the scratch, cs samples).
-int g_rows_scratch(nk_ctx* ctx, Scratch& s, int slot, const CgDims& d, const void* g, int64_t cs, int64_t* ldg) {
+template <class D>
+int g_rows_scratch(nk_ctx* ctx, Scratch& s, int slot, const D& d, const void* g, int64_t cs, int64_t* ldg) {
   const bool copy = d.Lp != d.L || (reinterpret_cast<uintptr_t>(g) & 15);
   *ldg = copy ? d.Lp : d.L;
   return copy ? nk_alloc_uninit(ctx, size_t(cs * d.cout * d.Lp * 2), &s.p[slot]) : NK_OK;
 }
-int g_rows(nk_ctx* ctx, void* copy, const CgDims& d, const void* g, int64_t n0, int64_t nn, const __nv_bfloat16** out) {
+template <class D>
+int g_rows(nk_ctx* ctx, void* copy, const D& d, const void* g, int64_t n0, int64_t nn, const __nv_bfloat16** out) {
   const __nv_bfloat16* gn = static_cast<const __nv_bfloat16*>(g) + n0 * d.cout * d.L;
   *out = gn;
   if (d.Lp == d.L && (reinterpret_cast<uintptr_t>(g) & 15) == 0) return NK_OK;
@@ -251,15 +414,11 @@ int g_rows(nk_ctx* ctx, void* copy, const CgDims& d, const void* g, int64_t n0, 
   return NK_OK;
 }
 
-}  // namespace
-
-// all three return NK_ERR_UNSUPPORTED (last_error untouched) when the shape is outside this engine
-
-int nk_conv_gemm_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int relu, int64_t n, int64_t cin,
-                     int64_t h, int64_t wd, int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw) {
-  CgDims d;
-  if (!make_dims(d, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(x) & 3) || cout < 8) return NK_ERR_UNSUPPORTED;
+// ---- the three products, shared by the 2-D entry points and the 1-D / 3-D layers (launch_im2col / launch_col2im are
+// overloaded on the dims type)
+template <class D>
+int gemm_conv_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int relu, const D& d) {
+  const int64_t n = d.n, cout = d.cout;
   Scratch s(ctx);
   int rc = nk_alloc_uninit(ctx, size_t(cout * d.Kp * 2), &s.p[0]);
   if (rc) return rc;
@@ -278,15 +437,12 @@ int nk_conv_gemm_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const v
                                  relu, 0);
     if (rc) return rc;
   }
-  ctx->last_conv_kernel = "wgmma_im2col_gemm_fwd";
   return NK_OK;
 }
 
-int nk_conv_gemm_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int64_t n, int64_t cin, int64_t h, int64_t wd,
-                           int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw, float beta) {
-  CgDims d;
-  if (!make_dims(d, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
-  if (cout % 8 != 0) return NK_ERR_UNSUPPORTED;
+template <class D>
+int gemm_conv_dx(nk_ctx* ctx, void* dx, const void* g, const void* w, const D& d, float beta) {
+  const int64_t n = d.n, cout = d.cout;
   Scratch s(ctx);
   int rc = nk_alloc_uninit(ctx, size_t(cout * d.Kp * 2), &s.p[0]);
   if (rc) return rc;
@@ -310,16 +466,12 @@ int nk_conv_gemm_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, 
     rc = launch_col2im(ctx, (__nv_bfloat16*)dx, (const float*)s.p[1], d, n0, nn, beta);
     if (rc) return rc;
   }
-  ctx->last_conv_kernel = "wgmma_im2col_gemm_dx";
   return NK_OK;
 }
 
-int nk_conv_gemm_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, const void* x, int64_t n, int64_t cin, int64_t h,
-                            int64_t wd, int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw,
-                            float beta) {
-  CgDims d;
-  if (!make_dims(d, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
-  if (reinterpret_cast<uintptr_t>(x) & 3) return NK_ERR_UNSUPPORTED;
+template <class D>
+int gemm_conv_dw(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, const void* x, const D& d, float beta) {
+  const int64_t n = d.n, cout = d.cout;
   Scratch s(ctx);
   const int64_t cs = chunk_samples(d);
   int rc = nk_alloc_uninit(ctx, size_t(cs * d.Lp * d.Kp * 2), &s.p[1]);
@@ -347,6 +499,94 @@ int nk_conv_gemm_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g,
   else
     finalize_dw_padded<float><<<fb, kThreads, 0, ctx->stream>>>((float*)dwt, (const float*)s.p[2], cout, d.K, d.Kp, beta);
   NK_LAUNCHED(ctx, "conv_dw_finalize_padded");
-  ctx->last_conv_kernel = "wgmma_im2col_gemm_dw";
   return NK_OK;
+}
+
+// the layer's geometry: output extents of the padded input, and the 2-D engine's applicability rules (make_dims)
+bool make_nd_dims(CgNdDims& d, int nsp, int64_t n, int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k,
+                  const int64_t* s, const int64_t* dil, const int64_t* pad, int mode, float value) {
+  d = CgNdDims{};
+  d.n = n, d.cin = cin, d.cout = cout, d.mode = mode, d.value = value;
+  d.K = cin, d.L = 1;
+  for (int a = 0; a < 3; ++a) d.in[a] = d.k[a] = d.s[a] = d.d[a] = d.out[a] = 1, d.pad[a] = 0;
+  for (int a = 0; a < nsp; ++a) {
+    const int j = 3 - nsp + a;
+    d.in[j] = in_sp[a], d.k[j] = k[a], d.s[j] = s[a], d.d[j] = dil[a], d.pad[j] = pad[a];
+    d.out[j] = (in_sp[a] + 2 * pad[a] - dil[a] * (k[a] - 1) - 1) / s[a] + 1;
+    d.K *= k[a];
+    d.L *= d.out[j];
+  }
+  d.Kp = (d.K + 7) & ~int64_t(7);
+  d.Lp = (d.L + 7) & ~int64_t(7);
+  return n > 0 && d.L > 0 && d.Kp >= 16 && d.Lp * d.Kp < (int64_t(1) << 31);
+}
+
+}  // namespace
+
+// all three return NK_ERR_UNSUPPORTED (last_error untouched) when the shape is outside this engine
+
+int nk_conv_gemm_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int relu, int64_t n, int64_t cin,
+                     int64_t h, int64_t wd, int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw) {
+  CgDims d;
+  if (!make_dims(d, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
+  if ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(x) & 3) || cout < 8) return NK_ERR_UNSUPPORTED;
+  const int rc = gemm_conv_fwd(ctx, y, x, w, bias, relu, d);
+  if (rc == NK_OK) ctx->last_conv_kernel = "wgmma_im2col_gemm_fwd";
+  return rc;
+}
+
+int nk_conv_gemm_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int64_t n, int64_t cin, int64_t h, int64_t wd,
+                           int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw, float beta) {
+  CgDims d;
+  if (!make_dims(d, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
+  if (cout % 8 != 0) return NK_ERR_UNSUPPORTED;
+  const int rc = gemm_conv_dx(ctx, dx, g, w, d, beta);
+  if (rc == NK_OK) ctx->last_conv_kernel = "wgmma_im2col_gemm_dx";
+  return rc;
+}
+
+int nk_conv_gemm_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, const void* x, int64_t n, int64_t cin, int64_t h,
+                            int64_t wd, int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw,
+                            float beta) {
+  CgDims d;
+  if (!make_dims(d, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
+  if (reinterpret_cast<uintptr_t>(x) & 3) return NK_ERR_UNSUPPORTED;
+  const int rc = gemm_conv_dw(ctx, dwt, dw_dtype, g, x, d, beta);
+  if (rc == NK_OK) ctx->last_conv_kernel = "wgmma_im2col_gemm_dw";
+  return rc;
+}
+
+// The 1-D / 3-D layer (nsp sample dims, groups = 1, padding `pad` with nk_pad_mode `mode`): arguments validated by the
+// caller (nk_conv_layer_nd_*, nk_conv_nd.cu); same applicability and return protocol as the 2-D entry points above.
+int nk_conv_gemm_nd_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int nsp, int64_t n, int64_t cin,
+                        const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s, const int64_t* dil,
+                        const int64_t* pad, int mode, float value) {
+  CgNdDims d;
+  if (!make_nd_dims(d, nsp, n, cin, in_sp, cout, k, s, dil, pad, mode, value) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
+  if ((reinterpret_cast<uintptr_t>(y) & 15) || (reinterpret_cast<uintptr_t>(x) & 3) || cout < 8) return NK_ERR_UNSUPPORTED;
+  const int rc = gemm_conv_fwd(ctx, y, x, w, bias, 0, d);
+  if (rc == NK_OK) ctx->last_conv_kernel = "wgmma_im2col_nd_fwd";
+  return rc;
+}
+
+int nk_conv_gemm_nd_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int nsp, int64_t n, int64_t cin,
+                              const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s, const int64_t* dil,
+                              const int64_t* pad, int mode, float beta) {
+  CgNdDims d;
+  if (!make_nd_dims(d, nsp, n, cin, in_sp, cout, k, s, dil, pad, mode, 0.f) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
+  if (cout % 8 != 0) return NK_ERR_UNSUPPORTED;
+  const int rc = gemm_conv_dx(ctx, dx, g, w, d, beta);
+  if (rc == NK_OK) ctx->last_conv_kernel = "wgmma_im2col_nd_dx";
+  return rc;
+}
+
+int nk_conv_gemm_nd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, const void* x, int nsp, int64_t n,
+                               int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s,
+                               const int64_t* dil, const int64_t* pad, int mode, float value, float beta) {
+  CgNdDims d;
+  if (!make_nd_dims(d, nsp, n, cin, in_sp, cout, k, s, dil, pad, mode, value) || !ctx->encode_tiled) return NK_ERR_UNSUPPORTED;
+  if (reinterpret_cast<uintptr_t>(x) & 3) return NK_ERR_UNSUPPORTED;
+  const int rc = gemm_conv_dw(ctx, dwt, dw_dtype, g, x, d, beta);
+  if (rc == NK_OK) ctx->last_conv_kernel = "wgmma_im2col_nd_dw";
+  return rc;
 }

@@ -172,7 +172,63 @@ inline int nd_blocks(nk_ctx* ctx, int64_t total) {
   return int(b < 1 ? 1 : b);
 }
 
+// ---- the 1-D / 3-D convolution layers: y = conv(pad(x), W) + b
+struct LayerDims {
+  NdDims d;            // the convolution of the padded input
+  int64_t padded[3];   // its sample extents (nsp of them)
+  bool any_pad;
+};
+
+int layer_dims(nk_ctx* ctx, const char* who, int nsp, int64_t n, int64_t cin, const int64_t* in_sp, int64_t cout,
+               const int64_t* k, const int64_t* s, const int64_t* dil, const int64_t* pad, int mode, LayerDims* ld) {
+  NK_REQUIRE(ctx, nsp == 1 || nsp == 3, "%s: 1 or 3 sample dimensions (got %d); 2-d layers use nk_conv2d_*", who, nsp);
+  NK_REQUIRE(ctx, in_sp && pad, "%s: NULL shape pointer", who);
+  NK_REQUIRE(ctx, mode >= NK_PAD_CONSTANT && mode <= NK_PAD_REPLICATIVE, "pad: bad mode %d", mode);
+  ld->any_pad = false;
+  for (int a = 0; a < nsp; ++a) {
+    NK_REQUIRE(ctx, in_sp[a] >= 0 && pad[a] >= 0, "pad: negative size");
+    NK_REQUIRE(ctx, mode != NK_PAD_REFLECTIVE || pad[a] == 0 || pad[a] < in_sp[a],
+               "pad: reflective padding %lld must be smaller than the dimension %lld", (long long)pad[a], (long long)in_sp[a]);
+    NK_REQUIRE(ctx, mode != NK_PAD_REPLICATIVE || pad[a] == 0 || in_sp[a] > 0, "pad: replicative padding of an empty dimension");
+    ld->padded[a] = in_sp[a] + 2 * pad[a];
+    ld->any_pad = ld->any_pad || pad[a] > 0;
+  }
+  return make_dims(ctx, who, nsp, n, cin, ld->padded, cout, k, s, dil, 1, &ld->d);
+}
+
+// the (Cout, 1, ..) bias against the (N, Cout, out...) output: the shapes the Addition node of the composed graph uses
+void bias_shapes(const NdDims& d, int nsp, int64_t* bshape, int64_t* yshape) {
+  bshape[0] = d.cout, yshape[0] = d.n, yshape[1] = d.cout;
+  for (int a = 0; a < nsp; ++a) bshape[1 + a] = 1, yshape[2 + a] = d.out[3 - nsp + a];
+}
+
+// the padded input (planes, padded...) in a stream-ordered temporary, as the composed graph's Pad node writes it
+int padded_copy(nk_ctx* ctx, const void* x, const LayerDims& ld, int nsp, const int64_t* in_sp, const int64_t* pad, int mode,
+                float value, int dtype, void** out) {
+  int64_t elems = ld.d.n * ld.d.cin;
+  for (int a = 0; a < nsp; ++a) elems *= ld.padded[a];
+  int rc = nk_alloc_uninit(ctx, size_t(elems) * nk_dtype_size(dtype), out);
+  if (rc) return rc;
+  rc = nk_padnd_fwd(ctx, *out, x, ld.d.n * ld.d.cin, nsp, in_sp, pad, mode, value, dtype);
+  if (rc) {
+    nk_free(ctx, *out);
+    *out = nullptr;
+  }
+  return rc;
+}
+
 }  // namespace
+
+// im2col + batched wgmma GEMM with the padding folded into the gather (nk_conv_gemm.cu)
+int nk_conv_gemm_nd_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int nsp, int64_t n, int64_t cin,
+                        const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s, const int64_t* dil,
+                        const int64_t* pad, int mode, float value);
+int nk_conv_gemm_nd_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int nsp, int64_t n, int64_t cin,
+                              const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s, const int64_t* dil,
+                              const int64_t* pad, int mode, float beta);
+int nk_conv_gemm_nd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, const void* x, int nsp, int64_t n,
+                               int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s,
+                               const int64_t* dil, const int64_t* pad, int mode, float value, float beta);
 
 extern "C" {
 
@@ -254,6 +310,99 @@ int nk_convnd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, co
   NK_LAUNCHED(ctx, "convnd_finalize");
   ctx->last_conv_kernel = "direct_nd_dw";
   return NK_OK;
+}
+
+// The layers pick the engine as nk_conv2d_* do: the tensor cores for bf16 shapes the im2col engine takes (unless
+// nk_conv_config(DIRECT)); otherwise the padded input in a temporary and the CUDA-core kernels above, i.e. the calls of
+// the composed graph pad -> convolution -> + bias, with the same results.
+int nk_conv_layer_nd_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int nsp, int64_t n, int64_t cin,
+                         const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* stride,
+                         const int64_t* dilation, const int64_t* pad, int pad_mode, float pad_value, int dtype) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, nk_dtype_ok(dtype), "nk_conv_layer_nd_fwd: bad dtype %d", dtype);
+  LayerDims ld;
+  int rc = layer_dims(ctx, "nk_conv_layer_nd_fwd", nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, &ld);
+  if (rc) return rc;
+  if (ld.d.n * ld.d.cout * ld.d.out[0] * ld.d.out[1] * ld.d.out[2] == 0) return NK_OK;
+  NK_REQUIRE(ctx, y && x && w, "nk_conv_layer_nd_fwd: NULL pointer");
+  if (dtype == NK_BF16 && ctx->conv_engine != NK_CONV_DIRECT) {
+    rc = nk_conv_gemm_nd_fwd(ctx, y, x, w, bias, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, pad_value);
+    if (rc != NK_ERR_UNSUPPORTED) return rc;
+  }
+  void* xp = nullptr;
+  if (ld.any_pad) {
+    rc = padded_copy(ctx, x, ld, nsp, in_sp, pad, pad_mode, pad_value, dtype, &xp);
+    if (rc) return rc;
+  }
+  rc = nk_convnd_fwd(ctx, y, xp ? xp : x, w, nsp, n, cin, ld.padded, cout, k, stride, dilation, 1, dtype);
+  nk_free(ctx, xp);
+  if (rc || !bias) return rc;
+  int64_t bshape[4], yshape[5];
+  bias_shapes(ld.d, nsp, bshape, yshape);
+  return nk_add_bcast_fwd(ctx, y, y, bias, dtype, nsp + 2, yshape, nsp + 2, yshape, nsp + 1, bshape);
+}
+
+int nk_conv_layer_nd_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int nsp, int64_t n, int64_t cin,
+                               const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* stride,
+                               const int64_t* dilation, const int64_t* pad, int pad_mode, int dtype, float beta) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, nk_dtype_ok(dtype), "nk_conv_layer_nd_bwd_input: bad dtype %d", dtype);
+  LayerDims ld;
+  int rc = layer_dims(ctx, "nk_conv_layer_nd_bwd_input", nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, &ld);
+  if (rc) return rc;
+  int64_t total = n * cin;
+  for (int a = 0; a < nsp; ++a) total *= in_sp[a];
+  if (total == 0) return NK_OK;
+  NK_REQUIRE(ctx, dx && g && w, "nk_conv_layer_nd_bwd_input: NULL pointer");
+  if (dtype == NK_BF16 && ctx->conv_engine != NK_CONV_DIRECT) {
+    rc = nk_conv_gemm_nd_bwd_input(ctx, dx, g, w, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, beta);
+    if (rc != NK_ERR_UNSUPPORTED) return rc;
+  }
+  if (!ld.any_pad)
+    return nk_convnd_bwd_input(ctx, dx, g, w, nsp, n, cin, in_sp, cout, k, stride, dilation, 1, dtype, beta);
+  // the gradient of the padded input, then its interior slice (pad/mod.rs:157-182)
+  int64_t elems = n * cin;
+  for (int a = 0; a < nsp; ++a) elems *= ld.padded[a];
+  void* dxp = nullptr;
+  rc = nk_alloc_uninit(ctx, size_t(elems) * nk_dtype_size(dtype), &dxp);
+  if (rc) return rc;
+  rc = nk_convnd_bwd_input(ctx, dxp, g, w, nsp, n, cin, ld.padded, cout, k, stride, dilation, 1, dtype, 0.f);
+  if (rc == NK_OK) rc = nk_padnd_bwd(ctx, dx, dxp, n * cin, nsp, in_sp, pad, dtype, beta);
+  nk_free(ctx, dxp);
+  return rc;
+}
+
+int nk_conv_layer_nd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbias, const void* g, const void* x, int nsp,
+                                int64_t n, int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k,
+                                const int64_t* stride, const int64_t* dilation, const int64_t* pad, int pad_mode,
+                                float pad_value, int dtype, float beta) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, nk_dtype_ok(dtype) && nk_dtype_ok(dw_dtype), "nk_conv_layer_nd_bwd_kernel: bad dtype");
+  LayerDims ld;
+  int rc = layer_dims(ctx, "nk_conv_layer_nd_bwd_kernel", nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, &ld);
+  if (rc) return rc;
+  // an empty batch adds nothing: dW (and dbias) = beta * dW; g and x may then be NULL
+  NK_REQUIRE(ctx, dwt && (n == 0 || (g && x)), "nk_conv_layer_nd_bwd_kernel: NULL pointer");
+  int64_t bshape[4], gshape[5];
+  bias_shapes(ld.d, nsp, bshape, gshape);
+  if (dbias) {   // the composed graph's AdditionBackward: the un-broadcast of g onto (Cout, 1, ..)
+    rc = nk_unbroadcast_acc(ctx, dbias, dw_dtype, nsp + 1, bshape, g, dtype, nsp + 2, gshape, beta);
+    if (rc) return rc;
+  }
+  if (n > 0 && dtype == NK_BF16 && ctx->conv_engine != NK_CONV_DIRECT) {
+    rc = nk_conv_gemm_nd_bwd_kernel(ctx, dwt, dw_dtype, g, x, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode,
+                                    pad_value, beta);
+    if (rc != NK_ERR_UNSUPPORTED) return rc;
+  }
+  void* xp = nullptr;
+  if (n > 0 && ld.any_pad) {
+    rc = padded_copy(ctx, x, ld, nsp, in_sp, pad, pad_mode, pad_value, dtype, &xp);
+    if (rc) return rc;
+  }
+  rc = nk_convnd_bwd_kernel(ctx, dwt, dw_dtype, g, xp ? xp : x, nsp, n, cin, ld.padded, cout, k, stride, dilation, 1, dtype,
+                            beta);
+  nk_free(ctx, xp);
+  return rc;
 }
 
 }  // extern "C"

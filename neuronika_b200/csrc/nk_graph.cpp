@@ -1103,6 +1103,74 @@ struct ConvolutionNdBackward : Backward {  // convolution/mod.rs:357-510
   }
 };
 
+// ------------------------------------------------------------------------------- 1-d / 3-d convolution layer
+// nn.Conv1d / nn.Conv3d (neuronika-nn/src/lib.rs:630-916): pad -> convolution -> + bias as one node
+struct ConvLayerArgs {
+  int nsp, mode;
+  float value;
+  int64_t n, cin, cout;
+  int64_t in[3], k[3], s[3], d[3], pad[3];
+};
+struct ConvLayer : Forward {
+  TensorP input, weight, bias, data;  // bias may be null
+  ConvLayerArgs a;
+  ConvLayer(nk_ctx* c, TensorP x, TensorP w, TensorP b, TensorP d, const ConvLayerArgs& args)
+      : Forward(c), input(std::move(x)), weight(std::move(w)), bias(std::move(b)), data(std::move(d)), a(args) {}
+  const char* name() const override { return "ConvLayer"; }
+  void forward() override {
+    ck(ctx, nk_conv_layer_nd_fwd(ctx, data->wptr(), input->rptr(), weight->rptr(), bias ? bias->rptr() : nullptr, a.nsp, a.n,
+                                 a.cin, a.in, a.cout, a.k, a.s, a.d, a.pad, a.mode, a.value, data->dtype));
+  }
+};
+struct ConvLayerBackward : Backward {
+  TensorP input, weight;
+  GradientP input_grad, weight_grad, bias_grad;  // each may be null
+  ConvLayerArgs a;
+  ConvLayerBackward(nk_ctx* c, GradientP g, TensorP x, TensorP w, GradientP xg, GradientP wg, GradientP bg,
+                    const ConvLayerArgs& args)
+      : Backward(c, std::move(g)), input(std::move(x)), weight(std::move(w)), input_grad(std::move(xg)),
+        weight_grad(std::move(wg)), bias_grad(std::move(bg)), a(args) {}
+  const char* name() const override { return "ConvLayerBackward"; }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad, &weight_grad, &bias_grad}); }
+  void backward() override {
+    const void* g = gradient->get();   // a deferred root fill is materialised here
+    const int gdt = gradient->dtype;
+    if (input_grad) {
+      accumulate(ctx, input_grad, gdt, [&](void* d, float beta) {
+        ck(ctx, nk_conv_layer_nd_bwd_input(ctx, d, g, weight->rptr(), a.nsp, a.n, a.cin, a.in, a.cout, a.k, a.s, a.d, a.pad,
+                                           a.mode, gdt, beta));
+      });
+      grad_written(input_grad);
+    }
+    // the bias gradient rides along with dW when both have one element type and one accumulate mode
+    bool bias_done = false;
+    if (weight_grad) {
+      void* dbias = nullptr;
+      if (bias_grad && bias_grad->dtype == weight_grad->dtype) {
+        Gradient* wr = weight_grad->root();
+        Gradient* br = bias_grad->root();
+        if (!wr->is_const && !br->is_const && wr->is_zero == br->is_zero) {
+          float bbeta;
+          dbias = bias_grad->acc(&bbeta);
+          bias_done = true;
+        }
+      }
+      accumulate(ctx, weight_grad, [&](void* d, float beta) {
+        ck(ctx, nk_conv_layer_nd_bwd_kernel(ctx, d, weight_grad->dtype, dbias, g, input->rptr(), a.nsp, a.n, a.cin, a.in,
+                                            a.cout, a.k, a.s, a.d, a.pad, a.mode, a.value, gdt, beta));
+      });
+      grad_written(weight_grad);
+    }
+    if (bias_grad && !bias_done) {
+      accumulate(ctx, bias_grad, [&](void* d, float beta) {
+        ck(ctx, nk_unbroadcast_acc(ctx, d, bias_grad->dtype, (int)bias_grad->shape.size(), bias_grad->shape.data(), g, gdt,
+                                   (int)gradient->shape.size(), gradient->shape.data(), beta));
+      });
+    }
+    grad_written(bias_grad);
+  }
+};
+
 // ------------------------------------------------------------------------------- chunks (chunk/mod.rs)
 struct Chunk : Forward {
   TensorP operand, data;
@@ -1684,6 +1752,13 @@ Shape cobroadcast(const Shape& l, const Shape& r) {  // utils.rs:97-125
     }
   }
   return out;
+}
+
+// "(2, 3)" / "(4,)" in the messages of the shape checks
+std::string shape_str(const Shape& s) {
+  std::string out = "(";
+  for (size_t i = 0; i < s.size(); ++i) out += (i ? ", " : "") + std::to_string(s[i]);
+  return out + (s.size() == 1 ? ",)" : ")");
 }
 
 // Records one op: the result's history is the union of the operands' (History::merge) plus one node; its data is a
@@ -2388,6 +2463,53 @@ int nkg_convolution_nd(nkg_var* kernel, nkg_var* input, int nsp, const int64_t* 
   });
 }
 
+int nkg_conv_layer(nkg_var* input, nkg_var* weight, nkg_var* bias, int nsp, const int64_t* padding, int mode, float value,
+                   const int64_t* stride, const int64_t* dilation, nkg_var** out) {
+  return guard([&] {
+    not_null({input, weight, out, padding, stride, dilation}, "conv_layer");
+    if (nsp != 1 && nsp != 3) fail(NK_ERR_INVALID_ARG, "conv_layer: 1 or 3 sample dimensions (got %d)", nsp);
+    require_same_dtype(weight, input, "conv_layer");
+    if (bias) require_same_dtype(bias, input, "conv_layer");
+    const Shape &ks = weight->data->shape, &is = input->data->shape;
+    if ((int)is.size() != nsp + 2) fail(NK_ERR_INVALID_ARG, "conv_layer: input rank does not match %dd conv", nsp);
+    if (ks.size() != is.size()) fail(NK_ERR_INVALID_ARG, "Invalid kernel shape for %dd conv", nsp);
+    if (mode < NK_PAD_CONSTANT || mode > NK_PAD_REPLICATIVE) fail(NK_ERR_INVALID_ARG, "pad: bad mode %d", mode);
+    check_conv_channels(ks, is, 1);
+    ConvLayerArgs a;
+    a.nsp = nsp, a.mode = mode, a.value = value, a.n = is[0], a.cin = is[1], a.cout = ks[0];
+    Shape os{is[0], ks[0]};
+    for (int k = 0; k < nsp; ++k) {
+      if (padding[k] < 0) fail(NK_ERR_INVALID_ARG, "pad: padding must be >= 0");
+      if (mode == NK_PAD_REFLECTIVE && padding[k] > 0 && padding[k] >= is[2 + k])
+        fail(NK_ERR_INVALID_ARG, "pad: reflective padding %lld must be smaller than the dimension %lld",
+             (long long)padding[k], (long long)is[2 + k]);
+      if (stride[k] < 1 || dilation[k] < 1) fail(NK_ERR_INVALID_ARG, "Invalid stride/dilation for %dd conv.", nsp);
+      const int64_t padded = is[2 + k] + 2 * padding[k];
+      if (padded < (ks[2 + k] - 1) * dilation[k] + 1)
+        fail(NK_ERR_INVALID_ARG, "The kernel size can't be greater than actual input size.");
+      a.in[k] = is[2 + k], a.k[k] = ks[2 + k], a.s[k] = stride[k], a.d[k] = dilation[k], a.pad[k] = padding[k];
+      os.push_back((padded - dilation[k] * (ks[2 + k] - 1) - 1) / stride[k] + 1);
+    }
+    if (bias) {
+      Shape bs(nsp + 1, 1);
+      bs[0] = ks[0];
+      if (bias->data->shape != bs)
+        fail(NK_ERR_INVALID_ARG, "conv_layer: bias must be %s, got %s", shape_str(bs).c_str(), shape_str(bias->data->shape).c_str());
+    }
+    std::vector<nkg_var*> operands{input, weight};
+    if (bias) operands.push_back(bias);
+    *out = record(
+        operands, os, input->data->dtype,
+        [&](const TensorP& d) {
+          return std::make_shared<ConvLayer>(input->ctx, input->data, weight->data, bias ? bias->data : nullptr, d, a);
+        },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<ConvLayerBackward>(input->ctx, g, input->data, weight->data, input->grad, weight->grad,
+                                                     bias ? bias->grad : nullptr, a);
+        });
+  });
+}
+
 // ---------------------------------------------------------------- chunks / recurrent cells / sequence layers
 int nkg_chunks(nkg_var* a, int ndim, const int64_t* chunk_shape, int capacity, nkg_var** outs, int* count) {
   return guard([&] {
@@ -2517,11 +2639,6 @@ static std::vector<nkg_var*> check_rnn_operands(const char* who, bool lstm, bool
     if (a.v->ctx != x->ctx) fail(NK_ERR_INVALID_ARG, "%s: %s lives on another device than the input", who, a.name);
   }
   const int64_t G = lstm ? 4 : 3;
-  auto shape_str = [](const Shape& s) {
-    std::string out = "(";
-    for (size_t i = 0; i < s.size(); ++i) out += (i ? ", " : "") + std::to_string(s[i]);
-    return out + (s.size() == 1 ? ",)" : ")");
-  };
   const Shape& xs = x->data->shape;
   if (xs.size() != (seq ? 3u : 2u))
     fail(NK_ERR_INVALID_ARG, "%s: input must be %s, got %s", who, seq ? "(seq_len, batch, input_size)" : "(batch, input_size)",

@@ -1,5 +1,5 @@
-"""Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell and Conv2d (neuronika-nn/src/lib.rs:406-626, 724-815),
-and the sequence layers LSTM and GRU over them (stacked and bidirectional like torch.nn.LSTM / GRU)."""
+"""Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell, Conv1d, Conv2d and Conv3d (neuronika-nn/src/lib.rs:
+406-916), and the sequence layers LSTM and GRU over them (stacked and bidirectional like torch.nn.LSTM / GRU)."""
 from __future__ import annotations
 
 import math
@@ -17,14 +17,26 @@ def uniform(rng: np.random.Generator, shape, low: float, high: float) -> np.ndar
 
 class ZeroPad:
     """`Zero` padding mode (pad/zero/mod.rs:14-22)."""
-    value = 0.0
+    mode, value = "zero", 0.0
 
 
 class ConstantPad:
     """`Constant(value)` padding mode (pad/constant/mod.rs:14-39)."""
+    mode = "constant"
 
     def __init__(self, value: float):
         self.value = float(value)
+
+
+class ReflectivePad:
+    """`Reflective` padding mode (pad/reflective/mod.rs:14-31): the border mirrored without repeating the edge, like
+    numpy's "reflect"; the padding must be smaller than the padded dimension."""
+    mode, value = "reflective", 0.0
+
+
+class ReplicativePad:
+    """`Replicative` padding mode (pad/replicative/mod.rs:14-31): the edge element repeated, like numpy's "edge"."""
+    mode, value = "replicative", 0.0
 
 
 class Linear:
@@ -64,11 +76,75 @@ class Conv2d:
         self.bias = V.from_ndarray(device, uniform(rng, (out_channels, 1, 1), -k, k), dtype).requires_grad(grad_dtype)
 
     def forward(self, input: V.Var) -> V.VarDiff:
-        x = input.pad(self.padding, self.padding_mode.value) if any(self.padding) else input
+        mode = getattr(self.padding_mode, "mode", "constant")
+        if not any(self.padding):
+            x = input
+        elif mode in ("zero", "constant"):
+            x = input.pad(self.padding, self.padding_mode.value)
+        else:
+            x = input.pad(self.padding, mode=mode)
         return self.weight.convolution(x, self.stride, self.dilation, 1) + self.bias
 
     def parameters(self):
         return [self.weight, self.bias]
+
+
+class _ConvNd:
+    """The 1-D / 3-D convolution layers (neuronika-nn/src/lib.rs:630-723, 817-916): weight (Cout, Cin, k...), bias
+    (Cout, 1) / (Cout, 1, 1, 1), both ~ U(-k, k), k = sqrt(1/(Cin*prod(kernel))).  The reference's `forward` is
+    `todo!()`; the documented intent, pad(input) -> weight.convolution(padded, stride, dilation, 1) + bias, runs as ONE
+    graph node (variable.conv_layer): bf16 layers on the tensor cores with the padding applied inside the im2col gather,
+    so neither the padded input nor its gradient is ever stored.  The input gradient follows the reference's pad
+    backward: the interior slice of the padded input's gradient for every mode (torch folds the border gradient of
+    reflect / replicate padding back instead)."""
+
+    nsp = 0
+
+    def __init__(self, device: Device, in_channels: int, out_channels: int, kernel_size, padding, padding_mode, stride,
+                 dilation, dtype, grad_dtype, rng):
+        rng = rng or np.random.default_rng()
+        kernel = self._tuple(kernel_size, "kernel_size")
+        self.padding = self._tuple(padding, "padding")
+        self.stride = self._tuple(stride, "stride")
+        self.dilation = self._tuple(dilation, "dilation")
+        self.padding_mode = padding_mode or ZeroPad()
+        k = math.sqrt(1.0 / (in_channels * math.prod(kernel)))
+        self.weight = V.from_ndarray(device, uniform(rng, (out_channels, in_channels) + kernel, -k, k), dtype).requires_grad(grad_dtype)
+        self.bias = V.from_ndarray(device, uniform(rng, (out_channels,) + (1,) * self.nsp, -k, k), dtype).requires_grad(grad_dtype)
+
+    def _tuple(self, v, name):
+        t = (int(v),) * self.nsp if np.isscalar(v) else tuple(int(x) for x in v)
+        if len(t) != self.nsp:
+            raise ValueError(f"{name} must have {self.nsp} entries, got {t}")
+        return t
+
+    def forward(self, input: V.Var) -> V.VarDiff:
+        return V.conv_layer(input, self.weight, self.bias, self.padding, getattr(self.padding_mode, "mode", "constant"),
+                            self.padding_mode.value, self.stride, self.dilation)
+
+    def parameters(self):
+        return [self.weight, self.bias]
+
+
+class Conv1d(_ConvNd):
+    """1-D convolution over (N, Cin, L): kernel_size, padding, stride and dilation as ints or 1-tuples."""
+    nsp = 1
+
+    def __init__(self, device: Device, in_channels: int, out_channels: int, kernel_size, padding=0, padding_mode=None,
+                 stride=1, dilation=1, dtype=F32, grad_dtype=None, rng: np.random.Generator | None = None):
+        super().__init__(device, in_channels, out_channels, kernel_size, padding, padding_mode, stride, dilation, dtype,
+                         grad_dtype, rng)
+
+
+class Conv3d(_ConvNd):
+    """3-D convolution over (N, Cin, D, H, W): kernel_size, padding, stride and dilation as ints or 3-tuples."""
+    nsp = 3
+
+    def __init__(self, device: Device, in_channels: int, out_channels: int, kernel_size, padding=(0, 0, 0),
+                 padding_mode=None, stride=(1, 1, 1), dilation=(1, 1, 1), dtype=F32, grad_dtype=None,
+                 rng: np.random.Generator | None = None):
+        super().__init__(device, in_channels, out_channels, kernel_size, padding, padding_mode, stride, dilation, dtype,
+                         grad_dtype, rng)
 
 
 class LSTMCell:

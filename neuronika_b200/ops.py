@@ -409,6 +409,43 @@ def convnd_bwd_kernel(dw: CuArray, g: CuArray, x: CuArray, stride, dilation, gro
     return dw
 
 
+def _layer_args(x_shape, w_shape, stride, dilation, padding, mode):
+    nsp = len(x_shape) - 2
+    stride, dilation = stride or (1,) * nsp, dilation or (1,) * nsp
+    return [nsp, x_shape[0], x_shape[1], L.shape_arr(x_shape[2:]), w_shape[0], L.shape_arr(w_shape[2:]),
+            L.shape_arr(stride), L.shape_arr(dilation), L.shape_arr(padding), PAD[mode]]
+
+
+def conv_layer_nd(x: CuArray, w: CuArray, padding, mode="constant", value=0.0, stride=None, dilation=None, bias=None,
+                  out=None) -> CuArray:
+    """y = conv(pad(x, padding, mode), w) + bias for 1-D / 3-D x (nk_conv_layer_nd_fwd); bias (Cout) or None."""
+    stride, dilation = stride or (1,) * len(padding), dilation or (1,) * len(padding)
+    padded = x.shape[:2] + tuple(s + 2 * p for s, p in zip(x.shape[2:], padding))
+    out = out or CuArray(x.device, conv_out_shape(padded, w.shape, stride, dilation), x.dtype)
+    _ck(lib.nk_conv_layer_nd_fwd(x.device.ctx, out.ptr, x.ptr, w.ptr, _ptr(bias),
+                                 *_layer_args(x.shape, w.shape, stride, dilation, padding, mode), float(value), x.dtype),
+        x.device)
+    return out
+
+
+def conv_layer_nd_bwd_input(dx: CuArray, g: CuArray, w: CuArray, padding, mode="constant", stride=None, dilation=None,
+                            beta=1.0) -> CuArray:
+    """dx = beta*dx + the interior slice of the padded input's gradient (nk_conv_layer_nd_bwd_input)."""
+    _ck(lib.nk_conv_layer_nd_bwd_input(g.device.ctx, dx.ptr, g.ptr, w.ptr,
+                                       *_layer_args(dx.shape, w.shape, stride, dilation, padding, mode), g.dtype,
+                                       float(beta)), g.device)
+    return dx
+
+
+def conv_layer_nd_bwd_kernel(dw: CuArray, g: CuArray, x: CuArray, padding, mode="constant", value=0.0, stride=None,
+                             dilation=None, beta=1.0, dbias: CuArray | None = None) -> CuArray:
+    """dw = beta*dw + dW of the layer, and dbias likewise when given (nk_conv_layer_nd_bwd_kernel)."""
+    _ck(lib.nk_conv_layer_nd_bwd_kernel(g.device.ctx, dw.ptr, dw.dtype, _ptr(dbias), g.ptr, x.ptr,
+                                        *_layer_args(x.shape, dw.shape, stride, dilation, padding, mode), float(value),
+                                        g.dtype, float(beta)), g.device)
+    return dw
+
+
 # ---------------------------------------------------------------- 8-f: recurrent cells and chunks (csrc/nk_rnn.cu)
 def _ptr(a: CuArray | None):
     return a.ptr if a is not None else None

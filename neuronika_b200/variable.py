@@ -73,6 +73,7 @@ _G = {
     "nkg_vm": (i32, [vp, vp, pvp]),
     "nkg_vv": (i32, [vp, vp, pvp]),
     "nkg_convolution_nd": (i32, [vp, vp, i32, pi64, pi64, i64, pvp]),
+    "nkg_conv_layer": (i32, [vp, vp, vp, i32, pi64, i32, f32, pi64, pi64, pvp]),
     "nkg_adam_step": (i32, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, f32]),
     "nkg_rmsprop_step": (i32, [vp, vp, vp, vp, vp, f32, f32, f32, f32, f32, f32, f32]),
     "nkg_adagrad_step": (i32, [vp, vp, vp, i64, f32, f32, f32, f32, f32, f32]),
@@ -288,14 +289,10 @@ class Var:
     def pad(self, padding, value: float = 0.0, mode: str = "constant"):
         """`pad(padding, mode)` (var.rs:726-737): Zero / Constant(value) / Reflective / Replicative over the 1..3
         sample dimensions of a (N, C, ...) operand."""
-        modes = {"constant": L.NK_PAD_CONSTANT, "zero": L.NK_PAD_CONSTANT, "reflective": L.NK_PAD_REFLECTIVE,
-                 "replicative": L.NK_PAD_REPLICATIVE}
-        if mode not in modes:
-            raise L.NkError(-1, f"unknown padding mode {mode!r}")
         padding = tuple(int(p) for p in padding)
-        if len(padding) == 2 and modes[mode] == L.NK_PAD_CONSTANT:
+        if len(padding) == 2 and _pad_mode(mode) == L.NK_PAD_CONSTANT:
             return self._unary(lib.nkg_pad, padding[0], padding[1], float(value))
-        return self._unary(lib.nkg_pad_mode, len(padding), L.shape_arr(padding), modes[mode], float(value))
+        return self._unary(lib.nkg_pad_mode, len(padding), L.shape_arr(padding), _pad_mode(mode), float(value))
 
     def convolution(self, input, stride=(1, 1), dilation=(1, 1), groups: int = 1):
         """`kernel.convolution(input, stride, dilation, groups)` -- the receiver is the kernel
@@ -403,6 +400,36 @@ class VarDiff(Var):
         cb = GRAD_RS_HOOK(lambda _user, pushed: fn(int(pushed)))
         self._rs_ref = (cb, arr)
         _ck(lib.nkg_set_grad_rs(self._h, int(world), int(rank), arr, C.cast(cb, vp), None))
+
+
+_PAD_MODES = {"constant": L.NK_PAD_CONSTANT, "zero": L.NK_PAD_CONSTANT, "reflective": L.NK_PAD_REFLECTIVE,
+              "replicative": L.NK_PAD_REPLICATIVE}
+
+
+def _pad_mode(mode: str) -> int:
+    if mode not in _PAD_MODES:
+        raise L.NkError(-1, f"unknown padding mode {mode!r}")
+    return _PAD_MODES[mode]
+
+
+# ---- the 1-d / 3-d convolution layer (one node; see include/nk_graph.h nkg_conv_layer)
+def conv_layer(input: Var, weight: Var, bias: Var | None, padding, mode: str = "zero", value: float = 0.0, stride=None,
+               dilation=None):
+    """`conv(pad(input, padding, mode), weight, stride, dilation) + bias` as ONE node, for input (N, Cin, L) or
+    (N, Cin, D, H, W): weight (Cout, Cin, k...), bias (Cout, 1) / (Cout, 1, 1, 1) or None.  `mode` is one of
+    Var.pad's modes ("zero", "constant" with `value`, "reflective", "replicative").  The same results as those three
+    nodes; the input gradient is the interior slice of the padded input's gradient for every mode, as in Var.pad."""
+    nsp = len(input.shape) - 2
+    padding = tuple(int(p) for p in padding)
+    stride = tuple(int(s) for s in (stride or (1,) * nsp))
+    dilation = tuple(int(d) for d in (dilation or (1,) * nsp))
+    for name, t in (("padding", padding), ("stride", stride), ("dilation", dilation)):
+        if len(t) != nsp:
+            raise L.NkError(-1, f"Invalid {name} {list(t)} for {nsp}d conv.")
+    out = vp()
+    _ck(lib.nkg_conv_layer(input._h, weight._h, bias._h if bias is not None else None, nsp, L.shape_arr(padding),
+                           _pad_mode(mode), float(value), L.shape_arr(stride), L.shape_arr(dilation), C.byref(out)))
+    return input._wrap(out)
 
 
 # ---- concatenation (neuronika-variable/src/lib.rs:258, 281)
