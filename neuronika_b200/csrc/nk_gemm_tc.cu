@@ -16,9 +16,12 @@
 //                    between k-blocks (the consumer holds two slots; the producer prefetches kStages - 2 ahead).
 //                    Then the epilogue, one of two:
 //                    - TMA store (column bias, alpha, ReLU, beta == 0, no mask / column sums / reduce-scatter, C
-//                      TMA-addressable): the fragments are converted to C's type straight into one of two 128B-swizzled
-//                      64-row x 128-byte staging buffers per warpgroup and written by cp.async.bulk.tensor stores that
-//                      drain while the warpgroup already runs the next tile's main loop;
+//                      TMA-addressable): every warp converts its 16 rows of fragments to C's type straight into one of
+//                      two 128B-swizzled 16-row x 128-byte staging buffers of its own (stmatrix for bf16) and writes
+//                      them with cp.async.bulk.tensor stores it issues itself, so the warps of a warpgroup never wait
+//                      for each other; the stores drain while the warpgroup already runs the next tile's main loop.
+//                      A bf16 column bias is copied into shared memory by the producer with the tile's first k-block,
+//                      so the epilogue reads it without a global-memory round trip;
 //                    - the drain: through a swizzled shared-memory stage, alpha/bias/ReLU, mask, beta, column sums,
 //                      reduce-scatter over NVLink and batched outputs as 16-byte global stores per row.
 // Pipeline: smem full/empty mbarriers (TMA <-> the two consumer warpgroups); bulk async-groups for the output stores.
@@ -65,6 +68,8 @@ struct GemmParams {
   int batch, a_batched, b_batched, batch_reduce, splits;
   int64_t c_batch_stride;
   int tma_store;   // the epilogue writes C through the C tensor map (see the header); the host checks the conditions
+  int bias_stage;  // TMA-store epilogue: the producer copies each tile's slice of the (bf16, 16-byte aligned, N % 8 == 0)
+                   // column bias into shared memory
   int64_t bias_batch_stride;   // the bias of product b starts this many elements further (nk_gemm_strided_batched)
 };
 
@@ -100,10 +105,11 @@ struct Cfg {
   static constexpr uint32_t A_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
   static constexpr uint32_t B_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  // after the ring: 1 KB of barriers, then kEpiStageBytes of epilogue staging
-  static constexpr int kStagesMax = (kSmemLimit - 2048 - kEpiStageBytes) / STAGE_BYTES;
+  // after the ring: 1 KB of barriers, kEpiStageBytes of epilogue staging, then two BLOCK_N-wide bf16 bias slots (1 KB)
+  static constexpr int kStagesMax = (kSmemLimit - 3072 - kEpiStageBytes) / STAGE_BYTES;
   static constexpr int kStages = kStagesMax > 8 ? 8 : kStagesMax;
-  static constexpr uint32_t SMEM_BYTES = kStages * STAGE_BYTES + 2048 + kEpiStageBytes;  // + alignment slack + barriers
+  static constexpr uint32_t SMEM_BYTES = kStages * STAGE_BYTES + 3072 + kEpiStageBytes;  // + alignment slack + barriers
+  static_assert(2 * BLOCK_N * 2 <= 1024, "bias slots");
 };
 
 // v[j] = alpha * acc[j] + bias (row- or column-indexed) for one 32-column chunk of one output row.  The product is
@@ -285,10 +291,77 @@ __device__ __forceinline__ float col_bias(const GemmParams& p, int64_t col) {
 }
 
 // one output value of the TMA-store epilogue: the drain's alpha (rounded product), bias and ReLU
+template <bool kAddBias>
 __device__ __forceinline__ float epi_value(const GemmParams& p, float acc, float bias) {
   float v = __fmul_rn(p.alpha, acc);
-  if (p.bias) v += bias;
+  if (kAddBias) v += bias;
   return p.relu ? (v > 0.f ? v : 0.f) : v;
+}
+
+// where the TMA-store epilogue takes the column bias from
+enum { kBiasNone, kBiasStaged, kBiasLoaded };
+
+// TMA-store epilogue of one tile, per warp: chunk ch = columns [ch kStoreCols, +kStoreCols) of the warp's 16 rows.
+// Lane holds rows r, r + 8 (r = lane / 4) and columns 8 jj + 2 (lane & 3) + {0, 1} of each 8-column block jj; they go,
+// converted, to the 128B-swizzled layout of the C tensor map's 16-row box (16-byte unit u of row r at unit u ^ (r & 7);
+// conflict-free: the eight rows of one 8 x 8 block hit eight different units).  Lane 0 issues and waits for the warp's
+// own bulk stores, so a __syncwarp is all the hand-off a chunk needs.  The bias source is a template parameter: with a
+// run-time choice inside the chunk loop the bias-free NN form paid about 2.5 kcycles more per tile (H100 SXM, 700 W)
+template <int BLOCK_N, typename TC, int kBias>
+__device__ __forceinline__ void tma_store_tile(const GemmParams& p, const CUtensorMap* tmap_c, const float (&acc)[BLOCK_N / 2],
+                                               int lane, int row0, int64_t n0, uint32_t stg0, uint32_t bias_s,
+                                               uint32_t& store_buf) {
+  constexpr int kStoreCols = 128 / int(sizeof(TC));
+  const int r = lane >> 2;
+  const int q = lane & 3;
+  // stmatrix: lanes 8i .. 8i + 7 address the rows of matrix i = (rows 8 (i & 1) + [0, 8), 8-column block jj + (i >> 1))
+  // of a pair of blocks jj, jj + 1
+  const int sm_row = (lane & 7) + ((lane >> 3) & 1) * 8;
+  const int sm_blk = lane >> 4;
+#pragma unroll
+  for (int ch = 0; ch < BLOCK_N / kStoreCols; ++ch) {
+    const uint32_t buf = stg0 + store_buf * (64 * 128);
+    if (lane == 0) ptx::tma_store_wait_read<1>();   // the store that last read this buffer is done with it
+    __syncwarp();
+    const int64_t col0 = n0 + ch * kStoreCols;
+    uint32_t packed[4];   // bf16: blocks jj - 1 and jj, rows r and r + 8, for one stmatrix per pair of blocks
+#pragma unroll
+    for (int jj = 0; jj < kStoreCols / 8; ++jj) {
+      const int j = (ch * (kStoreCols / 8) + jj) * 4;   // acc[j..j+1]: row r, acc[j+2..j+3]: row r + 8
+      float b0 = 0.f, b1 = 0.f;
+      if constexpr (kBias == kBiasStaged) {
+        const uint32_t w = ptx::ld_shared_b32(bias_s + uint32_t(ch * kStoreCols + jj * 8 + 2 * q) * 2);
+        b0 = __uint_as_float(w << 16), b1 = __uint_as_float(w & 0xffff0000u);
+      } else if constexpr (kBias == kBiasLoaded) {
+        const int64_t col = col0 + jj * 8 + 2 * q;
+        b0 = col_bias(p, col), b1 = col_bias(p, col + 1);
+      }
+      constexpr bool kAdd = kBias != kBiasNone;
+      const float v0 = epi_value<kAdd>(p, acc[j], b0), v1 = epi_value<kAdd>(p, acc[j + 1], b1);
+      const float v2 = epi_value<kAdd>(p, acc[j + 2], b0), v3 = epi_value<kAdd>(p, acc[j + 3], b1);
+      if constexpr (sizeof(TC) == 2) {
+        const __nv_bfloat162 lo = __floats2bfloat162_rn(v0, v1), hi = __floats2bfloat162_rn(v2, v3);
+        packed[2 * (jj & 1)] = *reinterpret_cast<const uint32_t*>(&lo);
+        packed[2 * (jj & 1) + 1] = *reinterpret_cast<const uint32_t*>(&hi);
+        if (jj & 1) {
+          const uint32_t off = sm_row * 128 + (((jj - 1 + sm_blk) ^ (sm_row & 7)) << 4);
+          ptx::stmatrix_x4(buf + off, packed[0], packed[1], packed[2], packed[3]);
+        }
+      } else {
+        // two f32 per row and block (stmatrix is b16 only): 8-byte stores, the eight rows of a store on distinct units
+        const uint32_t off = r * 128 + (((2 * jj + (q >> 1)) ^ r) << 4) + (q & 1) * 8;
+        ptx::st_shared_v2_f32(buf + off, v0, v1);
+        ptx::st_shared_v2_f32(buf + off + 8 * 128, v2, v3);
+      }
+    }
+    ptx::fence_proxy_async();   // the staged chunk is visible to the TMA unit ...
+    __syncwarp();
+    if (lane == 0) {            // ... which clips the box at M, N (the ldc - N gap is never written)
+      if (row0 < p.M && col0 < p.N) ptx::tma_store_2d(tmap_c, buf, int(col0), row0);
+      ptx::tma_store_commit();   // (an empty group when nothing was issued: one group per chunk)
+    }
+    store_buf ^= 1u;
+  }
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false, bool BATCH_BIAS = false>
@@ -297,8 +370,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
   using C_ = Cfg<BLOCK_N>;
   constexpr int kStages = C_::kStages;
-  // TMA-store epilogue: chunks of one 128-byte swizzle row (64 bf16 / 32 f32 columns) x 64 rows, two 8 KB staging
-  // buffers per consumer warpgroup in its half of the epilogue stage
+  // TMA-store epilogue: chunks of one 128-byte swizzle row (64 bf16 / 32 f32 columns) x 16 rows per warp, two 2 KB
+  // staging buffers per consumer warp (two 8 KB buffers per warpgroup in its half of the epilogue stage)
   constexpr int kStoreCols = 128 / int(sizeof(TC));
   constexpr bool kTmaStore = !BATCH && BLOCK_N % kStoreCols == 0;
   static_assert(2 * 2 * 64 * 128 <= kEpiStageBytes, "staging buffers");
@@ -309,8 +382,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   const uint32_t bar_base = smem_base + kStages * C_::STAGE_BYTES;  // 8-byte aligned
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
+  // bias slot s (tiles of even / odd local index) is free again once all eight consumer warps have read it
+  auto bias_empty_bar = [&](int s) { return bar_base + 8u * (2 * kStages + s); };
   const uint32_t epi_stage = bar_base + 1024;
   float* epi = reinterpret_cast<float*>(smem_raw + (epi_stage - ptx::smem_u32(smem_raw)));
+  auto bias_slot = [&](int s) { return epi_stage + kEpiStageBytes + uint32_t(s) * (BLOCK_N * 2); };
+  const bool stage_bias = kTmaStore && p.tma_store && p.bias_stage;
 
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
@@ -323,6 +400,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       ptx::mbar_init(full_bar(s), 1);
       ptx::mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
     }
+    for (int s = 0; s < 2; ++s) ptx::mbar_init(bias_empty_bar(s), 8);   // one arrive per consumer warp
     ptx::fence_barrier_init();
   }
   __syncthreads();
@@ -346,7 +424,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x, local = 0; tile < num_tiles; tile += gridDim.x, ++local) {
         int m_blk, n_blk, b0 = 0, b1 = 1;
         tile_coords(p, BATCH ? tile % tiles_mn : tile, m_blk, n_blk);
         if (BATCH) batch_range(tile / tiles_mn, b0, b1);
@@ -354,7 +432,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         for (int bb = b0; bb < b1; ++bb)
         for (int kb = 0; kb < p.num_k_blocks; ++kb) {
           ptx::mbar_wait_spin(empty_bar(stage), phase ^ 1u);
-          ptx::mbar_expect_tx(full_bar(stage), C_::STAGE_BYTES);
+          if (stage_bias && kb == 0) {
+            // the tile's bias slice rides on its first k-block's barrier.  With one or two k-blocks per tile this thread
+            // can run more than a tile ahead of the consumers: the slot is reused only after they have read it
+            const int s = local & 1;
+            const uint32_t bytes = 2u * uint32_t(min(int64_t(BLOCK_N), p.N - n0));   // a multiple of 16: N % 8 == 0
+            ptx::mbar_wait_spin(bias_empty_bar(s), ((local >> 1) & 1) ^ 1u);
+            ptx::mbar_expect_tx(full_bar(stage), C_::STAGE_BYTES + bytes);
+            ptx::bulk_load(bias_slot(s), static_cast<const __nv_bfloat16*>(p.bias) + n0, bytes, full_bar(stage));
+          } else {
+            ptx::mbar_expect_tx(full_bar(stage), C_::STAGE_BYTES);
+          }
           const int k0 = kb * BLOCK_K;
           const uint32_t sa = smem_a0 + stage * C_::A_BYTES;
           const uint32_t sb = smem_b0 + stage * C_::B_BYTES;
@@ -410,7 +498,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   int stage = 0;
   uint32_t phase = 0;
   uint32_t store_buf = 0;   // TMA-store epilogue: the staging buffer the next chunk goes to
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  for (int tile = blockIdx.x, local = 0; tile < num_tiles; tile += gridDim.x, ++local) {
     int m_blk, n_blk;
     tile_coords(p, BATCH ? tile % tiles_mn : tile, m_blk, n_blk);
     int k_total = p.num_k_blocks;
@@ -446,46 +534,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 
     if constexpr (kTmaStore) {
       if (p.tma_store) {
-        // ---- TMA-store epilogue: chunk ch = columns [ch kStoreCols, +kStoreCols) of this warpgroup's 64 rows.  Thread
-        // (warp w, lane) holds rows fr, fr + 8 and columns 8 jj + 2 (lane & 3) + {0, 1} of each 8-column block jj; it
-        // writes them, converted, to the 128B-swizzled layout of the C tensor map's box (16-byte unit u of row r at
-        // unit u ^ (r & 7); conflict-free: the eight rows of a warp's store hit eight different units)
-        const int fr = warp * 16 + (lane >> 2);
-        const int q = lane & 3;
-        const int row0 = m_blk * BLOCK_M + cw * 64;
-        const uint32_t stg0 = epi_stage + uint32_t(cw) * (2 * 64 * 128);
-#pragma unroll
-        for (int ch = 0; ch < BLOCK_N / kStoreCols; ++ch) {
-          const uint32_t buf = stg0 + store_buf * (64 * 128);
-          if (t == 0) ptx::tma_store_wait_read<1>();   // the store that last read this buffer is done with it
-          ptx::named_barrier(1 + cw, 128);
-          const int64_t col0 = int64_t(n_blk) * BLOCK_N + ch * kStoreCols;
-#pragma unroll
-          for (int jj = 0; jj < kStoreCols / 8; ++jj) {
-            const int j = (ch * (kStoreCols / 8) + jj) * 4;   // acc[j..j+1]: row fr, acc[j+2..j+3]: row fr + 8
-            const int64_t col = col0 + jj * 8 + 2 * q;
-            float b0 = 0.f, b1 = 0.f;
-            if (p.bias) b0 = col_bias(p, col), b1 = col_bias(p, col + 1);
-            const float v0 = epi_value(p, acc[j], b0), v1 = epi_value(p, acc[j + 1], b1);
-            const float v2 = epi_value(p, acc[j + 2], b0), v3 = epi_value(p, acc[j + 3], b1);
-            if constexpr (sizeof(TC) == 2) {
-              const uint32_t off = fr * 128 + ((jj ^ (fr & 7)) << 4) + 4 * q;
-              const __nv_bfloat162 lo = __floats2bfloat162_rn(v0, v1), hi = __floats2bfloat162_rn(v2, v3);
-              ptx::st_shared_b32(buf + off, *reinterpret_cast<const uint32_t*>(&lo));
-              ptx::st_shared_b32(buf + off + 8 * 128, *reinterpret_cast<const uint32_t*>(&hi));
-            } else {
-              const uint32_t off = fr * 128 + (((2 * jj + (q >> 1)) ^ (fr & 7)) << 4) + (q & 1) * 8;
-              ptx::st_shared_v2_f32(buf + off, v0, v1);
-              ptx::st_shared_v2_f32(buf + off + 8 * 128, v2, v3);
-            }
-          }
-          ptx::fence_proxy_async();   // the staged chunk is visible to the TMA unit ...
-          ptx::named_barrier(1 + cw, 128);
-          if (t == 0) {               // ... which clips the box at M, N (the ldc - N gap is never written)
-            if (row0 < p.M && col0 < p.N) ptx::tma_store_2d(&tmap_c, buf, int(col0), row0);
-            ptx::tma_store_commit();   // (an empty group when nothing was issued: one group per chunk)
-          }
-          store_buf ^= 1u;
+        // ---- TMA-store epilogue (tma_store_tile), each warp on its own two 16-row staging buffers
+        const int row0 = m_blk * BLOCK_M + cw * 64 + warp * 16;
+        const int64_t n0 = int64_t(n_blk) * BLOCK_N;
+        const uint32_t stg0 = epi_stage + uint32_t(cw) * (2 * 64 * 128) + uint32_t(warp) * (16 * 128);
+        const uint32_t bias_s = bias_slot(local & 1);
+        if (stage_bias)
+          tma_store_tile<BLOCK_N, TC, kBiasStaged>(p, &tmap_c, acc, lane, row0, n0, stg0, bias_s, store_buf);
+        else if (p.bias)
+          tma_store_tile<BLOCK_N, TC, kBiasLoaded>(p, &tmap_c, acc, lane, row0, n0, stg0, bias_s, store_buf);
+        else
+          tma_store_tile<BLOCK_N, TC, kBiasNone>(p, &tmap_c, acc, lane, row0, n0, stg0, bias_s, store_buf);
+        if (stage_bias) {   // this warp is done with the tile's bias slot
+          __syncwarp();
+          if (lane == 0) ptx::mbar_arrive(bias_empty_bar(local & 1));
         }
         continue;   // the stores drain while the next tile's main loop runs
       }
@@ -566,7 +628,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       }
     }
   }
-  if (kTmaStore && p.tma_store && t == 0) ptx::tma_store_wait<0>();   // the staging buffers outlive the last stores
+  if (kTmaStore && p.tma_store && lane == 0) ptx::tma_store_wait<0>();   // the staging buffers outlive the last stores
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -736,7 +798,7 @@ int nk_gemm_wgmma(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int
     rc = make_tmap_2d(ctx, &tb, B, N, K, ldb, BLOCK_K, (uint32_t)block_n);
   if (rc) return rc;
   // TMA-store epilogue: an output the epilogue only writes (beta 0; alpha, column bias and ReLU are applied on the way)
-  // and that TMA can address; box = one 64-row x 128-byte staging buffer, whole chunks per tile.  The rows must also end
+  // and that TMA can address; box = one warp's 16-row x 128-byte staging buffer, whole chunks per tile.  The rows must also end
   // on a 16-byte boundary: a store box clips at the last row exactly but at the last column only to the 16-byte unit
   // that holds it, which would write into the ldc - N gap
   const int64_t c_size = int64_t(nk_dtype_size(c_dtype));
@@ -745,9 +807,12 @@ int nk_gemm_wgmma(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int
   p.tma_store = beta == 0.f && !mask && !colsum && !p.rs_world && (block_n * c_size) % 128 == 0 &&
                 (reinterpret_cast<uintptr_t>(C) & 15) == 0 && (ldc * c_size) % 16 == 0 && (N * c_size) % 16 == 0;
   if (p.tma_store) {
-    rc = make_tmap_2d(ctx, &tc, C, M, N, ldc, uint32_t(128 / c_size), 64, c_dtype);
+    rc = make_tmap_2d(ctx, &tc, C, M, N, ldc, uint32_t(128 / c_size), 16, c_dtype);
     if (rc) return rc;
   }
+  // a bias slice every tile can fetch with one bulk copy: bf16 (f32 would not fit the slots), 16-byte aligned, and
+  // N % 8 == 0 so that the last tile's slice is a whole number of 16-byte units; otherwise the epilogue loads it
+  p.bias_stage = p.tma_store && bias && bias_dtype == NK_BF16 && (reinterpret_cast<uintptr_t>(bias) & 15) == 0 && N % 8 == 0;
 
   static const char* names[2][2][5] = {
       {{"wgmma_nt_128x256", "wgmma_nt_128x128", "wgmma_nt_128x64", "wgmma_nt_128x32", "wgmma_nt_128x16"},
@@ -811,6 +876,7 @@ static int gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, in
   p.batch = int(batch), p.a_batched = strideA != 0, p.b_batched = strideB != 0, p.batch_reduce = reduce ? 1 : 0, p.splits = 1;
   p.c_batch_stride = strideC;
   p.tma_store = 0;   // batched outputs (and the row-indexed bias) keep the drain
+  p.bias_stage = 0;
   p.a_lbo = a_mn ? BLOCK_K * 128 : 16, p.a_sbo = 1024, p.a_kstep = a_mn ? WGMMA_K * 128 : WGMMA_K * 2;
   p.b_lbo = b_mn ? BLOCK_K * 128 : 16, p.b_sbo = 1024, p.b_kstep = b_mn ? WGMMA_K * 128 : WGMMA_K * 2;
   CUtensorMap ta, tb;

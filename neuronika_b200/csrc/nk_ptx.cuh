@@ -123,6 +123,12 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const CUtensorMap
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// non-tensor bulk copy global -> shared (bytes, addresses: multiples of 16), completing on an mbarrier's tx count
+__device__ __forceinline__ void bulk_load(uint32_t smem_dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_dst),
+               "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(bar)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tmap, uint32_t smem_src, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(tmap)),
@@ -142,6 +148,19 @@ __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
 }
 __device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float x, float y) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+// four 8 x 8 b16 matrices: lanes 8i .. 8i + 7 give the addresses of matrix i's rows (16 bytes each), and every lane
+// holds row lane / 4, columns 2 (lane % 4) + {0, 1} of matrix i in r_i -- the wgmma accumulator fragment of one
+// 8-column block, converted to bf16x2
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
 }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
