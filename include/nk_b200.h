@@ -50,6 +50,13 @@ typedef enum { NK_F32 = 0, NK_BF16 = 1 } nk_dtype;
 /* GEMM engine selection (nk_gemm_config): AUTO picks the wgmma tensor-core engine
  * whenever the operands are bf16 and TMA-addressable, else the SIMT kernel. */
 typedef enum { NK_GEMM_AUTO = 0, NK_GEMM_SIMT = 1, NK_GEMM_TC = 2, NK_GEMM_TCGEN05 = NK_GEMM_TC /* former name */ } nk_gemm_engine;
+/* How f32 products use the tensor cores (nk_gemm_f32_config).  IEEE (the default): f32 operands run on the CUDA cores,
+ * as they always did.  TF32: every operand element is rounded to TF32 (cvt.rna: to nearest, ties away from zero) and the
+ * product runs on the wgmma engine with f32 accumulation.  TF32X3: each element x is split into hi = tf32(x) and
+ * lo = tf32(x - hi), and C = A_hi.B_hi + A_hi.B_lo + A_lo.B_hi (the lo.lo term, ~2^-22 of each product, is dropped):
+ * close to f32 accuracy, at about a fifth of the TF32 rate (README).  The mode is read when a GEMM is called; a captured step keeps the
+ * mode it was captured with. */
+typedef enum { NK_F32_GEMM_IEEE = 0, NK_F32_GEMM_TF32 = 1, NK_F32_GEMM_TF32X3 = 2 } nk_f32_gemm_mode;
 /* Convolution engine selection (nk_conv_config): AUTO = tensor-core kernels wherever they apply; DIRECT = the CUDA-core
  * kernels only (the parity path the reference's goldens run on); UNFUSED = AUTO (the backward runs dW and dX as two
  * products on every engine). */
@@ -69,6 +76,10 @@ uint64_t nk_launch_count(nk_ctx* ctx);
 int nk_sm_count(nk_ctx* ctx);
 int nk_gemm_config(nk_ctx* ctx, int engine /* nk_gemm_engine */);
 int nk_conv_config(nk_ctx* ctx, int engine /* nk_conv_engine */);
+/* f32 products of nk_gemm / nk_gemm_bias_act / nk_gemm_strided_batched / nk_gemm_relu_bwd (and every graph node built on
+ * them) in `mode` (nk_f32_gemm_mode).  The GEMM engine setting wins: NK_GEMM_SIMT keeps every product on the CUDA cores.
+ * Errors: NK_ERR_INVALID_ARG for an unknown mode. */
+int nk_gemm_f32_config(nk_ctx* ctx, int mode /* nk_f32_gemm_mode */);
 /* name of the kernel variant the last nk_gemm call used ("wgmma_nt_128x256", "simt", ...) */
 const char* nk_last_gemm_kernel(nk_ctx* ctx);
 

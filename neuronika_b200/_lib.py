@@ -55,6 +55,7 @@ _PROTOS = {
     "nk_launch_count": (u64, [vp]),
     "nk_sm_count": (i32, [vp]),
     "nk_gemm_config": (i32, [vp, i32]),
+    "nk_gemm_f32_config": (i32, [vp, i32]),
     "nk_conv_config": (i32, [vp, i32]),
     "nk_last_gemm_kernel": (C.c_char_p, [vp]),
     "nk_last_conv_kernel": (C.c_char_p, [vp]),

@@ -179,6 +179,12 @@ int nk_gemm_config(nk_ctx* ctx, int engine) {
   ctx->gemm_engine = engine;
   return NK_OK;
 }
+int nk_gemm_f32_config(nk_ctx* ctx, int mode) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, mode >= NK_F32_GEMM_IEEE && mode <= NK_F32_GEMM_TF32X3, "nk_gemm_f32_config: bad mode %d", mode);
+  ctx->f32_gemm = mode;
+  return NK_OK;
+}
 int nk_conv_config(nk_ctx* ctx, int engine) {
   if (!ctx) return NK_ERR_INVALID_ARG;
   NK_REQUIRE(ctx, engine >= NK_CONV_AUTO && engine <= NK_CONV_UNFUSED, "nk_conv_config: bad engine %d", engine);

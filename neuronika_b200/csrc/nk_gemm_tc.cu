@@ -631,6 +631,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   if (kTmaStore && p.tma_store && lane == 0) ptx::tma_store_wait<0>();   // the staging buffers outlive the last stores
 }
 
+}  // namespace
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -638,7 +640,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 // 2-D tensor map (bf16 or f32 elements): `rows` x `cols` row-major with leading dimension ld, box (box_cols, box_rows)
 // with box_cols elements = 128 bytes, 128B-swizzled
 int make_tmap_2d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t rows, int64_t cols, int64_t ld,
-                 uint32_t box_cols, uint32_t box_rows, int dtype = NK_BF16) {
+                 uint32_t box_cols, uint32_t box_rows, int dtype) {
   if (!ctx->encode_tiled) return nk_set_error(ctx, NK_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * nk_dtype_size(dtype)};
@@ -654,6 +656,8 @@ int make_tmap_2d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t rows, i
                         (long long)rows, (long long)cols, (long long)ld);
   return NK_OK;
 }
+
+namespace {
 
 template <int BLOCK_N, bool A_MN, bool B_MN, typename TC, bool BATCH = false, bool BATCH_BIAS = false>
 int launch_cfg(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, GemmParams& p) {
@@ -922,6 +926,13 @@ int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_
                             c_dtype, row_bias, bias_dtype, 1, 0, relu, reduce);
 }
 
+// f32 products go to the tf32 engine (nk_gemm_tf32.cu) in a non-IEEE f32 mode unless the SIMT engine is forced; the
+// data-parallel reduce-scatter epilogue (ctx->rs_world) exists on the bf16 engine only
+static bool f32_on_tensor_cores(const nk_ctx* ctx, int ab_dtype, int64_t K) {
+  return ab_dtype == NK_F32 && ctx->f32_gemm != NK_F32_GEMM_IEEE && ctx->gemm_engine != NK_GEMM_SIMT && K > 0 &&
+         ctx->rs_world == 0;
+}
+
 extern "C" {
 
 int nk_gemm_bias_act(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha,
@@ -936,6 +947,9 @@ int nk_gemm_bias_act(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, 
              "nk_gemm: leading dimension too small (lda=%lld ldb=%lld ldc=%lld for M=%lld N=%lld K=%lld tA=%d tB=%d)",
              (long long)lda, (long long)ldb, (long long)ldc, (long long)M, (long long)N, (long long)K, transA, transB);
   NK_REQUIRE(ctx, !bias || nk_dtype_ok(bias_dtype), "nk_gemm: bad bias dtype");
+  // f32 operands in TF32 / 3xTF32 mode: every shape goes to the tf32 engine (it packs whatever TMA cannot read)
+  if (f32_on_tensor_cores(ctx, ab_dtype, K))
+    return nk_gemm_tf32(ctx, transA, transB, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, c_dtype, bias, bias_dtype, relu);
   const bool want_tc = ab_dtype == NK_BF16 && ctx->gemm_engine != NK_GEMM_SIMT && K > 0;
   if (want_tc) {
     int rc = nk_gemm_wgmma(ctx, transA, transB, M, N, K, alpha, A, lda, B, ldb, beta, C, ldc, c_dtype, bias,
@@ -1008,11 +1022,16 @@ int nk_gemm_relu_bwd_colsum(nk_ctx* ctx, int transA, int transB, int64_t M, int6
     if (rc != NK_ERR_UNSUPPORTED) return rc;
   }
   if (colsum) return NK_ERR_UNSUPPORTED;   // nothing done: the caller sums the columns itself after the plain call
-  // operands the tensor-core engine cannot take: the product into a temporary, then the ordinary ReLU backward
+  // operands the tensor-core engine cannot take: the product into a temporary, then the ordinary ReLU backward.  The
+  // product of f32 operands in TF32 / 3xTF32 mode runs on the tf32 engine (the skinny K <= 16 kernel above stays on the
+  // CUDA cores in every mode: it masks and sums in its own epilogue)
   void* tmp = nullptr;
   int rc = nk_alloc_uninit(ctx, size_t(M) * size_t(N) * nk_dtype_size(c_dtype), &tmp);
   if (rc) return rc;
-  rc = nk_gemm_simt(ctx, transA, transB, M, N, K, 1.f, A, lda, B, ldb, 0.f, tmp, N, ab_dtype, c_dtype, nullptr, NK_F32, 0);
+  if (f32_on_tensor_cores(ctx, ab_dtype, K))
+    rc = nk_gemm_tf32(ctx, transA, transB, M, N, K, 1.f, A, lda, B, ldb, 0.f, tmp, N, c_dtype, nullptr, NK_F32, 0);
+  else
+    rc = nk_gemm_simt(ctx, transA, transB, M, N, K, 1.f, A, lda, B, ldb, 0.f, tmp, N, ab_dtype, c_dtype, nullptr, NK_F32, 0);
   if (rc == NK_OK) {
     if (ldc == N) {
       rc = nk_relu_bwd(ctx, C, relu_operand, tmp, size_t(M) * size_t(N), c_dtype, beta);

@@ -34,6 +34,7 @@ struct nk_ctx {
   size_t workspace_bytes = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int gemm_engine = NK_GEMM_AUTO;
+  int f32_gemm = NK_F32_GEMM_IEEE;   // nk_gemm_f32_config: how f32 products use the tensor cores
   int conv_engine = NK_CONV_AUTO;
   const char* last_gemm_kernel = "none";
   const char* last_conv_kernel = "none";
@@ -168,5 +169,14 @@ int nk_gemm_simt(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int6
 int nk_gemm_wgmma(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha,
                     const void* A, int64_t lda, const void* B, int64_t ldb, float beta, void* C,
                     int64_t ldc, int c_dtype, const void* bias, int bias_dtype, int relu, const void* mask, float* colsum);
+// 2-D tensor map (bf16 or f32 elements) of a `rows` x `cols` row-major matrix with leading dimension ld: boxes of
+// box_cols (= 128 bytes) x box_rows elements, 128B-swizzled (nk_gemm_tc.cu)
+int make_tmap_2d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t rows, int64_t cols, int64_t ld, uint32_t box_cols,
+                 uint32_t box_rows, int dtype = NK_BF16);
+// f32 products on the tensor cores in the context's TF32 / 3xTF32 mode (nk_gemm_tf32.cu); the caller has checked the
+// arguments, K > 0
+int nk_gemm_tf32(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
+                 int64_t lda, const void* B, int64_t ldb, float beta, void* C, int64_t ldc, int c_dtype, const void* bias,
+                 int bias_dtype, int relu);
 bool nk_gemm_wgmma_supported(int transA, int transB, int64_t M, int64_t N, int64_t K,
                              const void* A, int64_t lda, const void* B, int64_t ldb);

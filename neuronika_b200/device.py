@@ -59,6 +59,19 @@ class Device:
     def gemm_engine(self, engine: str) -> None:
         L.check(L.lib.nk_gemm_config(self.ctx, {"auto": 0, "simt": 1, "wgmma": 2}[engine]), self.ctx)
 
+    F32_MATMUL_MODES = {"ieee": 0, "tf32": 1, "tf32x3": 2}
+
+    def f32_matmul(self, mode: str) -> None:
+        """How f32 matrix products use the tensor cores (off by default, like torch's allow_tf32):
+        "ieee": on the CUDA cores in full f32; "tf32": operands rounded to TF32 (10-bit mantissa, to nearest, ties away
+        from zero), products on the wgmma engine with f32 accumulation; "tf32x3": each operand split into a TF32 high
+        and low part and three TF32 products summed, close to f32 accuracy.  Applies to every f32 GEMM (mm, mm_t,
+        Linear forward and backward, the RNN cells and sequence layers); gemm_engine("simt") still keeps them all on the
+        CUDA cores.  The mode is read when a GEMM is launched: a captured step replays with the mode it was captured with."""
+        if mode not in self.F32_MATMUL_MODES:
+            raise ValueError(f"f32_matmul: mode must be one of {sorted(self.F32_MATMUL_MODES)}, got {mode!r}")
+        L.check(L.lib.nk_gemm_f32_config(self.ctx, self.F32_MATMUL_MODES[mode]), self.ctx)
+
     def conv_engine(self, engine: str) -> None:
         """"auto": tensor-core kernels wherever they apply; "direct": CUDA-core kernels only; "unfused": the same as auto
         (the backward runs dW and dX as two products on every engine)"""
