@@ -478,6 +478,77 @@ int nk_adagrad_step(nk_ctx* ctx, void* w, int w_dtype, void* g, int g_dtype, flo
                     size_t n, int64_t step, float lr, float lr_decay, float eps, float l1, float l2,
                     float grad_scale, int write_back_grad);
 
+/* ---- capturable optimizers and learning-rate schedulers (csrc/nk_optim_multi.cu) ----
+ * The per-parameter entry points above take lr and the step count as kernel arguments, so a captured step replays the
+ * lr and the bias correction (or lr decay) of the step it was captured at.  Here both live in device memory, in a
+ * caller-allocated nk_optim_hyper block that the kernels read (and the prologue and the scheduler write), so a captured
+ * step advances them on every replay.
+ *   nk_optim_hyper_set / _get copy the whole block to / from the device and synchronise; NK_ERR_UNSUPPORTED while
+ *   capturing (a replay would not repeat them).
+ *   nk_optim_prologue (one thread): step += 1, then, for NK_OPTIM_ADAM (Adam and AMSGrad), step_size = lr/(1-b1^t) and
+ *   sqrt_bc2 = sqrt(1-b2^t), b^t by repeated squaring; for NK_OPTIM_ADAGRAD clr = lr/(1+(t-1)*lr_decay).  Every
+ *   operation is rounded on its own in the order nk_adam_step / nk_adagrad_step use on the host, so the scalars are
+ *   bit-identical to theirs.  SGD and RMSProp need no prologue: their kernels read lr.
+ *   nk_multi_*_step: the update of nk_sgd_step / nk_adam_step / nk_rmsprop_step / nk_adagrad_step, with the same
+ *   per-element arithmetic (bit-identical results, written-back gradient included), over `count` <=
+ *   NK_OPTIM_TENSORS_PER_LAUNCH tensors of one (w_dtype, g_dtype) pair in ONE launch.  w, g and n are arrays of `count`
+ *   entries; each state / master argument is an array of `count` device pointers or NULL (= every entry NULL); a NULL
+ *   master entry means that tensor has none.  The tensor table travels in the kernel parameters: no allocation, no
+ *   host-to-device copy, so the call can be captured.  A tensor takes 4-element (16-byte f32) accesses when all its
+ *   pointers allow them, element accesses otherwise.  nk_multi_sgd_step skips the gradient write-back when l2 = 0 and
+ *   grad_scale = 1, as nk_sgd_step does.
+ * Learning-rate schedulers (lr_scheduler/{step_lr,multi_step_lr,exponential_lr,multiplicative_lr,lambda_lr}/mod.rs):
+ * nk_lr_sched_step (one thread) advances epoch to t = epoch + 1 and applies the rule to the optimizer block's lr in f32:
+ *   STEP           lr *= gamma when t % step_size == 0        MULTI_STEP  lr *= gamma when t is one of the milestones
+ *   EXPONENTIAL    lr *= gamma                                MULTIPLICATIVE  lr *= f(t)    LAMBDA  lr = initial_lr * f(t)
+ * last_lr receives lr before the step and current_lr after it.  `table` is a device array of table_len entries: the
+ * milestones (int64) or f(1..table_len) (f32).  A closure-based step with t > table_len changes nothing and sets
+ * past_horizon, which stays set: nk_lr_sched_get then fails with NK_ERR_INVALID_ARG until nk_lr_sched_set clears it.
+ * nk_lr_sched_set / _get copy the block like nk_optim_hyper_set / _get (synchronous, refused while capturing). */
+#define NK_OPTIM_TENSORS_PER_LAUNCH 64
+typedef enum { NK_OPTIM_ADAM = 0, NK_OPTIM_ADAGRAD = 1 } nk_optim_prologue_kind;
+typedef struct nk_optim_hyper {
+  float lr;
+  float step_size;  /* Adam: lr / (1 - beta1^step) */
+  float sqrt_bc2;   /* Adam: sqrt(1 - beta2^step) */
+  float clr;        /* Adagrad: lr / (1 + (step - 1) * lr_decay) */
+  int64_t step;     /* optimizer steps taken */
+} nk_optim_hyper;
+typedef enum { NK_LR_STEP = 0, NK_LR_MULTI_STEP = 1, NK_LR_EXPONENTIAL = 2, NK_LR_MULTIPLICATIVE = 3,
+               NK_LR_LAMBDA = 4 } nk_lr_kind;
+typedef struct nk_lr_sched {
+  int64_t epoch;
+  int64_t step_size;   /* NK_LR_STEP, >= 1 */
+  const void* table;   /* milestones (int64) or factors f(1..table_len) (f32), device memory */
+  int64_t table_len;
+  float gamma;
+  float initial_lr;    /* NK_LR_LAMBDA */
+  float last_lr;
+  float current_lr;
+  int32_t kind;        /* nk_lr_kind */
+  int32_t past_horizon;
+} nk_lr_sched;
+int nk_optim_hyper_set(nk_ctx* ctx, nk_optim_hyper* hyper, const nk_optim_hyper* host);
+int nk_optim_hyper_get(nk_ctx* ctx, const nk_optim_hyper* hyper, nk_optim_hyper* host);
+int nk_optim_prologue(nk_ctx* ctx, nk_optim_hyper* hyper, int kind, float beta1, float beta2, float lr_decay);
+int nk_multi_sgd_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                      void* const* momentum_buf, void* const* master, const int64_t* n, const nk_optim_hyper* hyper,
+                      float l2, float momentum, float dampening, int nesterov, float grad_scale, int write_back_grad);
+int nk_multi_adam_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                       void* const* exp_avg, void* const* exp_avg_sq, void* const* max_exp_avg_sq, void* const* master,
+                       const int64_t* n, const nk_optim_hyper* hyper, float beta1, float beta2, float eps, float l1,
+                       float l2, float grad_scale, int write_back_grad);
+int nk_multi_rmsprop_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                          void* const* square_avg, void* const* grad_avg, void* const* momentum_buf, void* const* master,
+                          const int64_t* n, const nk_optim_hyper* hyper, float alpha, float eps, float momentum,
+                          float l1, float l2, float grad_scale, int write_back_grad);
+int nk_multi_adagrad_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                          void* const* grad_sq, void* const* master, const int64_t* n, const nk_optim_hyper* hyper,
+                          float eps, float l1, float l2, float grad_scale, int write_back_grad);
+int nk_lr_sched_set(nk_ctx* ctx, nk_lr_sched* sched, const nk_lr_sched* host);
+int nk_lr_sched_get(nk_ctx* ctx, const nk_lr_sched* sched, nk_lr_sched* host);
+int nk_lr_sched_step(nk_ctx* ctx, nk_lr_sched* sched, nk_optim_hyper* hyper);
+
 /* ---- NCCL all-reduce behind the ABI (SURVEY.md 8-b, 8-e; csrc/nk_comm.cu) ----
  * The context owns the communicator; libnccl.so.2 is bound at run time (dlopen), so the library loads
  * without it.  Rank 0 creates the 128-byte id and ships it to the others by any means; every rank then

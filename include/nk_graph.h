@@ -226,6 +226,23 @@ int nkg_rmsprop_step(nkg_var* param, float* square_avg, float* grad_avg, float* 
 int nkg_adagrad_step(nkg_var* param, float* grad_sq, float* master, int64_t step, float lr, float lr_decay, float eps,
                      float l1, float l2, float grad_scale);
 
+/* ---- capturable optimizers over many leaves (nk_b200.h nk_multi_*_step): one optimizer step over `count` parameters,
+ * lr and the step count in the device block `hyper`.  State and master arguments are arrays of `count` device pointers
+ * in parameter order (or NULL: none).  Each parameter is checked and its gradient handled as by nkg_*_step; Adam and
+ * Adagrad then launch nk_optim_prologue once; the parameters are grouped by (data, gradient) element types and each
+ * group is updated by one nk_multi_*_step call per NK_OPTIM_TENSORS_PER_LAUNCH tensors, in parameter order.  A
+ * parameter that is not differentiable fails the call before anything is launched. */
+int nkg_multi_sgd_step(nkg_var* const* params, int count, void* const* momentum_buf, void* const* master,
+                       nk_optim_hyper* hyper, float l2, float momentum, float dampening, int nesterov, float grad_scale);
+int nkg_multi_adam_step(nkg_var* const* params, int count, void* const* exp_avg, void* const* exp_avg_sq,
+                        void* const* max_exp_avg_sq, void* const* master, nk_optim_hyper* hyper, float beta1,
+                        float beta2, float eps, float l1, float l2, float grad_scale);
+int nkg_multi_rmsprop_step(nkg_var* const* params, int count, void* const* square_avg, void* const* grad_avg,
+                           void* const* momentum_buf, void* const* master, nk_optim_hyper* hyper, float alpha, float eps,
+                           float momentum, float l1, float l2, float grad_scale);
+int nkg_multi_adagrad_step(nkg_var* const* params, int count, void* const* grad_sq, void* const* master,
+                           nk_optim_hyper* hyper, float lr_decay, float eps, float l1, float l2, float grad_scale);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,9 @@ NK_BIN_ADD, NK_BIN_SUB, NK_BIN_MUL, NK_BIN_DIV = 0, 1, 2, 3
 (NK_UN_NEG, NK_UN_EXP, NK_UN_LN, NK_UN_SQRT, NK_UN_SIGMOID, NK_UN_TANH, NK_UN_SOFTPLUS, NK_UN_LEAKY_RELU,
  NK_UN_POWI) = range(9)
 NK_PAD_CONSTANT, NK_PAD_REFLECTIVE, NK_PAD_REPLICATIVE = 0, 1, 2
+NK_OPTIM_TENSORS_PER_LAUNCH = 64
+NK_OPTIM_ADAM, NK_OPTIM_ADAGRAD = 0, 1
+NK_LR_STEP, NK_LR_MULTI_STEP, NK_LR_EXPONENTIAL, NK_LR_MULTIPLICATIVE, NK_LR_LAMBDA = range(5)
 NK_OK = 0
 NK_ERR = {-1: "NK_ERR_INVALID_ARG", -2: "NK_ERR_CUDA", -3: "NK_ERR_NCCL", -4: "NK_ERR_OOM",
           -5: "NK_ERR_UNSUPPORTED"}
@@ -31,6 +34,19 @@ class NkError(RuntimeError):
         super().__init__(f"{NK_ERR.get(code, code)}: {message}")
         self.code = code
         self.message = message
+
+
+class OptimHyper(C.Structure):
+    """nk_optim_hyper: the device-resident lr and step count of a capturable optimizer"""
+    _fields_ = [("lr", C.c_float), ("step_size", C.c_float), ("sqrt_bc2", C.c_float), ("clr", C.c_float),
+                ("step", C.c_int64)]
+
+
+class LrSched(C.Structure):
+    """nk_lr_sched: the device-resident state of a learning-rate scheduler"""
+    _fields_ = [("epoch", C.c_int64), ("step_size", C.c_int64), ("table", C.c_void_p), ("table_len", C.c_int64),
+                ("gamma", C.c_float), ("initial_lr", C.c_float), ("last_lr", C.c_float), ("current_lr", C.c_float),
+                ("kind", C.c_int32), ("past_horizon", C.c_int32)]
 
 
 if not os.path.exists(LIB_PATH):
@@ -137,6 +153,18 @@ _PROTOS = {
     "nk_adam_step": (i32, [vp, vp, i32, vp, i32, vp, vp, vp, vp, sz, i64, f32, f32, f32, f32, f32, f32, f32, i32]),
     "nk_rmsprop_step": (i32, [vp, vp, i32, vp, i32, vp, vp, vp, vp, sz, f32, f32, f32, f32, f32, f32, f32, i32]),
     "nk_adagrad_step": (i32, [vp, vp, i32, vp, i32, vp, vp, sz, i64, f32, f32, f32, f32, f32, f32, i32]),
+    "nk_optim_hyper_set": (i32, [vp, vp, vp]),
+    "nk_optim_hyper_get": (i32, [vp, vp, vp]),
+    "nk_optim_prologue": (i32, [vp, vp, i32, f32, f32, f32]),
+    "nk_multi_sgd_step": (i32, [vp, i32, pvp, pvp, i32, i32, pvp, pvp, pi64, vp, f32, f32, f32, i32, f32, i32]),
+    "nk_multi_adam_step": (i32, [vp, i32, pvp, pvp, i32, i32, pvp, pvp, pvp, pvp, pi64, vp, f32, f32, f32, f32, f32, f32,
+                                 i32]),
+    "nk_multi_rmsprop_step": (i32, [vp, i32, pvp, pvp, i32, i32, pvp, pvp, pvp, pvp, pi64, vp, f32, f32, f32, f32, f32,
+                                    f32, i32]),
+    "nk_multi_adagrad_step": (i32, [vp, i32, pvp, pvp, i32, i32, pvp, pvp, pi64, vp, f32, f32, f32, f32, i32]),
+    "nk_lr_sched_set": (i32, [vp, vp, vp]),
+    "nk_lr_sched_get": (i32, [vp, vp, vp]),
+    "nk_lr_sched_step": (i32, [vp, vp, vp]),
     "nk_comm_unique_id": (i32, [vp, vp]),
     "nk_comm_init_rank": (i32, [vp, i32, i32, vp]),
     "nk_comm_destroy": (i32, [vp]),

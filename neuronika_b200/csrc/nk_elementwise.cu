@@ -8,6 +8,7 @@
 #include <float.h>
 
 #include "nk_internal.cuh"
+#include "nk_optim_math.cuh"
 
 namespace {
 
@@ -484,16 +485,11 @@ __global__ void __launch_bounds__(kThreads) sgd_kernel(TW* __restrict__ w, TG* _
   const size_t stride = size_t(gridDim.x) * blockDim.x;
   for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
     float wv = master ? master[i] : nk_to_f32<TW>(w[i]);
-    float gv = nk_to_f32<TG>(g[i]) * grad_scale;
-    gv += l2x2 * wv;  // grad += penalty.penalize(w) = 2*lambda*w
+    const float gv = nk_sgd_grad(nk_to_f32<TG>(g[i]), wv, grad_scale, l2x2);
     if (write_back_grad) g[i] = nk_from_f32<TG>(gv);
-    if (!use_momentum) {
-      wv -= gv * lr;
-    } else {
-      float b = buf[i] * mu + gv * one_minus_damp;
-      buf[i] = b;
-      wv -= (nesterov ? (gv + b * mu) : b) * lr;
-    }
+    float b = use_momentum ? buf[i] : 0.f;
+    wv = nk_sgd_update(wv, gv, b, lr, mu, one_minus_damp, use_momentum, nesterov);
+    if (use_momentum) buf[i] = b;
     if (master) master[i] = wv;
     w[i] = nk_from_f32<TW>(wv);
   }
@@ -520,16 +516,9 @@ __global__ void __launch_bounds__(kThreads) sgd_kernel_vec4(TW* __restrict__ w, 
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       float wv = master ? mq.v[e] : nk_to_f32<TW>(wq.v[e]);
-      float gv = nk_to_f32<TG>(gq.v[e]) * grad_scale;
-      gv += l2x2 * wv;
+      const float gv = nk_sgd_grad(nk_to_f32<TG>(gq.v[e]), wv, grad_scale, l2x2);
       gq.v[e] = nk_from_f32<TG>(gv);
-      if (!use_momentum) {
-        wv -= gv * lr;
-      } else {
-        float b = bq.v[e] * mu + gv * one_minus_damp;
-        bq.v[e] = b;
-        wv -= (nesterov ? (gv + b * mu) : b) * lr;
-      }
+      wv = nk_sgd_update(wv, gv, bq.v[e], lr, mu, one_minus_damp, use_momentum, nesterov);
       mq.v[e] = wv;
       wq.v[e] = nk_from_f32<TW>(wv);
     }

@@ -2816,6 +2816,131 @@ int nkg_adagrad_step(nkg_var* p, float* grad_sq, float* master, int64_t step, fl
   });
 }
 
+// ---------------------------------------------------------------- capturable optimizers over many leaves
+// Every parameter gets nkg_*_step's checks and gradient handling in parameter order (the differentiable check first, for
+// all of them, so that an error launches nothing); the tensors are then grouped by (data dtype, gradient dtype) in the
+// order each pair first appears, and each group is updated NK_OPTIM_TENSORS_PER_LAUNCH tensors per call.
+extern "C++" {
+namespace {
+struct MultiGroup {
+  int w_dtype, g_dtype;
+  std::vector<int> idx;
+};
+
+template <typename Launch>
+void multi_step(const char* who, nkg_var* const* params, int count, void* const* const* states, int nstates,
+                void* const* master, Launch launch) {
+  if (count < 0 || (count > 0 && !params)) fail(NK_ERR_INVALID_ARG, "%s: bad parameter array", who);
+  for (int i = 0; i < count; ++i)
+    if (!params[i] || !params[i]->diff())
+      fail(NK_ERR_INVALID_ARG, "%s: parameter %d is not differentiable", who, i);
+  if (count == 0) return;
+  nk_ctx* ctx = params[0]->ctx;
+  for (int i = 1; i < count; ++i)
+    if (params[i]->ctx != ctx) fail(NK_ERR_INVALID_ARG, "%s: parameters on different devices", who);
+  std::vector<void*> w(count), g(count);
+  std::vector<int64_t> n(count);
+  std::vector<Gradient*> roots(count);
+  std::vector<MultiGroup> groups;
+  for (int i = 0; i < count; ++i) {
+    nkg_var* p = params[i];
+    roots[i] = p->grad->root();
+    w[i] = p->data->rptr();
+    g[i] = p->grad->get();
+    n[i] = p->data->n();
+    const int wd = p->data->dtype, gd = roots[i]->dtype;
+    auto it = std::find_if(groups.begin(), groups.end(), [&](const MultiGroup& m) { return m.w_dtype == wd && m.g_dtype == gd; });
+    if (it == groups.end()) it = groups.insert(groups.end(), MultiGroup{wd, gd, {}});
+    it->idx.push_back(i);
+  }
+  std::vector<void*> cw, cg, cm, cs[3];
+  std::vector<int64_t> cn;
+  for (const MultiGroup& m : groups)
+    for (size_t first = 0; first < m.idx.size(); first += NK_OPTIM_TENSORS_PER_LAUNCH) {
+      const size_t last = std::min(m.idx.size(), first + NK_OPTIM_TENSORS_PER_LAUNCH);
+      cw.clear(), cg.clear(), cm.clear(), cn.clear();
+      for (int k = 0; k < nstates; ++k) cs[k].clear();
+      for (size_t j = first; j < last; ++j) {
+        const int i = m.idx[j];
+        cw.push_back(w[i]);
+        cg.push_back(g[i]);
+        cn.push_back(n[i]);
+        cm.push_back(master ? master[i] : nullptr);
+        for (int k = 0; k < nstates; ++k) cs[k].push_back(states[k] ? states[k][i] : nullptr);
+      }
+      void* const* st[3];
+      for (int k = 0; k < nstates; ++k) st[k] = states[k] ? cs[k].data() : nullptr;
+      ck(ctx, launch(ctx, int(cw.size()), cw.data(), cg.data(), m.w_dtype, m.g_dtype, st, master ? cm.data() : nullptr,
+                     cn.data()));
+    }
+  for (Gradient* r : roots) r->is_zero = false;
+}
+}  // namespace
+}  // extern "C++"
+
+int nkg_multi_sgd_step(nkg_var* const* params, int count, void* const* momentum_buf, void* const* master,
+                       nk_optim_hyper* hyper, float l2, float momentum, float dampening, int nesterov, float grad_scale) {
+  return guard([&] {
+    void* const* states[1] = {momentum_buf};
+    multi_step("multi_sgd", params, count, states, 1, master,
+               [&](nk_ctx* ctx, int c, void* const* w, void* const* g, int wd, int gd, void* const* const* st,
+                   void* const* m, const int64_t* n) {
+                 return nk_multi_sgd_step(ctx, c, w, g, wd, gd, st[0], m, n, hyper, l2, momentum, dampening, nesterov,
+                                          grad_scale, 1);
+               });
+  });
+}
+
+int nkg_multi_adam_step(nkg_var* const* params, int count, void* const* exp_avg, void* const* exp_avg_sq,
+                        void* const* max_exp_avg_sq, void* const* master, nk_optim_hyper* hyper, float beta1,
+                        float beta2, float eps, float l1, float l2, float grad_scale) {
+  return guard([&] {
+    bool first = true;
+    void* const* states[3] = {exp_avg, exp_avg_sq, max_exp_avg_sq};
+    multi_step("multi_adam", params, count, states, 3, master,
+               [&](nk_ctx* ctx, int c, void* const* w, void* const* g, int wd, int gd, void* const* const* st,
+                   void* const* m, const int64_t* n) {
+                 if (first) {   // once per optimizer step, after every check, before the first update
+                   first = false;
+                   if (int rc = nk_optim_prologue(ctx, hyper, NK_OPTIM_ADAM, beta1, beta2, 0.f)) return rc;
+                 }
+                 return nk_multi_adam_step(ctx, c, w, g, wd, gd, st[0], st[1], st[2], m, n, hyper, beta1, beta2, eps,
+                                           l1, l2, grad_scale, 1);
+               });
+  });
+}
+
+int nkg_multi_rmsprop_step(nkg_var* const* params, int count, void* const* square_avg, void* const* grad_avg,
+                           void* const* momentum_buf, void* const* master, nk_optim_hyper* hyper, float alpha, float eps,
+                           float momentum, float l1, float l2, float grad_scale) {
+  return guard([&] {
+    void* const* states[3] = {square_avg, grad_avg, momentum_buf};
+    multi_step("multi_rmsprop", params, count, states, 3, master,
+               [&](nk_ctx* ctx, int c, void* const* w, void* const* g, int wd, int gd, void* const* const* st,
+                   void* const* m, const int64_t* n) {
+                 return nk_multi_rmsprop_step(ctx, c, w, g, wd, gd, st[0], st[1], st[2], m, n, hyper, alpha, eps,
+                                              momentum, l1, l2, grad_scale, 1);
+               });
+  });
+}
+
+int nkg_multi_adagrad_step(nkg_var* const* params, int count, void* const* grad_sq, void* const* master,
+                           nk_optim_hyper* hyper, float lr_decay, float eps, float l1, float l2, float grad_scale) {
+  return guard([&] {
+    bool first = true;
+    void* const* states[1] = {grad_sq};
+    multi_step("multi_adagrad", params, count, states, 1, master,
+               [&](nk_ctx* ctx, int c, void* const* w, void* const* g, int wd, int gd, void* const* const* st,
+                   void* const* m, const int64_t* n) {
+                 if (first) {
+                   first = false;
+                   if (int rc = nk_optim_prologue(ctx, hyper, NK_OPTIM_ADAGRAD, 0.f, 0.f, lr_decay)) return rc;
+                 }
+                 return nk_multi_adagrad_step(ctx, c, w, g, wd, gd, st[0], m, n, hyper, eps, l1, l2, grad_scale, 1);
+               });
+  });
+}
+
 int nkg_set_grad_rs(nkg_var* leaf, int world, int rank, void* const* slots, nkg_grad_rs_hook cb, void* user) {
   return guard([&] {
     if (!leaf || !leaf->diff()) fail(NK_ERR_INVALID_ARG, "nkg_set_grad_rs: not a differentiable variable");

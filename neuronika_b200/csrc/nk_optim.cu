@@ -7,6 +7,7 @@
 #include <float.h>
 
 #include "nk_internal.cuh"
+#include "nk_optim_math.cuh"
 
 namespace {
 
@@ -19,21 +20,12 @@ inline int opt_blocks(nk_ctx* ctx, size_t n) {
   return int(b < 1 ? 1 : b);
 }
 
-struct Common {
-  float l1, l2x2, grad_scale;
-  int write_back_grad;
-};
-
-__device__ __forceinline__ float signum_f32(float w) {  // f32::signum: 1.0 for +0.0, -1.0 for -0.0, NaN for NaN
-  return w != w ? w : copysignf(1.f, w);
-}
+using Common = NkOptPenalty;
 
 template <typename TW, typename TG>
 __device__ __forceinline__ float penalised_grad(const Common& c, TW* w, TG* g, const float* master, size_t i, float* wv) {
   *wv = master ? master[i] : nk_to_f32<TW>(w[i]);
-  float gv = nk_to_f32<TG>(g[i]) * c.grad_scale;
-  if (c.l1 != 0.f) gv += c.l1 * signum_f32(*wv);
-  gv += c.l2x2 * (*wv);
+  const float gv = nk_opt_grad(c, nk_to_f32<TG>(g[i]), *wv);
   if (c.write_back_grad) g[i] = nk_from_f32<TG>(gv);  // the reference adds the penalty INTO the gradient (adam/mod.rs:146-148)
   return gv;
 }
@@ -54,16 +46,11 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(TW* __restrict__ w, TG* 
   for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
     float wv;
     const float gv = penalised_grad<TW, TG>(c, w, g, master, i, &wv);
-    const float m = exp_avg[i] * beta1 + gv * (1.f - beta1);
-    const float v = exp_avg_sq[i] * beta2 + gv * gv * (1.f - beta2);
+    float m = exp_avg[i], v = exp_avg_sq[i], mx = max_sq ? max_sq[i] : 0.f;
+    wv = nk_adam_update(wv, gv, m, v, max_sq != nullptr, mx, beta1, beta2, sqrt_bc2, step_size, eps);
     exp_avg[i] = m;
     exp_avg_sq[i] = v;
-    float vv = v;
-    if (max_sq) {  // AMSGrad: running maximum of the second moment
-      vv = fmaxf(max_sq[i], v);
-      max_sq[i] = vv;
-    }
-    wv -= m / ((sqrtf(vv) / sqrt_bc2) + eps) * step_size;
+    if (max_sq) max_sq[i] = mx;
     store_w<TW>(w, master, i, wv);
   }
 }
@@ -78,23 +65,11 @@ __global__ void __launch_bounds__(kThreads) rmsprop_kernel(TW* __restrict__ w, T
   for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
     float wv;
     const float gv = penalised_grad<TW, TG>(c, w, g, master, i, &wv);
-    const float sq = square_avg[i] * alpha + gv * gv * (1.f - alpha);
+    float sq = square_avg[i], ga = grad_avg ? grad_avg[i] : 0.f, b = buf ? buf[i] : 0.f;
+    wv = nk_rmsprop_update(wv, gv, sq, grad_avg != nullptr, ga, buf != nullptr, b, lr, alpha, eps, momentum);
     square_avg[i] = sq;
-    float denom;
-    if (grad_avg) {  // centered
-      const float ga = grad_avg[i] * alpha + gv * (1.f - alpha);
-      grad_avg[i] = ga;
-      denom = sqrtf(sq + (-ga * ga)) + eps;
-    } else {
-      denom = sqrtf(sq) + eps;
-    }
-    if (buf) {
-      const float b = buf[i] * momentum + gv / denom;
-      buf[i] = b;
-      wv -= b * lr;
-    } else {
-      wv -= gv / denom * lr;
-    }
+    if (grad_avg) grad_avg[i] = ga;
+    if (buf) buf[i] = b;
     store_w<TW>(w, master, i, wv);
   }
 }
@@ -108,9 +83,9 @@ __global__ void __launch_bounds__(kThreads) adagrad_kernel(TW* __restrict__ w, T
   for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
     float wv;
     const float gv = penalised_grad<TW, TG>(c, w, g, master, i, &wv);
-    const float s = grad_sq[i] + gv * gv;
+    float s = grad_sq[i];
+    wv = nk_adagrad_update(wv, gv, s, clr, eps);
     grad_sq[i] = s;
-    wv -= gv / (sqrtf(s) + eps) * clr;
     store_w<TW>(w, master, i, wv);
   }
 }

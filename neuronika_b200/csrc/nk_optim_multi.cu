@@ -1,0 +1,392 @@
+// Capturable optimizers: the update of every parameter tensor of one (w dtype, g dtype) pair in one launch per
+// NK_OPTIM_TENSORS_PER_LAUNCH tensors, with lr and the step count in device memory (nk_optim_hyper), plus the
+// learning-rate scheduler step as a one-thread kernel on the same block.
+//
+// The tensor table travels in the kernel parameters (__grid_constant__), as nk_cat.cu's operand table does: the grid
+// is the concatenation of every tensor's CTAs, the host computes the CTA prefix and each CTA finds its tensor with a
+// binary search.  A CTA covers kChunk consecutive elements of its tensor.  Each thread takes 4 consecutive elements
+// (16-byte f32 / 8-byte bf16 accesses) when all of the tensor's pointers are aligned for it, and walks the chunk with
+// element accesses otherwise.  The per-element arithmetic is nk_optim_math.cuh's, the same code the per-parameter
+// kernels inline, so both paths give the same bits.
+// HBM bound: algorithmic bytes per element as nk_optim.cu (24..28 B in f32 for two states).
+#include <float.h>
+#include <limits.h>
+
+#include "nk_internal.cuh"
+#include "nk_optim_math.cuh"
+
+// a named namespace: kernel symbol names stay the same from build to build (torch.profiler traces)
+namespace nk_optim_multi {
+
+constexpr int kThreads = 256;
+constexpr int kTensors = NK_OPTIM_TENSORS_PER_LAUNCH;
+constexpr int kChunk = kThreads * 4;  // elements per CTA
+
+enum Kind { SGD = 0, ADAM = 1, RMSPROP = 2, ADAGRAD = 3 };
+
+struct Tensor {
+  void* w;
+  void* g;
+  float* s[3];     // optimizer state, by kind: SGD {buf}, Adam {exp_avg, exp_avg_sq, max_sq}, RMSProp {square_avg,
+                   // grad_avg, buf}, Adagrad {grad_sq}
+  float* master;
+  int64_t n;
+};
+struct Table {
+  Tensor t[kTensors];
+  int32_t blk[kTensors + 1];  // CTA prefix
+  uint64_t vec;               // bit i: tensor i takes the 4-element path
+  int count;
+};
+// every hyperparameter that is not in the device block; uniform over the launch
+struct Args {
+  float beta1, beta2, eps;                       // Adam (eps: also RMSProp, Adagrad)
+  float alpha, momentum;                         // RMSProp (momentum: also SGD)
+  float one_minus_damp, sgd_l2x2;                // SGD
+  NkOptPenalty pen;                              // Adam family; pen.grad_scale and write_back_grad serve SGD too
+  int has[3];                                    // which of the state slots are in use
+  int nesterov;
+};
+static_assert(sizeof(Table) + sizeof(Args) + sizeof(void*) <= 4096, "tensor table exceeds the kernel parameter limit");
+
+static inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
+
+__device__ __forceinline__ int find_tensor(const int32_t* blk, int count, int b) {
+  int lo = 0, hi = count - 1;  // the largest i with blk[i] <= b (empty tensors own no CTA)
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (blk[mid] <= b) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// the scalars a launch reads from the device block
+struct Derived {
+  float lr, step_size, sqrt_bc2, clr;
+};
+
+// one element: wv (f32 weight or master) and the raw gradient in, the new weight out; st[] is the element's state
+template <int K>
+__device__ __forceinline__ float update(const Args& a, const Derived& d, float wv, float& graw, float (&st)[3]) {
+  if (K == SGD) {
+    const float gv = nk_sgd_grad(graw, wv, a.pen.grad_scale, a.sgd_l2x2);
+    graw = gv;
+    return nk_sgd_update(wv, gv, st[0], d.lr, a.momentum, a.one_minus_damp, a.has[0], a.nesterov);
+  }
+  const float gv = nk_opt_grad(a.pen, graw, wv);
+  graw = gv;
+  if (K == ADAM)
+    return nk_adam_update(wv, gv, st[0], st[1], a.has[2], st[2], a.beta1, a.beta2, d.sqrt_bc2, d.step_size, a.eps);
+  if (K == RMSPROP)
+    return nk_rmsprop_update(wv, gv, st[0], a.has[1], st[1], a.has[2], st[2], d.lr, a.alpha, a.eps, a.momentum);
+  return nk_adagrad_update(wv, gv, st[0], d.clr, a.eps);
+}
+
+template <typename T>
+struct alignas(sizeof(T) * 4) Quad {
+  T v[4];
+};
+
+template <int K, typename TW, typename TG>
+__global__ void __launch_bounds__(kThreads) nk_optim_multi_kernel(const __grid_constant__ Table tab,
+                                                                  const __grid_constant__ Args a,
+                                                                  const nk_optim_hyper* __restrict__ hyper) {
+  const int b = blockIdx.x;
+  const int i = find_tensor(tab.blk, tab.count, b);
+  const Tensor& t = tab.t[i];
+  const Derived d{hyper->lr, hyper->step_size, hyper->sqrt_bc2, hyper->clr};
+  TW* __restrict__ w = static_cast<TW*>(t.w);
+  TG* __restrict__ g = static_cast<TG*>(t.g);
+  float* __restrict__ master = t.master;
+  const int wb = a.pen.write_back_grad;
+  const int64_t base = int64_t(b - tab.blk[i]) * kChunk;
+  if ((tab.vec >> i) & 1) {
+    const int64_t e0 = base + int64_t(threadIdx.x) * 4;
+    if (e0 + 4 <= t.n) {
+      const int64_t q = e0 / 4;
+      Quad<TW> wq = reinterpret_cast<const Quad<TW>*>(w)[q];
+      Quad<TG> gq = reinterpret_cast<const Quad<TG>*>(g)[q];
+      Quad<float> mq, sq[3];
+      if (master) mq = reinterpret_cast<const Quad<float>*>(master)[q];
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (a.has[k]) sq[k] = reinterpret_cast<const Quad<float>*>(t.s[k])[q];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        float st[3] = {sq[0].v[e], sq[1].v[e], sq[2].v[e]};
+        float gv = nk_to_f32<TG>(gq.v[e]);
+        const float wv = update<K>(a, d, master ? mq.v[e] : nk_to_f32<TW>(wq.v[e]), gv, st);
+        gq.v[e] = nk_from_f32<TG>(gv);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) sq[k].v[e] = st[k];
+        mq.v[e] = wv;
+        wq.v[e] = nk_from_f32<TW>(wv);
+      }
+      if (wb) reinterpret_cast<Quad<TG>*>(g)[q] = gq;
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (a.has[k]) reinterpret_cast<Quad<float>*>(t.s[k])[q] = sq[k];
+      if (master) reinterpret_cast<Quad<float>*>(master)[q] = mq;
+      reinterpret_cast<Quad<TW>*>(w)[q] = wq;
+      return;
+    }
+    // the last (n % 4) elements of the tensor: element accesses by the thread that owns them
+    for (int64_t e = e0; e < t.n; ++e) {
+      float st[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) st[k] = a.has[k] ? t.s[k][e] : 0.f;
+      float gv = nk_to_f32<TG>(g[e]);
+      const float wv = update<K>(a, d, master ? master[e] : nk_to_f32<TW>(w[e]), gv, st);
+      if (wb) g[e] = nk_from_f32<TG>(gv);
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (a.has[k]) t.s[k][e] = st[k];
+      if (master) master[e] = wv;
+      w[e] = nk_from_f32<TW>(wv);
+    }
+    return;
+  }
+#pragma unroll 4
+  for (int j = 0; j < kChunk / kThreads; ++j) {
+    const int64_t e = base + int64_t(j) * kThreads + threadIdx.x;
+    if (e >= t.n) break;
+    float st[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) st[k] = a.has[k] ? t.s[k][e] : 0.f;
+    float gv = nk_to_f32<TG>(g[e]);
+    const float wv = update<K>(a, d, master ? master[e] : nk_to_f32<TW>(w[e]), gv, st);
+    if (wb) g[e] = nk_from_f32<TG>(gv);
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      if (a.has[k]) t.s[k][e] = st[k];
+    if (master) master[e] = wv;
+    w[e] = nk_from_f32<TW>(wv);
+  }
+}
+
+// step += 1 and the per-step scalars, each operation rounded on its own in the host's order (nk_optim.cu)
+__global__ void nk_optim_prologue_kernel(nk_optim_hyper* h, int kind, float beta1, float beta2, float lr_decay) {
+  const int64_t step = h->step + 1;
+  h->step = step;
+  if (kind == NK_OPTIM_ADAM) {
+    float p1 = 1.f, p2 = 1.f, b1 = beta1, b2 = beta2;
+    for (uint64_t e = uint64_t(step); e; e >>= 1) {
+      if (e & 1) p1 = __fmul_rn(p1, b1), p2 = __fmul_rn(p2, b2);
+      b1 = __fmul_rn(b1, b1), b2 = __fmul_rn(b2, b2);
+    }
+    const float bc1 = __fsub_rn(1.f, p1), bc2 = __fsub_rn(1.f, p2);
+    h->sqrt_bc2 = __fsqrt_rn(bc2);
+    h->step_size = __fdiv_rn(h->lr, bc1);
+  } else {
+    h->clr = __fdiv_rn(h->lr, __fadd_rn(1.f, __fmul_rn(__ll2float_rn(step - 1), lr_decay)));
+  }
+}
+
+__global__ void nk_lr_sched_kernel(nk_lr_sched* s, nk_optim_hyper* h) {
+  const int64_t t = s->epoch + 1;
+  const float lr = h->lr;
+  float next = lr;
+  switch (s->kind) {
+    case NK_LR_STEP:
+      if (t % s->step_size == 0) next = __fmul_rn(lr, s->gamma);
+      break;
+    case NK_LR_MULTI_STEP: {
+      const int64_t* m = static_cast<const int64_t*>(s->table);
+      for (int64_t k = 0; k < s->table_len; ++k)
+        if (m[k] == t) {
+          next = __fmul_rn(lr, s->gamma);
+          break;
+        }
+      break;
+    }
+    case NK_LR_EXPONENTIAL:
+      next = __fmul_rn(lr, s->gamma);
+      break;
+    default: {  // the closure-based schedulers: f(t) from the table
+      if (t > s->table_len) {
+        s->past_horizon = 1;
+        return;
+      }
+      const float f = static_cast<const float*>(s->table)[t - 1];
+      next = __fmul_rn(s->kind == NK_LR_LAMBDA ? s->initial_lr : lr, f);
+    }
+  }
+  s->epoch = t;
+  s->last_lr = lr;
+  s->current_lr = next;
+  h->lr = next;
+}
+
+// ------------------------------------------------------------------------------------------------- host side
+static int copy_block(nk_ctx* ctx, const char* who, void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  if (ctx->capturing)
+    return nk_set_error(ctx, NK_ERR_UNSUPPORTED, "%s: a host copy of the block cannot be captured (a replay would not "
+                        "repeat it)", who);
+  NK_REQUIRE(ctx, dst && src, "%s: NULL pointer", who);
+  NK_CUDA(ctx, cudaMemcpyAsync(dst, src, bytes, kind, ctx->stream));
+  NK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return NK_OK;
+}
+
+static inline void* entry(void* const* a, int i) { return a ? a[i] : nullptr; }
+
+// builds the table of one launch (checks everything first: an error launches nothing) and launches it
+template <int K>
+static int multi_step(nk_ctx* ctx, const char* who, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                      void* const* st[3], void* const* master, const int64_t* n, const nk_optim_hyper* hyper,
+                      const Args& args) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, nk_dtype_ok(w_dtype) && nk_dtype_ok(g_dtype), "%s: bad dtype", who);
+  NK_REQUIRE(ctx, count >= 0 && count <= kTensors, "%s: %d tensors (1..%d per launch)", who, count, kTensors);
+  if (count == 0) return NK_OK;
+  NK_REQUIRE(ctx, w && g && n && hyper, "%s: NULL pointer", who);
+  Table tab = {};
+  tab.count = count;
+  int64_t blocks = 0;
+  const size_t ws = nk_dtype_size(w_dtype), gs = nk_dtype_size(g_dtype);
+  for (int i = 0; i < count; ++i) {
+    Tensor& t = tab.t[i];
+    NK_REQUIRE(ctx, n[i] >= 0, "%s: tensor %d has %lld elements", who, i, (long long)n[i]);
+    t.w = w[i];
+    t.g = g[i];
+    t.n = n[i];
+    t.master = static_cast<float*>(entry(master, i));
+    bool vec = aligned(t.w, 4 * ws) && aligned(t.g, 4 * gs) && aligned(t.master, 16);
+    for (int k = 0; k < 3; ++k) {
+      t.s[k] = args.has[k] ? static_cast<float*>(entry(st[k], i)) : nullptr;
+      vec = vec && aligned(t.s[k], 16);
+    }
+    tab.blk[i] = int32_t(blocks);
+    if (t.n == 0) continue;
+    NK_REQUIRE(ctx, t.w && t.g, "%s: tensor %d: NULL weight or gradient", who, i);
+    for (int k = 0; k < 3; ++k)
+      NK_REQUIRE(ctx, !args.has[k] || t.s[k], "%s: tensor %d: NULL state %d", who, i, k);
+    if (vec) tab.vec |= uint64_t(1) << i;
+    blocks += (t.n + kChunk - 1) / kChunk;
+    NK_REQUIRE(ctx, blocks <= INT_MAX, "%s: %lld CTAs exceed the grid limit", who, (long long)blocks);
+  }
+  tab.blk[count] = int32_t(blocks);
+  if (blocks == 0) return NK_OK;
+  const int grid = int(blocks);
+  if (w_dtype == NK_F32 && g_dtype == NK_F32)
+    nk_optim_multi_kernel<K, float, float><<<grid, kThreads, 0, ctx->stream>>>(tab, args, hyper);
+  else if (w_dtype == NK_BF16 && g_dtype == NK_BF16)
+    nk_optim_multi_kernel<K, __nv_bfloat16, __nv_bfloat16><<<grid, kThreads, 0, ctx->stream>>>(tab, args, hyper);
+  else if (w_dtype == NK_BF16)
+    nk_optim_multi_kernel<K, __nv_bfloat16, float><<<grid, kThreads, 0, ctx->stream>>>(tab, args, hyper);
+  else
+    nk_optim_multi_kernel<K, float, __nv_bfloat16><<<grid, kThreads, 0, ctx->stream>>>(tab, args, hyper);
+  NK_LAUNCHED(ctx, who);
+  return NK_OK;
+}
+
+}  // namespace nk_optim_multi
+
+using namespace nk_optim_multi;
+
+extern "C" {
+
+int nk_optim_hyper_set(nk_ctx* ctx, nk_optim_hyper* hyper, const nk_optim_hyper* host) {
+  return copy_block(ctx, "nk_optim_hyper_set", hyper, host, sizeof(nk_optim_hyper), cudaMemcpyHostToDevice);
+}
+
+int nk_optim_hyper_get(nk_ctx* ctx, const nk_optim_hyper* hyper, nk_optim_hyper* host) {
+  return copy_block(ctx, "nk_optim_hyper_get", host, hyper, sizeof(nk_optim_hyper), cudaMemcpyDeviceToHost);
+}
+
+int nk_optim_prologue(nk_ctx* ctx, nk_optim_hyper* hyper, int kind, float beta1, float beta2, float lr_decay) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, hyper, "nk_optim_prologue: NULL block");
+  NK_REQUIRE(ctx, kind == NK_OPTIM_ADAM || kind == NK_OPTIM_ADAGRAD, "nk_optim_prologue: bad kind %d", kind);
+  nk_optim_prologue_kernel<<<1, 1, 0, ctx->stream>>>(hyper, kind, beta1, beta2, lr_decay);
+  NK_LAUNCHED(ctx, "optim_prologue");
+  return NK_OK;
+}
+
+int nk_multi_sgd_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                      void* const* momentum_buf, void* const* master, const int64_t* n, const nk_optim_hyper* hyper,
+                      float l2, float momentum, float dampening, int nesterov, float grad_scale, int write_back_grad) {
+  Args a = {};
+  a.momentum = momentum;
+  a.one_minus_damp = 1.f - dampening;
+  a.sgd_l2x2 = 2.f * l2;
+  a.nesterov = nesterov;
+  a.has[0] = momentum > FLT_EPSILON;  // `.filter(|val| *val > f32::EPSILON)`, sgd/mod.rs:202
+  a.pen.grad_scale = grad_scale;
+  a.pen.write_back_grad = (a.sgd_l2x2 == 0.f && grad_scale == 1.f) ? 0 : write_back_grad;  // as nk_sgd_step
+  void* const* st[3] = {momentum_buf, nullptr, nullptr};
+  return multi_step<SGD>(ctx, "nk_multi_sgd_step", count, w, g, w_dtype, g_dtype, st, master, n, hyper, a);
+}
+
+int nk_multi_adam_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                       void* const* exp_avg, void* const* exp_avg_sq, void* const* max_exp_avg_sq, void* const* master,
+                       const int64_t* n, const nk_optim_hyper* hyper, float beta1, float beta2, float eps, float l1,
+                       float l2, float grad_scale, int write_back_grad) {
+  Args a = {};
+  a.beta1 = beta1;
+  a.beta2 = beta2;
+  a.eps = eps;
+  a.pen = NkOptPenalty{l1, 2.f * l2, grad_scale, write_back_grad};
+  a.has[0] = a.has[1] = 1;
+  a.has[2] = max_exp_avg_sq != nullptr;
+  void* const* st[3] = {exp_avg, exp_avg_sq, max_exp_avg_sq};
+  return multi_step<ADAM>(ctx, "nk_multi_adam_step", count, w, g, w_dtype, g_dtype, st, master, n, hyper, a);
+}
+
+int nk_multi_rmsprop_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                          void* const* square_avg, void* const* grad_avg, void* const* momentum_buf, void* const* master,
+                          const int64_t* n, const nk_optim_hyper* hyper, float alpha, float eps, float momentum,
+                          float l1, float l2, float grad_scale, int write_back_grad) {
+  Args a = {};
+  a.alpha = alpha;
+  a.eps = eps;
+  a.momentum = momentum;
+  a.pen = NkOptPenalty{l1, 2.f * l2, grad_scale, write_back_grad};
+  a.has[0] = 1;
+  a.has[1] = grad_avg != nullptr;
+  a.has[2] = momentum_buf != nullptr && momentum > FLT_EPSILON;  // rmsprop/mod.rs:213-216, as nk_rmsprop_step
+  void* const* st[3] = {square_avg, grad_avg, momentum_buf};
+  return multi_step<RMSPROP>(ctx, "nk_multi_rmsprop_step", count, w, g, w_dtype, g_dtype, st, master, n, hyper, a);
+}
+
+int nk_multi_adagrad_step(nk_ctx* ctx, int count, void* const* w, void* const* g, int w_dtype, int g_dtype,
+                          void* const* grad_sq, void* const* master, const int64_t* n, const nk_optim_hyper* hyper,
+                          float eps, float l1, float l2, float grad_scale, int write_back_grad) {
+  Args a = {};
+  a.eps = eps;
+  a.pen = NkOptPenalty{l1, 2.f * l2, grad_scale, write_back_grad};
+  a.has[0] = 1;
+  void* const* st[3] = {grad_sq, nullptr, nullptr};
+  return multi_step<ADAGRAD>(ctx, "nk_multi_adagrad_step", count, w, g, w_dtype, g_dtype, st, master, n, hyper, a);
+}
+
+int nk_lr_sched_set(nk_ctx* ctx, nk_lr_sched* sched, const nk_lr_sched* host) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, host, "nk_lr_sched_set: NULL pointer");
+  NK_REQUIRE(ctx, host->kind >= NK_LR_STEP && host->kind <= NK_LR_LAMBDA, "nk_lr_sched_set: bad kind %d", host->kind);
+  NK_REQUIRE(ctx, host->epoch >= 0, "nk_lr_sched_set: negative epoch %lld", (long long)host->epoch);
+  NK_REQUIRE(ctx, host->kind != NK_LR_STEP || host->step_size >= 1, "nk_lr_sched_set: step_size must be >= 1 (got %lld)",
+             (long long)host->step_size);
+  NK_REQUIRE(ctx, host->table_len >= 0 && (host->table_len == 0 || host->table),
+             "nk_lr_sched_set: table of %lld entries at NULL", (long long)host->table_len);
+  return copy_block(ctx, "nk_lr_sched_set", sched, host, sizeof(nk_lr_sched), cudaMemcpyHostToDevice);
+}
+
+int nk_lr_sched_get(nk_ctx* ctx, const nk_lr_sched* sched, nk_lr_sched* host) {
+  if (int rc = copy_block(ctx, "nk_lr_sched_get", host, sched, sizeof(nk_lr_sched), cudaMemcpyDeviceToHost)) return rc;
+  if (host->past_horizon)
+    return nk_set_error(ctx, NK_ERR_INVALID_ARG, "lr scheduler stepped past the end of its table of %lld factors "
+                        "(epoch %lld): lr was left unchanged", (long long)host->table_len, (long long)host->epoch);
+  return NK_OK;
+}
+
+int nk_lr_sched_step(nk_ctx* ctx, nk_lr_sched* sched, nk_optim_hyper* hyper) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, sched && hyper, "nk_lr_sched_step: NULL pointer");
+  nk_lr_sched_kernel<<<1, 1, 0, ctx->stream>>>(sched, hyper);
+  NK_LAUNCHED(ctx, "lr_sched");
+  return NK_OK;
+}
+
+}  // extern "C"

@@ -1,11 +1,18 @@
 """Optimizer registry and optimizers: the mirror of neuronika-optim (optimizer.rs:4-104, sgd/mod.rs:11-236,
 adam/mod.rs, amsgrad/mod.rs, rmsprop/mod.rs, adagrad/mod.rs, penalty.rs:2-79).  Every `optimize()` is ONE fused kernel
 over the parameter (nk_sgd_step / nk_adam_step / nk_rmsprop_step / nk_adagrad_step); optimizer state lives on the
-device in f32."""
+device in f32.
+
+`capturable=True` on any optimizer's `.new(...)` keeps lr and the step count in device memory instead (nk_optim_hyper)
+and updates every registered parameter with one multi-tensor launch per 64 tensors of one (data, gradient) dtype pair
+(nkg_multi_*_step), so a captured step advances the step count, and sees lr changes, on every replay."""
 from __future__ import annotations
+
+import ctypes as C
 
 import numpy as np
 
+from . import _lib as L
 from . import variable as V
 from .device import F32, CuArray
 
@@ -70,6 +77,84 @@ class Optimizer:
             p.zero_grad()
 
 
+class CapturableOptimizer(Optimizer):
+    """An optimizer built with `capturable=True`.  lr and the step count live in a device block that the first
+    register() allocates; step() launches (Adam, AMSGrad, Adagrad) the one-thread prologue that advances the step count,
+    then one update launch per 64 tensors per (data, gradient) dtype pair.  Every other hyperparameter is a kernel
+    argument: a captured step keeps the values it was captured with.  get_lr / set_lr read and write the device block
+    (synchronously; NkError while capturing).  All parameters must be registered before the first step, since the step
+    count is shared."""
+
+    def __init__(self, status):
+        super().__init__(status)
+        self._hyper = None
+        self._stepped = False
+
+    @property
+    def hyper_ptr(self):
+        """device address of the nk_optim_hyper block (None before the first register)"""
+        return self._hyper.ptr if self._hyper is not None else None
+
+    def _read(self) -> L.OptimHyper:
+        h = L.OptimHyper()
+        dev = self._hyper.device
+        L.check(L.lib.nk_optim_hyper_get(dev.ctx, self._hyper.ptr, C.byref(h)), dev.ctx)
+        return h
+
+    def _write(self, h: L.OptimHyper) -> None:
+        dev = self._hyper.device
+        L.check(L.lib.nk_optim_hyper_set(dev.ctx, self._hyper.ptr, C.byref(h)), dev.ctx)
+
+    def get_lr(self) -> float:
+        return self.status.lr if self._hyper is None else float(self._read().lr)
+
+    def set_lr(self, lr: float) -> None:
+        if self._hyper is None:
+            self.status.lr = float(lr)
+            return
+        h = self._read()
+        h.lr = float(lr)
+        self._write(h)
+
+    def register(self, variable: V.VarDiff) -> None:
+        if self._hyper is None:
+            block = CuArray(variable.device, (C.sizeof(L.OptimHyper) // 4,), F32)
+            self._hyper = block
+            try:
+                self._write(L.OptimHyper(lr=self.status.lr))
+            except L.NkError:
+                self._hyper = None
+                raise
+        else:
+            if variable.device is not self._hyper.device:
+                raise L.NkError(-1, "register: a capturable optimizer's parameters share one device")
+            self._read()                                  # refused while capturing, like every host access
+            if self._stepped:
+                raise L.NkError(-1, "register: a capturable optimizer counts steps for all its parameters together; "
+                                "register every parameter before the first step()")
+        self.params.append(self.status.into_param(variable))
+
+    def step(self) -> None:
+        if self.params:
+            self.status.multi_step(self.params, self._hyper.ptr)
+            self._stepped = True
+
+
+def _optimizer(status) -> Optimizer:
+    return CapturableOptimizer(status) if status.capturable else Optimizer(status)
+
+
+def _ptrs(arrays):
+    """ctypes array of device pointers (NULL for None), or None when every entry is None"""
+    if all(a is None for a in arrays):
+        return None
+    return (C.c_void_p * len(arrays))(*[a.ptr.value if a is not None else None for a in arrays])
+
+
+def _handles(params):
+    return (C.c_void_p * len(params))(*[p.variable._h.value for p in params])
+
+
 class _SGDParam:
     """SGDParam (sgd/mod.rs:150-236): momentum buffer created on first use."""
 
@@ -78,13 +163,17 @@ class _SGDParam:
         if status.master_weights and variable.dtype != F32:
             self.master = variable.data_array().astype(F32)
 
-    def optimize(self) -> None:
+    def prepare(self) -> None:
         s = self.status
         use_mom = s.momentum is not None and s.momentum > np.finfo(np.float32).eps
         if use_mom and self.buffer is None:
             self.buffer = CuArray(self.variable.device, self.variable.shape, F32)
         if not use_mom:
             self.buffer = None
+
+    def optimize(self) -> None:
+        s = self.status
+        self.prepare()
         V._ck(V.lib.nkg_sgd_step(self.variable._h, self.buffer.ptr if self.buffer is not None else None,
                                  self.master.ptr if self.master is not None else None, float(s.lr),
                                  float(s.penalty.lambda_), float(s.momentum or 0.0), float(s.dampening or 0.0),
@@ -99,7 +188,8 @@ class StochasticGD:
     same argument validation.  `grad_scale` (1/world_size under data parallel) and `master_weights`
     (f32 master copy of bf16 parameters, kept as optimizer state) are additions."""
 
-    def __init__(self, lr, penalty, momentum, dampening, nesterov, grad_scale=1.0, master_weights=False):
+    def __init__(self, lr, penalty, momentum, dampening, nesterov, grad_scale=1.0, master_weights=False,
+                 capturable=False):
         if momentum is None:
             assert dampening is None and not nesterov, \
                 "Dampening and Nesterov momentum flag should be enabled together with momentum."
@@ -107,13 +197,22 @@ class StochasticGD:
             assert 0.0 <= dampening <= 1.0, f"Dampening value should be between 0.0 and 1.0, got: {dampening}"
         self.lr, self.penalty, self.momentum, self.dampening, self.nesterov = float(lr), penalty, momentum, dampening, nesterov
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
+        self.capturable = bool(capturable)
 
     @staticmethod
     def new(lr, penalty=None, momentum=None, dampening=None, nesterov=False, **kw) -> Optimizer:
-        return Optimizer(StochasticGD(lr, penalty or NoPenalty(), momentum, dampening, nesterov, **kw))
+        return _optimizer(StochasticGD(lr, penalty or NoPenalty(), momentum, dampening, nesterov, **kw))
 
     def into_param(self, variable: V.VarDiff) -> _SGDParam:
         return _SGDParam(variable, self)
+
+    def multi_step(self, params, hyper) -> None:
+        for p in params:
+            p.prepare()
+        V._ck(V.lib.nkg_multi_sgd_step(_handles(params), len(params), _ptrs([p.buffer for p in params]),
+                                       _ptrs([p.master for p in params]), hyper, float(self.penalty.lambda_),
+                                       float(self.momentum or 0.0), float(self.dampening or 0.0),
+                                       int(bool(self.nesterov)), float(self.grad_scale)))
 
 
 # ------------------------------------------------------------------------------------------- Adam family (8-f rank 2)
@@ -157,16 +256,25 @@ class Adam:
     """`Adam::new(lr, beta1, beta2, penalty, eps)` (adam/mod.rs:43-60)."""
     amsgrad = False
 
-    def __init__(self, lr, beta1, beta2, penalty, eps, grad_scale=1.0, master_weights=False):
+    def __init__(self, lr, beta1, beta2, penalty, eps, grad_scale=1.0, master_weights=False, capturable=False):
         self.lr, self.beta1, self.beta2, self.penalty, self.eps = float(lr), float(beta1), float(beta2), penalty, float(eps)
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
+        self.capturable = bool(capturable)
 
     @classmethod
     def new(cls, lr, beta1=0.9, beta2=0.999, penalty=None, eps=1e-8, **kw) -> Optimizer:
-        return Optimizer(cls(lr, beta1, beta2, penalty or NoPenalty(), eps, **kw))
+        return _optimizer(cls(lr, beta1, beta2, penalty or NoPenalty(), eps, **kw))
 
     def into_param(self, variable):
         return _AdamParam(variable, self)
+
+    def multi_step(self, params, hyper) -> None:
+        l1, l2 = _l1_l2(self.penalty)
+        V._ck(V.lib.nkg_multi_adam_step(_handles(params), len(params), _ptrs([p.exp_avg for p in params]),
+                                        _ptrs([p.exp_avg_sq for p in params]),
+                                        _ptrs([p.max_exp_avg_sq for p in params]), _ptrs([p.master for p in params]),
+                                        hyper, float(self.beta1), float(self.beta2), float(self.eps), l1, l2,
+                                        float(self.grad_scale)))
 
 
 class AMSGrad(Adam):
@@ -184,7 +292,7 @@ class _RMSPropParam(_MasterMixin):
         self.grad_avg = _state(variable) if status.centered else None
         self._init_master(variable, status)
 
-    def optimize(self) -> None:
+    def prepare(self) -> None:
         s = self.status
         use_mom = s.momentum is not None and s.momentum > np.finfo(np.float32).eps
         if use_mom and self.buffer is None:
@@ -195,6 +303,10 @@ class _RMSPropParam(_MasterMixin):
             self.grad_avg = _state(self.variable)
         if not s.centered:
             self.grad_avg = None
+
+    def optimize(self) -> None:
+        s = self.status
+        self.prepare()
         l1, l2 = _l1_l2(s.penalty)
         V._ck(V.lib.nkg_rmsprop_step(self.variable._h, self.square_avg.ptr, _ptr(self.grad_avg), _ptr(self.buffer),
                                      _ptr(self.master), float(s.lr), float(s.alpha if s.alpha is not None else 0.0),
@@ -207,19 +319,31 @@ class _RMSPropParam(_MasterMixin):
 class RMSProp:
     """`RMSProp::new(lr, penalty, alpha, momentum, centered, eps)` (rmsprop/mod.rs:67-100), same validation."""
 
-    def __init__(self, lr, penalty, alpha, momentum, centered, eps, grad_scale=1.0, master_weights=False):
+    def __init__(self, lr, penalty, alpha, momentum, centered, eps, grad_scale=1.0, master_weights=False,
+                 capturable=False):
         if alpha is not None:
             assert 0.0 <= alpha <= 1.0, f"Dampening value should be between 0.0 and 1.0, got: {alpha}"
         self.lr, self.penalty, self.alpha, self.momentum = float(lr), penalty, alpha, momentum
         self.centered, self.eps = bool(centered), float(eps)
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
+        self.capturable = bool(capturable)
 
     @staticmethod
     def new(lr, penalty=None, alpha=0.99, momentum=None, centered=False, eps=1e-8, **kw) -> Optimizer:
-        return Optimizer(RMSProp(lr, penalty or NoPenalty(), alpha, momentum, centered, eps, **kw))
+        return _optimizer(RMSProp(lr, penalty or NoPenalty(), alpha, momentum, centered, eps, **kw))
 
     def into_param(self, variable):
         return _RMSPropParam(variable, self)
+
+    def multi_step(self, params, hyper) -> None:
+        for p in params:
+            p.prepare()
+        l1, l2 = _l1_l2(self.penalty)
+        V._ck(V.lib.nkg_multi_rmsprop_step(_handles(params), len(params), _ptrs([p.square_avg for p in params]),
+                                           _ptrs([p.grad_avg for p in params]), _ptrs([p.buffer for p in params]),
+                                           _ptrs([p.master for p in params]), hyper,
+                                           float(self.alpha if self.alpha is not None else 0.0), float(self.eps),
+                                           float(self.momentum or 0.0), l1, l2, float(self.grad_scale)))
 
 
 class _AdagradParam(_MasterMixin):
@@ -244,13 +368,23 @@ class _AdagradParam(_MasterMixin):
 class Adagrad:
     """`Adagrad::new(lr, lr_decay, penalty, eps)` (adagrad/mod.rs:50-63)."""
 
-    def __init__(self, lr, lr_decay, penalty, eps, grad_scale=1.0, master_weights=False):
+    def __init__(self, lr, lr_decay, penalty, eps, grad_scale=1.0, master_weights=False, capturable=False):
         self.lr, self.lr_decay, self.penalty, self.eps = float(lr), float(lr_decay), penalty, float(eps)
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
+        self.capturable = bool(capturable)
 
     @staticmethod
     def new(lr, lr_decay=0.0, penalty=None, eps=1e-10, **kw) -> Optimizer:
-        return Optimizer(Adagrad(lr, lr_decay, penalty or NoPenalty(), eps, **kw))
+        return _optimizer(Adagrad(lr, lr_decay, penalty or NoPenalty(), eps, **kw))
 
     def into_param(self, variable):
         return _AdagradParam(variable, self)
+
+    def multi_step(self, params, hyper) -> None:
+        l1, l2 = _l1_l2(self.penalty)
+        V._ck(V.lib.nkg_multi_adagrad_step(_handles(params), len(params), _ptrs([p.grad_sq for p in params]),
+                                           _ptrs([p.master for p in params]), hyper, float(self.lr_decay),
+                                           float(self.eps), l1, l2, float(self.grad_scale)))
+
+
+from . import lr_scheduler  # noqa: E402  (optim.lr_scheduler, as in the reference)

@@ -77,6 +77,10 @@ _G = {
     "nkg_adam_step": (i32, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, f32]),
     "nkg_rmsprop_step": (i32, [vp, vp, vp, vp, vp, f32, f32, f32, f32, f32, f32, f32]),
     "nkg_adagrad_step": (i32, [vp, vp, vp, i64, f32, f32, f32, f32, f32, f32]),
+    "nkg_multi_sgd_step": (i32, [pvp, i32, pvp, pvp, vp, f32, f32, f32, i32, f32]),
+    "nkg_multi_adam_step": (i32, [pvp, i32, pvp, pvp, pvp, pvp, vp, f32, f32, f32, f32, f32, f32]),
+    "nkg_multi_rmsprop_step": (i32, [pvp, i32, pvp, pvp, pvp, pvp, vp, f32, f32, f32, f32, f32, f32]),
+    "nkg_multi_adagrad_step": (i32, [pvp, i32, pvp, pvp, vp, f32, f32, f32, f32, f32]),
     "nkg_set_grad_hook": (i32, [vp, vp, vp, i32]),
     "nkg_set_grad_rs": (i32, [vp, i32, i32, pvp, vp, vp]),
     "nkg_chunks": (i32, [vp, i32, pi64, i32, pvp, C.POINTER(i32)]),
