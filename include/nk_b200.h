@@ -58,9 +58,8 @@ typedef enum { NK_GEMM_AUTO = 0, NK_GEMM_SIMT = 1, NK_GEMM_TC = 2, NK_GEMM_TCGEN
  * mode it was captured with. */
 typedef enum { NK_F32_GEMM_IEEE = 0, NK_F32_GEMM_TF32 = 1, NK_F32_GEMM_TF32X3 = 2 } nk_f32_gemm_mode;
 /* Convolution engine selection (nk_conv_config): AUTO = tensor-core kernels wherever they apply; DIRECT = the CUDA-core
- * kernels only (the parity path the reference's goldens run on); UNFUSED = AUTO (the backward runs dW and dX as two
- * products on every engine). */
-typedef enum { NK_CONV_AUTO = 0, NK_CONV_DIRECT = 1, NK_CONV_UNFUSED = 2 } nk_conv_engine;
+ * kernels only (the parity path the reference's goldens run on). */
+typedef enum { NK_CONV_AUTO = 0, NK_CONV_DIRECT = 1 } nk_conv_engine;
 
 /* ---- context (replaces cuda::Device, neuronika-variable/src/cuda/device.rs:11-75) ---- */
 int nk_ctx_create(int device, nk_ctx** out);
@@ -314,22 +313,6 @@ int nk_conv2d_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbias, cons
                          const void* x, int64_t n, int64_t cin, int64_t h, int64_t wd,
                          int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh,
                          int64_t dw, int64_t groups, int dtype, float beta);
-/* Both halves of ConvolutionBackward::backward (convolution/mod.rs:146-226, which runs the input and
- * the kernel half back to back) in one call: dx = beta_dx*dx + ..., dw = beta_dw*dw + ...,
- * dbias likewise (or NULL).  The two calls above in sequence. */
-int nk_conv2d_bwd(nk_ctx* ctx, void* dx, float beta_dx, void* dwt, int dw_dtype, void* dbias,
-                  float beta_dw, const void* g, const void* x, const void* w, int64_t n,
-                  int64_t cin, int64_t h, int64_t wd, int64_t cout, int64_t kh, int64_t kw,
-                  int64_t sh, int64_t sw, int64_t dh, int64_t dw, int64_t groups, int dtype);
-/* The same when the output gradient is ONE value everywhere -- VarDiff::backward(seed) on the convolution's own
- * output fills the root gradient with the seed (vardiff.rs:125-141): the gradient is filled into a stream-ordered
- * temporary that is released when the call returns, then nk_conv2d_bwd runs on it, so the caller never keeps a
- * materialised root gradient.  Same results as fill + nk_conv2d_bwd.  Returns NK_ERR_UNSUPPORTED (nothing done) for
- * f32 or grouped convolutions: the caller then materialises the gradient itself. */
-int nk_conv2d_bwd_uniform(nk_ctx* ctx, void* dx, float beta_dx, void* dwt, int dw_dtype, void* dbias,
-                          float beta_dw, float g_value, const void* x, const void* w, int64_t n, int64_t cin,
-                          int64_t h, int64_t wd, int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw,
-                          int64_t dh, int64_t dw, int64_t groups, int dtype);
 /* 1-D / 3-D convolution, x (N, Cin, s[0..nsp)), w (Cout, Cin/groups, k[0..nsp)), nsp = 1..3 sample dims
  * (the reference's convolution is generic over them: convolution/mod.rs:85-226, goldens
  * convolution/test.rs:144-239, 306-444 and the strided / dilated / grouped siblings).  CUDA-core gather

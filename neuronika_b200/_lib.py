@@ -119,8 +119,6 @@ _PROTOS = {
     "nk_pad2d_bwd": (i32, [vp, vp, vp, i64, i64, i64, i64, i64, i32, f32]),
     "nk_conv2d_fwd": (i32, [vp, vp, vp, vp, vp, i32] + [i64] * 12 + [i32]),
     "nk_conv2d_bwd_input": (i32, [vp, vp, vp, vp] + [i64] * 12 + [i32, f32]),
-    "nk_conv2d_bwd": (i32, [vp, vp, f32, vp, i32, vp, f32, vp, vp, vp] + [i64] * 12 + [i32]),
-    "nk_conv2d_bwd_uniform": (i32, [vp, vp, f32, vp, i32, vp, f32, f32, vp, vp] + [i64] * 12 + [i32]),
     "nk_conv2d_bwd_kernel": (i32, [vp, vp, i32, vp, vp, vp] + [i64] * 12 + [i32, f32]),
     "nk_ipc_alloc": (i32, [vp, sz, pvp]),
     "nk_ipc_free": (i32, [vp, vp]),

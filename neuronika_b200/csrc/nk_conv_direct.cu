@@ -260,46 +260,4 @@ int nk_conv2d_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbias, cons
   return NK_OK;
 }
 
-// both halves of ConvolutionBackward::backward (convolution/mod.rs:146-226) in one call: the two operators above back to back
-int nk_conv2d_bwd(nk_ctx* ctx, void* dx, float beta_dx, void* dwt, int dw_dtype, void* dbias, float beta_dw,
-                  const void* g, const void* x, const void* w, int64_t n, int64_t cin, int64_t h, int64_t wd,
-                  int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw, int64_t groups,
-                  int dtype) {
-  if (!ctx) return NK_ERR_INVALID_ARG;
-  NK_REQUIRE(ctx, nk_dtype_ok(dtype) && nk_dtype_ok(dw_dtype), "nk_conv2d_bwd: bad dtype");
-  ConvDims d{n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw, groups, 0, 0};
-  int rc = check_dims(ctx, "nk_conv2d_bwd", d);
-  if (rc) return rc;
-  NK_REQUIRE(ctx, dx && dwt && g && x && w, "nk_conv2d_bwd: NULL pointer");
-  rc = nk_conv2d_bwd_kernel(ctx, dwt, dw_dtype, dbias, g, x, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw, groups, dtype,
-                            beta_dw);
-  if (rc) return rc;
-  return nk_conv2d_bwd_input(ctx, dx, g, w, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw, groups, dtype, beta_dx);
-}
-
-int nk_conv2d_bwd_uniform(nk_ctx* ctx, void* dx, float beta_dx, void* dwt, int dw_dtype, void* dbias, float beta_dw,
-                          float g_value, const void* x, const void* w, int64_t n, int64_t cin, int64_t h, int64_t wd,
-                          int64_t cout, int64_t kh, int64_t kw, int64_t sh, int64_t sw, int64_t dh, int64_t dw,
-                          int64_t groups, int dtype) {
-  if (!ctx) return NK_ERR_INVALID_ARG;
-  NK_REQUIRE(ctx, nk_dtype_ok(dtype) && nk_dtype_ok(dw_dtype), "nk_conv2d_bwd_uniform: bad dtype");
-  ConvDims d{n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw, groups, 0, 0};
-  int rc = check_dims(ctx, "nk_conv2d_bwd_uniform", d);
-  if (rc) return rc;
-  NK_REQUIRE(ctx, dx && dwt && x && w, "nk_conv2d_bwd_uniform: NULL pointer");
-  if (dtype != NK_BF16 || groups != 1 || d.n * d.ho * d.wo == 0)
-    return NK_ERR_UNSUPPORTED;   // (without touching last_error) -- the caller materialises the gradient and uses nk_conv2d_bwd
-  // the uniform gradient as a stream-ordered temporary, then the tensor-core backward
-  const size_t ng = size_t(d.n * d.cout * d.ho * d.wo);
-  void* g = nullptr;
-  rc = nk_alloc_uninit(ctx, ng * 2, &g);
-  if (rc) return rc;
-  rc = nk_fill(ctx, g, NK_BF16, ng, g_value);
-  if (rc == NK_OK)
-    rc = nk_conv2d_bwd(ctx, dx, beta_dx, dwt, dw_dtype, dbias, beta_dw, g, x, w, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw,
-                       groups, dtype);
-  nk_free(ctx, g);
-  return rc;
-}
-
 }  // extern "C"

@@ -187,7 +187,7 @@ int nk_gemm_f32_config(nk_ctx* ctx, int mode) {
 }
 int nk_conv_config(nk_ctx* ctx, int engine) {
   if (!ctx) return NK_ERR_INVALID_ARG;
-  NK_REQUIRE(ctx, engine >= NK_CONV_AUTO && engine <= NK_CONV_UNFUSED, "nk_conv_config: bad engine %d", engine);
+  NK_REQUIRE(ctx, engine >= NK_CONV_AUTO && engine <= NK_CONV_DIRECT, "nk_conv_config: bad engine %d", engine);
   ctx->conv_engine = engine;
   return NK_OK;
 }

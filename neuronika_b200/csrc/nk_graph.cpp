@@ -111,9 +111,8 @@ struct Gradient {
   void* rs_user = nullptr;
   int last_writer = -1;             // index (in reverse tape order) of the last node writing it in this pass
   bool hook_fired = false;
-  // fill(v) is deferred: the gradient is "v everywhere" until somebody needs the bytes (get / acc materialise it).
-  // A consumer that takes a uniform gradient as a value (ConvolutionBackward -> nk_conv2d_bwd_uniform) only needs the
-  // bytes for the duration of its own call: backward(seed) on a convolution's own output keeps no materialised G.
+  // fill(v) is deferred: the gradient is "v everywhere" until somebody needs the bytes (get / acc materialise it).  The
+  // nk_fill then runs right before the gradient's first reader, into a buffer allocated without nk_alloc's zero fill.
   bool is_const = false;
   float const_val = 0.f;
   bool is_leaf = false;             // created by requires_grad(): owned by the user, never aliased away by the peephole
@@ -430,7 +429,6 @@ struct MatMulBackward : Backward {
 
 // ------------------------------------------------------------------------------- addition
 struct Convolution;
-struct ConvolutionBackward;
 struct Addition : Forward {  // addition/mod.rs:11-50
   TensorP left, right, data;
   std::shared_ptr<MatMul> fused_gemm;        // peephole: data = mm_t(..) + right in one kernel
@@ -460,9 +458,8 @@ struct Addition : Forward {  // addition/mod.rs:11-50
 
 struct AdditionBackward : Backward {  // addition/mod.rs:52-135 (Left, Right and the composite)
   GradientP left_grad, right_grad;
-  bool left_aliased = false, right_aliased = false;  // right_aliased: the bias gradient is produced by the fused conv dW
+  bool left_aliased = false;
   bool right_fused = false;   // the bias gradient is summed in the epilogue of the dX GEMM above (MatMulBackward::left_colsum)
-  ConvolutionBackward* bias_producer = nullptr;  // the convolution whose dW kernel produces right_grad (right_aliased)
   AdditionBackward(nk_ctx* c, GradientP g, GradientP lg, GradientP rg)
       : Backward(c, std::move(g)), left_grad(std::move(lg)), right_grad(std::move(rg)) {}
   const char* name() const override { return "AdditionBackward"; }
@@ -480,9 +477,8 @@ struct AdditionBackward : Backward {  // addition/mod.rs:52-135 (Left, Right and
   }
   void backward() override {
     acc(left_grad, left_aliased);
-    acc(right_grad, right_aliased || right_fused);
+    acc(right_grad, right_fused);
     if (left_aliased) grad_written(left_grad);    // written by the consumers of this node's output
-    if (right_aliased) grad_written(right_grad);
   }
   void unalias() override;
 };
@@ -745,72 +741,33 @@ void Addition::run_fused_conv() {
   else
     fused_conv->run(right.get(), data.get());
 }
-struct ConvolutionBackward : Backward {  // convolution/mod.rs:357-510: input first, then kernel (:380-388)
+// dW first, as in MatMulBackward: a data-parallel hook on the kernel's gradient fires before dX is launched; the two
+// results are independent, so the order is invisible
+struct ConvolutionBackward : Backward {  // convolution/mod.rs:357-510
   TensorP input, kernel;
   GradientP input_grad, kernel_grad;
-  GradientP bias_grad;  // set by the peephole when the (Cout,1,1) bias add was fused: db rides along with dW
   ConvArgs a;
   ConvolutionBackward(nk_ctx* c, GradientP g, TensorP x, TensorP k, GradientP xg, GradientP kg, const ConvArgs& args)
       : Backward(c, std::move(g)), input(std::move(x)), kernel(std::move(k)), input_grad(std::move(xg)),
         kernel_grad(std::move(kg)), a(args) {}
   const char* name() const override { return "ConvolutionBackward"; }
-  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad, &kernel_grad, &bias_grad}); }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad, &kernel_grad}); }
   void backward() override {
-    void* dbias = nullptr;
-    if (bias_grad) {
-      float bbeta;
-      void* db = bias_grad->acc(&bbeta);
-      Gradient* kr = kernel_grad ? kernel_grad->root() : nullptr;
-      const float kbeta = kr ? (kr->is_zero ? 0.f : 1.f) : -1.f;
-      if (kr && kbeta == bbeta && bias_grad->dtype == kernel_grad->dtype) {
-        dbias = db;  // same accumulate mode and type as dW: one kernel produces both
-      } else {
-        const int64_t dshape[3] = {a.cout, 1, 1};
-        ck(ctx, nk_unbroadcast_acc(ctx, db, bias_grad->dtype, 3, dshape, gradient->get(), gradient->dtype, 4,
-                                   gradient->shape.data(), bbeta));
-      }
-    }
-    // dX is produced in the element type of the output gradient; an input gradient of another type goes through
-    // accumulate()'s temporary (and then the two halves run as separate kernels)
-    const bool dx_same = !input_grad || input_grad->dtype == gradient->dtype;
-    Gradient* gr = gradient->root();
-    if (input_grad && kernel_grad && dx_same) {  // both halves: one pass over the output gradient where the kernels allow it
-      float bx, bw;
-      void* dxp = input_grad->acc(&bx);
-      void* dwp = kernel_grad->acc(&bw);
-      int rc = NK_ERR_UNSUPPORTED;
-      if (gr->is_const && (!bias_grad || dbias))
-        // the output gradient is a deferred fill (backward(seed) on this convolution's own output): filled into a
-        // temporary for the duration of the call
-        rc = nk_conv2d_bwd_uniform(ctx, dxp, bx, dwp, kernel_grad->dtype, dbias, bw, gr->const_val, input->rptr(),
-                                   kernel->rptr(), a.n, a.cin, a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw, a.dh, a.dw,
-                                   a.groups, gradient->dtype);
-      if (rc == NK_ERR_UNSUPPORTED)
-        rc = nk_conv2d_bwd(ctx, dxp, bx, dwp, kernel_grad->dtype, dbias, bw, gradient->get(), input->rptr(),
-                           kernel->rptr(), a.n, a.cin, a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw, a.dh, a.dw, a.groups,
-                           gradient->dtype);
-      ck(ctx, rc);
+    if (kernel_grad) {
+      accumulate(ctx, kernel_grad, [&](void* d, float beta) {
+        ck(ctx, nk_conv2d_bwd_kernel(ctx, d, kernel_grad->dtype, nullptr, gradient->get(), input->rptr(), a.n, a.cin, a.h,
+                                     a.w, a.cout, a.kh, a.kw, a.sh, a.sw, a.dh, a.dw, a.groups, gradient->dtype, beta));
+      });
       grad_written(kernel_grad);
-      grad_written(input_grad);
-    } else {
-      if (input_grad) {
-        const void* g = gradient->get();
-        accumulate(ctx, input_grad, gradient->dtype, [&](void* d, float beta) {
-          ck(ctx, nk_conv2d_bwd_input(ctx, d, g, kernel->rptr(), a.n, a.cin, a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw,
-                                      a.dh, a.dw, a.groups, gradient->dtype, beta));
-        });
-        grad_written(input_grad);
-      }
-      if (kernel_grad) {
-        accumulate(ctx, kernel_grad, [&](void* d, float beta) {
-          ck(ctx, nk_conv2d_bwd_kernel(ctx, d, kernel_grad->dtype, dbias, gradient->get(), input->rptr(), a.n, a.cin,
-                                       a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw, a.dh, a.dw, a.groups, gradient->dtype,
-                                       beta));
-        });
-        grad_written(kernel_grad);
-      }
     }
-    grad_written(bias_grad);
+    if (input_grad) {
+      const void* g = gradient->get();
+      accumulate(ctx, input_grad, gradient->dtype, [&](void* d, float beta) {
+        ck(ctx, nk_conv2d_bwd_input(ctx, d, g, kernel->rptr(), a.n, a.cin, a.h, a.w, a.cout, a.kh, a.kw, a.sh, a.sw, a.dh,
+                                    a.dw, a.groups, gradient->dtype, beta));
+      });
+      grad_written(input_grad);
+    }
   }
 };
 
@@ -832,11 +789,6 @@ void AdditionBackward::unalias() {
   g->is_zero = false;
   g->stale = false;
   left_aliased = false;
-  if (right_aliased) {  // the bias gradient rode along with the convolution's dW: back to its own un-broadcast
-    bias_producer->bias_grad.reset();
-    bias_producer = nullptr;
-    right_aliased = false;
-  }
 }
 
 // ------------------------------------------------------------------------------- sub / mul / div (broadcasting)
@@ -1870,7 +1822,7 @@ void fuse(nkg_var* v) {
       auto abi = add_bwds.find(rb->operand_grad.get());
       if (g_fusion < 3 || abi == add_bwds.end()) continue;
       AdditionBackward* ab = abi->second.get();
-      if (ab->skip || ab->right_fused || ab->right_aliased || !ab->right_grad) continue;
+      if (ab->skip || ab->right_fused || !ab->right_grad) continue;
       Gradient* bg = ab->right_grad.get();
       const Shape& gs = rb->operand_grad->shape;
       if (bg->alias || bg->dtype != NK_F32 || gs.size() != 2 || bg->shape.size() != 1 || bg->shape[0] != gs[1]) continue;
@@ -1892,22 +1844,6 @@ void fuse(nkg_var* v) {
     if (g.use_count() != 2) continue;  // the producer's Backward node + this node
     g->alias = ab->gradient;
     ab->left_aliased = true;
-  }
-  // bias gradient of a fused Conv2d: let the dW kernel produce it (its all-ones K-row) instead of re-reading G
-  for (auto& kv : v->bwd) {
-    auto ab = std::dynamic_pointer_cast<AdditionBackward>(kv.second);
-    if (!ab || !ab->left_aliased || ab->right_aliased || !ab->right_grad) continue;
-    const Shape& bs = ab->right_grad->shape;
-    if (ab->gradient->shape.size() != 4 || bs.size() != 3 || bs[0] != ab->gradient->shape[1] || bs[1] != 1 || bs[2] != 1)
-      continue;
-    for (auto& kv2 : v->bwd) {
-      auto cb = std::dynamic_pointer_cast<ConvolutionBackward>(kv2.second);
-      if (!cb || cb->bias_grad || cb->gradient->root() != ab->gradient->root()) continue;
-      cb->bias_grad = ab->right_grad;
-      ab->bias_producer = cb.get();
-      ab->right_aliased = true;
-      break;
-    }
   }
 }
 

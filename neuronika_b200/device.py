@@ -73,9 +73,8 @@ class Device:
         L.check(L.lib.nk_gemm_f32_config(self.ctx, self.F32_MATMUL_MODES[mode]), self.ctx)
 
     def conv_engine(self, engine: str) -> None:
-        """"auto": tensor-core kernels wherever they apply; "direct": CUDA-core kernels only; "unfused": the same as auto
-        (the backward runs dW and dX as two products on every engine)"""
-        L.check(L.lib.nk_conv_config(self.ctx, {"auto": 0, "direct": 1, "unfused": 2}[engine]), self.ctx)
+        """"auto": tensor-core kernels wherever they apply; "direct": CUDA-core kernels only"""
+        L.check(L.lib.nk_conv_config(self.ctx, {"auto": 0, "direct": 1}[engine]), self.ctx)
 
     @property
     def last_gemm_kernel(self) -> str:

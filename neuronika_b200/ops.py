@@ -262,30 +262,6 @@ def conv2d_bwd_kernel(dw: CuArray, g: CuArray, x: CuArray, stride=(1, 1), dilati
     return dw
 
 
-def conv2d_bwd(dx: CuArray, dw: CuArray, g: CuArray, x: CuArray, w: CuArray, stride=(1, 1), dilation=(1, 1), groups=1,
-               beta_dx=1.0, beta_dw=1.0, dbias: CuArray | None = None):
-    """Both halves of ConvolutionBackward in one call (one pass over `g` on the tensor-core path)."""
-    dev = g.device
-    _ck(lib.nk_conv2d_bwd(dev.ctx, dx.ptr, float(beta_dx), dw.ptr, dw.dtype, dbias.ptr if dbias is not None else None,
-                          float(beta_dw), g.ptr, x.ptr, w.ptr,
-                          *_conv_args(x.shape, w.shape, stride, dilation, groups), g.dtype), dev)
-    return dx, dw
-
-
-def conv2d_bwd_uniform(dx: CuArray, dw: CuArray, g_value: float, x: CuArray, w: CuArray, stride=(1, 1), dilation=(1, 1),
-                       groups=1, beta_dx=1.0, beta_dw=1.0, dbias: CuArray | None = None) -> bool:
-    """ConvolutionBackward for an output gradient that is `g_value` everywhere (a deferred `backward(seed)` fill):
-    the kernel synthesises G.  Returns False (nothing done) when the shape is outside the tensor-core engine."""
-    dev = x.device
-    rc = lib.nk_conv2d_bwd_uniform(dev.ctx, dx.ptr, float(beta_dx), dw.ptr, dw.dtype, dbias.ptr if dbias is not None else None,
-                                   float(beta_dw), float(g_value), x.ptr, w.ptr,
-                                   *_conv_args(x.shape, w.shape, stride, dilation, groups), x.dtype)
-    if rc == -5:
-        return False
-    _ck(rc, dev)
-    return True
-
-
 # ---------------------------------------------------------------- sgd
 def sgd_step(w: CuArray, g: CuArray, lr, l2=0.0, momentum=0.0, dampening=0.0, nesterov=False,
              buf: CuArray | None = None, master: CuArray | None = None, grad_scale=1.0, write_back_grad=True):

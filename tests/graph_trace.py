@@ -682,10 +682,8 @@ SCENARIOS["mlp/level1_rs_and_hooks"] = lambda g: _mlp(g, 1, rs=2, hooks=2)
 
 
 # ---- Conv2d (+ bias) (+ ReLU)
-def _conv(g, level=1, seed_on_conv=False, input_diff=False, fail=None, repeat=1, input_grad=None):
+def _conv(g, level=1, seed_on_conv=False, input_diff=False, repeat=1, input_grad=None):
     g.fusion(level)
-    if fail:
-        g.fail(fail)
     k = g.param((8, 3, 3, 3), BF16, F32)
     b = g.param((8, 1, 1), BF16, F32)
     x = g.param((2, 3, 10, 10), BF16, input_grad) if input_diff else g.leaf((2, 3, 10, 10), BF16)
@@ -706,7 +704,6 @@ def _conv(g, level=1, seed_on_conv=False, input_diff=False, fail=None, repeat=1,
 SCENARIOS["conv/bias_relu_loss"] = lambda g: _conv(g)
 SCENARIOS["conv/bias_relu_loss_level0"] = lambda g: _conv(g, level=0)
 SCENARIOS["conv/seed_on_conv"] = lambda g: _conv(g, seed_on_conv=True)
-SCENARIOS["conv/seed_on_conv_uniform_unsupported"] = lambda g: _conv(g, seed_on_conv=True, fail="nk_conv2d_bwd_uniform")
 SCENARIOS["conv/seed_on_conv_input_diff"] = lambda g: _conv(g, seed_on_conv=True, input_diff=True)
 SCENARIOS["conv/input_diff_loss"] = lambda g: _conv(g, input_diff=True)
 SCENARIOS["conv/input_diff_f32_grad"] = lambda g: _conv(g, input_diff=True, input_grad=F32)

@@ -31,7 +31,7 @@ def O():
 
 def test_config3_conv2d_full_size_properties(nk, dev, O):
     """nn::Conv2d 3->64 k3 on 224x224, batch 256, bf16: forward + backward(seed) through the graph (the path bench.py runs:
-    conv + bias peephole, deferred uniform-gradient backward, both on the wgmma im2col engine).  Checked: samples 0 and 255 of y and dx
+    conv + bias peephole forward, seeded backward, both on the wgmma im2col engine).  Checked: samples 0 and 255 of y and dx
     against the oracle; dW and db against the oracle on a 4-sample problem plus LINEARITY over the batch (the gradient of
     the whole batch equals the sum of the gradients of its two halves, which run through the same kernels)."""
     from neuronika_b200 import ops
@@ -66,13 +66,11 @@ def test_config3_conv2d_full_size_properties(nk, dev, O):
     g4 = np.full((4, cout, h - 2, w - 2), seed, F32)
     ww = np.zeros_like(wt)
     O.conv_backward_kernel(ww, g4, x[:4], (1, 1), (1, 1))
-    Xd, Wd = dev.from_ndarray(x, nk.BF16), dev.from_ndarray(wt, nk.BF16)
     parts = []
     for lo, hi in ((0, 4), (0, n // 2), (n // 2, n)):
-        d_x = dev.zeros((hi - lo, cin, h, w), nk.BF16)
         d_w = dev.zeros(wt.shape, nk.F32)
         xs = dev.from_ndarray(x[lo:hi], nk.BF16)
-        assert ops.conv2d_bwd_uniform(d_x, d_w, seed, xs, Wd, beta_dx=0.0, beta_dw=0.0)
+        ops.conv2d_bwd_kernel(d_w, dev.full((hi - lo, cout, h - 2, w - 2), seed, nk.BF16), xs, beta=0.0)
         parts.append(d_w.as_ndarray().astype(np.float64))
     assert np.all(np.abs(parts[0] - ww) <= 2e-3 * float(np.sqrt((ww.astype(np.float64) ** 2).mean())) + 1e-5 * np.abs(ww))
     total = parts[1] + parts[2]

@@ -679,8 +679,8 @@ def test_fusion_level_2_relu_backward_in_the_gemm_epilogue(nk, dev, O):
 
 
 def test_conv_backward_with_a_uniform_output_gradient(nk, dev, O):
-    """backward(seed) on a convolution's own output: the fill of the root gradient is deferred to the convolution's
-    backward -- same results as filling the gradient and reading it back"""
+    """backward(seed) on a convolution's own output: the graph fills the root gradient and runs the convolution's two
+    backward calls on it -- the same launches and results as that sequence made by hand"""
     from neuronika_b200 import ops
     rng = np.random.default_rng(71)
     x = O.bf16_round(rng.uniform(0, 1, (3, 3, 20, 24)).astype(F32))
@@ -689,22 +689,19 @@ def test_conv_backward_with_a_uniform_output_gradient(nk, dev, O):
     seed = 0.37
     sb = float(O.bf16_round(np.array([seed], F32))[0])
     g = np.full((3, 64, 18, 22), sb, F32)
-    G = dev.from_ndarray(g, nk.BF16)
-    dx1, dw1, db1 = dev.zeros(x.shape, nk.BF16), dev.zeros(w.shape, nk.F32), dev.zeros((64, 1, 1), nk.F32)
-    ops.conv2d_bwd(dx1, dw1, G, X, W, beta_dx=0.0, beta_dw=0.0, dbias=db1)
     dx2, dw2, db2 = dev.zeros(x.shape, nk.BF16), dev.zeros(w.shape, nk.F32), dev.zeros((64, 1, 1), nk.F32)
     before = dev.launches
-    assert ops.conv2d_bwd_uniform(dx2, dw2, seed, X, W, beta_dx=0.0, beta_dw=0.0, dbias=db2)
-    uniform_launches = dev.launches - before
-    assert np.array_equal(dx1.as_ndarray(), dx2.as_ndarray())                  # same G, same kernels
-    assert np.allclose(dw1.as_ndarray(), dw2.as_ndarray(), rtol=1e-5, atol=1e-4)   # f32 atomics across CTAs
-    assert np.allclose(db1.as_ndarray(), db2.as_ndarray(), rtol=1e-5)
+    G = dev.full(g.shape, seed, nk.BF16)
+    ops.conv2d_bwd_kernel(dw2, G, X, beta=0.0, dbias=db2)
+    ops.conv2d_bwd_input(dx2, G, W, beta=0.0)
+    sequence_launches = dev.launches - before
+    assert np.array_equal(G.as_ndarray(), g)
     wx, ww = np.zeros_like(x), np.zeros_like(w)
     O.conv_backward_input(wx, g, w, (1, 1), (1, 1))
     O.conv_backward_kernel(ww, g, x, (1, 1), (1, 1))
     assert np.all(np.abs(dx2.as_ndarray() - wx) <= 2.0 ** -7 * np.abs(wx) + 1e-3)
     assert np.all(np.abs(dw2.as_ndarray() - ww) <= 1e-3 * (1 + np.abs(ww)))
-    # through the graph: y = conv(x) + b; y.backward(seed) never materialises y's gradient ...
+    # through the graph: y = conv(x) + b
     Xv = nk.from_ndarray(dev, x, nk.BF16).requires_grad()
     Wv = nk.from_ndarray(dev, w, nk.BF16).requires_grad(nk.F32)
     Bv = nk.from_ndarray(dev, np.zeros((64, 1, 1), F32), nk.BF16).requires_grad(nk.F32)
@@ -713,11 +710,10 @@ def test_conv_backward_with_a_uniform_output_gradient(nk, dev, O):
     before = dev.launches
     y.backward(seed)
     assert dev.last_conv_kernel == "wgmma_im2col_gemm_dx"
-    assert dev.launches - before <= uniform_launches + 2                       # the uniform call, no separate fill / bias pass
-    assert np.array_equal(Xv.grad(), dx2.as_ndarray())
-    assert np.allclose(Wv.grad(), dw2.as_ndarray(), rtol=1e-5, atol=1e-4)
+    assert dev.launches - before == sequence_launches
+    assert np.array_equal(Xv.grad(), dx2.as_ndarray())                          # same G, same kernels
+    assert np.allclose(Wv.grad(), dw2.as_ndarray(), rtol=1e-5, atol=1e-4)       # f32 atomics across CTAs
     assert np.allclose(Bv.grad().ravel(), db2.as_ndarray().ravel(), rtol=1e-5)
-    # ... but reading it gives the fill
     assert np.array_equal(y.grad(), g)
     # the f32 / direct-engine path materialises the fill and gives the oracle's numbers
     Xf, Wf = nk.from_ndarray(dev, x).requires_grad(), nk.from_ndarray(dev, w).requires_grad()

@@ -572,10 +572,10 @@ def test_conv2d_tensor_core_backward_input(nk, dev, O, shape, cout):
 @pytest.mark.parametrize("shape,cout", [((2, 3, 20, 24), 64), ((1, 3, 224, 224), 64), ((3, 1, 9, 40), 32),
                                         ((2, 2, 70, 16), 16), ((2, 3, 130, 256), 64), ((5, 3, 120, 64), 128),
                                         ((1, 3, 113, 24), 16)])
-def test_conv2d_tensor_core_backward_fused(nk, dev, O, shape, cout):
-    """ConvolutionBackward in one call (nk_conv2d_bwd): dW (+ dbias) and dX on the tensor cores.  Same contract as the two
-    separate operators: accumulate with beta = 1, overwrite with beta = 0; results agree with the oracle and with the
-    CUDA-core engine."""
+def test_conv2d_tensor_core_backward_kernel_then_input(nk, dev, O, shape, cout):
+    """ConvolutionBackward's two calls on one output gradient, in the graph's order: dW (+ dbias), then dX, on the tensor
+    cores.  Accumulate with beta = 1, overwrite with beta = 0; results agree with the oracle and with the CUDA-core
+    engine."""
     import os
     from neuronika_b200 import ops
     rng = np.random.default_rng(14)
@@ -594,22 +594,26 @@ def test_conv2d_tensor_core_backward_fused(nk, dev, O, shape, cout):
     sw = float(np.sqrt((want_dw.astype(np.float64) ** 2).mean())) + 1e-9
     G, X, Wd = dev.from_ndarray(g, nk.BF16), dev.from_ndarray(x, nk.BF16), dev.from_ndarray(w, nk.BF16)
 
+    def backward(dx, dw, beta, dbias=None):
+        ops.conv2d_bwd_kernel(dw, G, X, beta=beta, dbias=dbias)
+        ops.conv2d_bwd_input(dx, G, Wd, beta=beta)
+
     dx, dw, db = dev.from_ndarray(d0, nk.BF16), dev.from_ndarray(w0, nk.F32), dev.from_ndarray(b0, nk.F32)
-    ops.conv2d_bwd(dx, dw, G, X, Wd, beta_dx=1.0, beta_dw=1.0, dbias=db)
+    backward(dx, dw, 1.0, dbias=db)
     assert dev.last_conv_kernel == "wgmma_im2col_gemm_dx"
     assert np.all(np.abs(dx.as_ndarray() - (want_dx + d0)) <= 2e-3 * sx + 2.0 ** -7 * np.abs(want_dx + d0))
     assert np.all(np.abs(dw.as_ndarray() - (w0 + want_dw)) <= 2e-3 * sw + 1e-5)
     assert np.all(np.abs(db.as_ndarray() - (b0 + want_db)) <= 2e-3 * (np.abs(want_db).max() + 1) + 1e-4)
 
     dx2, dw2 = dev.from_ndarray(d0, nk.BF16), dev.from_ndarray(w0, nk.F32)   # overwrite mode, no dbias
-    ops.conv2d_bwd(dx2, dw2, G, X, Wd, beta_dx=0.0, beta_dw=0.0)
+    backward(dx2, dw2, 0.0)
     assert np.all(np.abs(dx2.as_ndarray() - want_dx) <= 2e-3 * sx + 2.0 ** -8 * np.abs(want_dx))
     assert np.all(np.abs(dw2.as_ndarray() - want_dw) <= 2e-3 * sw + 1e-5)
 
     dev.conv_engine("direct")                  # an independent implementation: the same numbers to rounding
     try:
         dx3, dw3 = dev.from_ndarray(d0, nk.BF16), dev.from_ndarray(w0, nk.F32)
-        ops.conv2d_bwd(dx3, dw3, G, X, Wd, beta_dx=0.0, beta_dw=0.0)
+        backward(dx3, dw3, 0.0)
         assert dev.last_conv_kernel == "direct_bwd_input"
     finally:
         dev.conv_engine("auto")
