@@ -58,7 +58,9 @@ typedef enum { NK_GEMM_AUTO = 0, NK_GEMM_SIMT = 1, NK_GEMM_TC = 2, NK_GEMM_TCGEN
  * mode it was captured with. */
 typedef enum { NK_F32_GEMM_IEEE = 0, NK_F32_GEMM_TF32 = 1, NK_F32_GEMM_TF32X3 = 2 } nk_f32_gemm_mode;
 /* Convolution engine selection (nk_conv_config): AUTO = tensor-core kernels wherever they apply; DIRECT = the CUDA-core
- * kernels only (the parity path the reference's goldens run on). */
+ * kernels only (the parity path the reference's goldens run on), in every f32 convolution mode.  f32 convolutions stay on
+ * the CUDA cores under AUTO too unless nk_conv_f32_config opts them into TF32 / 3xTF32; grouped (groups > 1) ones stay
+ * there in every mode. */
 typedef enum { NK_CONV_AUTO = 0, NK_CONV_DIRECT = 1 } nk_conv_engine;
 
 /* ---- context (replaces cuda::Device, neuronika-variable/src/cuda/device.rs:11-75) ---- */
@@ -79,6 +81,14 @@ int nk_conv_config(nk_ctx* ctx, int engine /* nk_conv_engine */);
  * them) in `mode` (nk_f32_gemm_mode).  The GEMM engine setting wins: NK_GEMM_SIMT keeps every product on the CUDA cores.
  * Errors: NK_ERR_INVALID_ARG for an unknown mode. */
 int nk_gemm_f32_config(nk_ctx* ctx, int mode /* nk_f32_gemm_mode */);
+/* f32, groups = 1 convolutions of nk_conv2d_* / nk_convnd_* / nk_conv_layer_nd_* (and every graph node built on them) in
+ * `mode` (nk_f32_gemm_mode values), separately from nk_gemm_f32_config.  IEEE (the default): the CUDA-core kernels, as
+ * always.  TF32 / TF32X3: im2col + the TF32 / 3xTF32 wgmma GEMM for every such call with a non-empty batch, whatever its
+ * shape, with x (fill values included), w and g rounded as nk_gemm_f32_config describes; nk_last_conv_kernel names it
+ * "tf32_im2col_*" / "tf32x3_im2col_*" (2-D) or "tf32_im2col_nd_*" / "tf32x3_im2col_nd_*" (1-D / 3-D).
+ * nk_conv_config(DIRECT) wins.  The mode is read when a convolution is called; a captured step keeps the mode it was
+ * captured with.  Errors: NK_ERR_INVALID_ARG for an unknown mode. */
+int nk_conv_f32_config(nk_ctx* ctx, int mode /* nk_f32_gemm_mode */);
 /* name of the kernel variant the last nk_gemm call used ("wgmma_nt_128x256", "simt", ...) */
 const char* nk_last_gemm_kernel(nk_ctx* ctx);
 

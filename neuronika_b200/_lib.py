@@ -73,6 +73,7 @@ _PROTOS = {
     "nk_gemm_config": (i32, [vp, i32]),
     "nk_gemm_f32_config": (i32, [vp, i32]),
     "nk_conv_config": (i32, [vp, i32]),
+    "nk_conv_f32_config": (i32, [vp, i32]),
     "nk_last_gemm_kernel": (C.c_char_p, [vp]),
     "nk_last_conv_kernel": (C.c_char_p, [vp]),
     "nk_alloc": (i32, [vp, sz, C.POINTER(vp)]),

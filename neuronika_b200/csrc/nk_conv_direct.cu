@@ -1,7 +1,7 @@
 // Direct (CUDA-core) 2-D convolution kernels: the general engine for every stride / dilation /
-// groups combination and both element types.  The tensor-core im2col engine (nk_conv_gemm.cu)
-// takes over for the shapes it supports; this file is the complete, always-valid
-// path and what the reference's own golden cases (tiny, integer valued) run through.
+// groups combination and both element types.  The tensor-core im2col engines take over for the shapes they support
+// (bf16: nk_conv_gemm.cu; f32 once nk_conv_f32_config has set TF32 / TF32X3: nk_conv_tf32.cu); this file is the
+// complete, always-valid path and what the reference's own golden cases (tiny, integer valued) run through.
 // Reference semantics: convolution/mod.rs:85-123 (fwd, beta = 0), :146-189 (dX, accumulate),
 // :191-226 (dW, accumulate), grouped variants :125-144, 228-294; arg checks utils.rs:427-496.
 #include <stdlib.h>
@@ -167,6 +167,9 @@ int nk_conv2d_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void
   const int64_t total = d.n * d.cout * d.ho * d.wo;
   if (total == 0) return NK_OK;
   NK_REQUIRE(ctx, y && x && w, "nk_conv2d_fwd: NULL pointer");
+  const int64_t in_sp[2] = {h, wd}, ks[2] = {kh, kw}, st[2] = {sh, sw}, dl[2] = {dh, dw}, no_pad[2] = {0, 0};
+  if (nk_conv_tf32_on(ctx, dtype, groups))
+    return nk_conv_tf32_fwd(ctx, y, x, w, bias, relu, 2, n, cin, in_sp, cout, ks, st, dl, no_pad, NK_PAD_CONSTANT, 0.f, false);
   if (dtype == NK_BF16 && groups == 1 && ctx->conv_engine != NK_CONV_DIRECT) {
     rc = nk_conv_gemm_fwd(ctx, y, x, w, bias, relu, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw);
     if (rc != NK_ERR_UNSUPPORTED) return rc;
@@ -192,6 +195,9 @@ int nk_conv2d_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int
   const int64_t total = d.n * d.cin * d.h * d.w;
   if (total == 0) return NK_OK;
   NK_REQUIRE(ctx, dx && g && w, "nk_conv2d_bwd_input: NULL pointer");
+  const int64_t in_sp[2] = {h, wd}, ks[2] = {kh, kw}, st[2] = {sh, sw}, dl[2] = {dh, dw}, no_pad[2] = {0, 0};
+  if (nk_conv_tf32_on(ctx, dtype, groups))
+    return nk_conv_tf32_bwd_input(ctx, dx, g, w, 2, n, cin, in_sp, cout, ks, st, dl, no_pad, NK_PAD_CONSTANT, beta, false);
   if (dtype == NK_BF16 && groups == 1 && ctx->conv_engine != NK_CONV_DIRECT) {
     rc = nk_conv_gemm_bwd_input(ctx, dx, g, w, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw, beta);
     if (rc != NK_ERR_UNSUPPORTED) return rc;
@@ -217,6 +223,17 @@ int nk_conv2d_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbias, cons
   const int64_t nw = d.cout * (d.cin / d.groups) * d.kh * d.kw;
   // an empty batch adds nothing: dW (and dbias) = beta * dW, as in nk_convnd_bwd_kernel; g and x may then be NULL
   NK_REQUIRE(ctx, dwt && (d.n == 0 || (g && x)), "nk_conv2d_bwd_kernel: NULL pointer");
+  const int64_t in_sp[2] = {h, wd}, ks[2] = {kh, kw}, st[2] = {sh, sw}, dl[2] = {dh, dw}, no_pad[2] = {0, 0};
+  if (d.n > 0 && nk_conv_tf32_on(ctx, dtype, groups)) {
+    rc = nk_conv_tf32_bwd_kernel(ctx, dwt, dw_dtype, g, x, 2, n, cin, in_sp, cout, ks, st, dl, no_pad, NK_PAD_CONSTANT, 0.f,
+                                 beta, false);
+    if (rc == NK_OK && dbias) {
+      int64_t dshape[3] = {d.cout, 1, 1};
+      int64_t gshape[4] = {d.n, d.cout, d.ho, d.wo};
+      rc = nk_unbroadcast_acc(ctx, dbias, dw_dtype, 3, dshape, g, dtype, 4, gshape, beta);
+    }
+    return rc;
+  }
   if (d.n > 0 && dtype == NK_BF16 && groups == 1 && ctx->conv_engine != NK_CONV_DIRECT) {
     rc = nk_conv_gemm_bwd_kernel(ctx, dwt, dw_dtype, g, x, n, cin, h, wd, cout, kh, kw, sh, sw, dh, dw, beta);
     if (rc == NK_OK && dbias) {

@@ -18,7 +18,7 @@
 // mapped to a source index by the padding mode exactly as nk_padnd_fwd maps it (a bit-exact copy or the fill value).
 // col2im writes only the interior dx positions, each the f32 sum of the taps that read padded coordinate u + pad: the
 // reference's pad backward, the interior slice for every mode (pad/mod.rs:157-182).
-#include "nk_internal.cuh"
+#include "nk_conv_im2col.cuh"
 
 int nk_gemm_wgmma_batched(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
                             int64_t lda, int64_t strideA, const void* B, int64_t ldb, int64_t strideB, void* C, int64_t ldc,
@@ -32,14 +32,6 @@ constexpr int64_t kChunkBytes = int64_t(4) << 30;
 
 struct CgDims {
   int64_t n, cin, h, w, cout, kh, kw, sh, sw, dh, dw, ho, wo, K, Kp, L, Lp;
-};
-
-// the 1-D / 3-D layer: sample dims padded to three with leading extents of 1 (kernel 1, stride 1, dilation 1, pad 0)
-struct CgNdDims {
-  int64_t n, cin, cout, K, Kp, L, Lp;
-  int64_t in[3], k[3], s[3], d[3], pad[3], out[3];
-  int mode;        // nk_pad_mode
-  float value;     // fill of the constant mode
 };
 
 // eight consecutive bf16 source elements x[off .. off+7] (2-byte aligned): aligned 4-byte loads + a funnel shift when the
@@ -192,16 +184,7 @@ __global__ void __launch_bounds__(kThreads) finalize_dw_padded(T* __restrict__ d
   dw[idx] = nk_from_f32<T>(v);
 }
 
-// ---- 1-D / 3-D layers with the padding folded into the gather
-// source index of padded coordinate u along an axis of length len padded by p on both sides, or -1 for the fill value:
-// the map of nk_padnd_fwd (nk_pointwise.cu pad_src; reflective/mod.rs:22-31, replicative/mod.rs:22-31)
-__device__ __forceinline__ int pad_src_index(int u, int len, int p, int mode) {
-  if (u >= p && u < len + p) return u - p;
-  if (mode == NK_PAD_REFLECTIVE) return (u < p ? 2 * p - u : 2 * (len + p - 1) - u) - p;
-  if (mode == NK_PAD_REPLICATIVE) return u < p ? 0 : len - 1;
-  return -1;
-}
-
+// ---- 1-D / 3-D layers with the padding folded into the gather (pad_src_index: nk_conv_im2col.cuh)
 // colsT[ns][(c, i0, i1, i2)][l0 .. l0+7] as im2col_kernel, through the padding map.  A vector of eight outputs along one
 // output row (unit stride on the last axis) reads one source row: the fill value when the padding puts that row outside x
 // (constant mode), else a contiguous run (load_run8) when the eight columns are interior; only runs that touch the border
@@ -272,53 +255,6 @@ __global__ void __launch_bounds__(kThreads) im2col_nd_kernel(__nv_bfloat16* __re
   }
 }
 
-// dx[n,c,u] = beta*dx + sum over the taps i and output positions p with p*s + i*d = u + pad (per axis) of
-// dcolsT[ns][(c,i)][p]: only the interior positions of the padded input, whatever the mode; one thread per dx element,
-// the taps summed in f32 and rounded once
-__global__ void __launch_bounds__(kThreads) col2im_nd_kernel(__nv_bfloat16* __restrict__ dx, const float* __restrict__ dcols,
-                                                             CgNdDims d, int64_t n0, int64_t nn, float beta) {
-  const int in0 = int(d.in[0]), in1 = int(d.in[1]), in2 = int(d.in[2]);
-  const int k0 = int(d.k[0]), k1 = int(d.k[1]), k2 = int(d.k[2]);
-  const int o0 = int(d.out[0]), o1 = int(d.out[1]), o2 = int(d.out[2]);
-  const int s0 = int(d.s[0]), s1 = int(d.s[1]), s2 = int(d.s[2]), d0 = int(d.d[0]), d1 = int(d.d[1]), d2 = int(d.d[2]);
-  const int cin = int(d.cin), ksz = k0 * k1 * k2;
-  const uint32_t isz = uint32_t(in0) * uint32_t(in1) * uint32_t(in2);
-  const int64_t total = nn * d.cin * int64_t(isz);
-  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
-  for (int64_t idx = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; idx < total; idx += stride) {
-    const uint32_t pl = uint32_t(idx / isz);            // (ns, c)
-    const uint32_t uv = uint32_t(idx - int64_t(pl) * isz);
-    const int U2 = int(uv % uint32_t(in2)) + int(d.pad[2]);
-    const int t = int(uv / uint32_t(in2));
-    const int U1 = t % in1 + int(d.pad[1]), U0 = t / in1 + int(d.pad[0]);
-    const uint32_t ns = pl / uint32_t(cin), c = pl - ns * uint32_t(cin);
-    const float* dc = dcols + (int64_t(ns) * d.K + int64_t(c) * ksz) * d.Lp;
-    float acc = 0.f;
-    for (int i0 = 0; i0 < k0; ++i0) {
-      const int pu0 = U0 - i0 * d0;
-      if (pu0 < 0) break;
-      const int q0 = pu0 / s0;
-      if (q0 * s0 != pu0 || q0 >= o0) continue;
-      for (int i1 = 0; i1 < k1; ++i1) {
-        const int pu1 = U1 - i1 * d1;
-        if (pu1 < 0) break;
-        const int q1 = pu1 / s1;
-        if (q1 * s1 != pu1 || q1 >= o1) continue;
-        for (int i2 = 0; i2 < k2; ++i2) {
-          const int pu2 = U2 - i2 * d2;
-          if (pu2 < 0) break;
-          const int q2 = pu2 / s2;
-          if (q2 * s2 != pu2 || q2 >= o2) continue;
-          acc += dc[int64_t((i0 * k1 + i1) * k2 + i2) * d.Lp + (int64_t(q0) * o1 + q1) * o2 + q2];
-        }
-      }
-    }
-    __nv_bfloat16* o = dx + n0 * d.cin * int64_t(isz) + idx;
-    if (beta != 0.f) acc += beta * __bfloat162float(*o);
-    *o = __float2bfloat16_rn(acc);
-  }
-}
-
 inline int cg_blocks(nk_ctx* ctx, int64_t items) {
   int64_t b = (items + kThreads - 1) / kThreads;
   const int64_t cap = int64_t(ctx->sm_count) * 16;
@@ -379,8 +315,8 @@ int launch_im2col(nk_ctx* ctx, __nv_bfloat16* cols, const __nv_bfloat16* x, cons
   return NK_OK;
 }
 int launch_col2im(nk_ctx* ctx, __nv_bfloat16* dx, const float* dcols, const CgNdDims& d, int64_t n0, int64_t nn, float beta) {
-  col2im_nd_kernel<<<cg_blocks(ctx, nn * d.cin * d.in[0] * d.in[1] * d.in[2]), kThreads, 0, ctx->stream>>>(dx, dcols, d, n0,
-                                                                                                          nn, beta);
+  col2im_nd_kernel<__nv_bfloat16><<<cg_blocks(ctx, nn * d.cin * d.in[0] * d.in[1] * d.in[2]), kThreads, 0, ctx->stream>>>(
+      dx, dcols, d, n0, nn, beta);
   NK_LAUNCHED(ctx, "col2im_nd");
   return NK_OK;
 }
@@ -502,20 +438,10 @@ int gemm_conv_dw(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, const void
   return NK_OK;
 }
 
-// the layer's geometry: output extents of the padded input, and the 2-D engine's applicability rules (make_dims)
+// the layer's geometry (conv_nd_geometry), and the 2-D engine's applicability rules (make_dims)
 bool make_nd_dims(CgNdDims& d, int nsp, int64_t n, int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k,
                   const int64_t* s, const int64_t* dil, const int64_t* pad, int mode, float value) {
-  d = CgNdDims{};
-  d.n = n, d.cin = cin, d.cout = cout, d.mode = mode, d.value = value;
-  d.K = cin, d.L = 1;
-  for (int a = 0; a < 3; ++a) d.in[a] = d.k[a] = d.s[a] = d.d[a] = d.out[a] = 1, d.pad[a] = 0;
-  for (int a = 0; a < nsp; ++a) {
-    const int j = 3 - nsp + a;
-    d.in[j] = in_sp[a], d.k[j] = k[a], d.s[j] = s[a], d.d[j] = dil[a], d.pad[j] = pad[a];
-    d.out[j] = (in_sp[a] + 2 * pad[a] - dil[a] * (k[a] - 1) - 1) / s[a] + 1;
-    d.K *= k[a];
-    d.L *= d.out[j];
-  }
+  conv_nd_geometry(d, nsp, n, cin, in_sp, cout, k, s, dil, pad, mode, value);
   d.Kp = (d.K + 7) & ~int64_t(7);
   d.Lp = (d.L + 7) & ~int64_t(7);
   return n > 0 && d.L > 0 && d.Kp >= 16 && d.Lp * d.Kp < (int64_t(1) << 31);

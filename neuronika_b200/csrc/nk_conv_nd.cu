@@ -243,6 +243,10 @@ int nk_convnd_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, int nsp, i
   const int64_t total = d.n * d.cout * d.out[0] * d.out[1] * d.out[2];
   if (total == 0) return NK_OK;
   NK_REQUIRE(ctx, y && x && w, "nk_convnd_fwd: NULL pointer");
+  const int64_t no_pad[3] = {0, 0, 0};
+  if (nk_conv_tf32_on(ctx, dtype, groups))
+    return nk_conv_tf32_fwd(ctx, y, x, w, nullptr, 0, nsp, n, cin, in_sp, cout, k, stride, dilation, no_pad, NK_PAD_CONSTANT,
+                            0.f, true);
   const int blocks = nd_blocks(ctx, total);
   if (dtype == NK_BF16)
     convnd_fwd_kernel<__nv_bfloat16><<<blocks, kThreads, 0, ctx->stream>>>((__nv_bfloat16*)y, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, d);
@@ -264,6 +268,10 @@ int nk_convnd_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int
   const int64_t total = d.n * d.cin * d.in[0] * d.in[1] * d.in[2];
   if (total == 0) return NK_OK;
   NK_REQUIRE(ctx, dx && g && w, "nk_convnd_bwd_input: NULL pointer");
+  const int64_t no_pad[3] = {0, 0, 0};
+  if (nk_conv_tf32_on(ctx, dtype, groups))
+    return nk_conv_tf32_bwd_input(ctx, dx, g, w, nsp, n, cin, in_sp, cout, k, stride, dilation, no_pad, NK_PAD_CONSTANT, beta,
+                                  true);
   const int blocks = nd_blocks(ctx, total);
   if (dtype == NK_BF16)
     convnd_bwd_input_kernel<__nv_bfloat16><<<blocks, kThreads, 0, ctx->stream>>>((__nv_bfloat16*)dx, (const __nv_bfloat16*)g, (const __nv_bfloat16*)w, d, beta);
@@ -284,6 +292,10 @@ int nk_convnd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, co
   if (rc) return rc;
   const int64_t welems = d.cout * (d.cin / d.groups) * d.k[0] * d.k[1] * d.k[2];
   NK_REQUIRE(ctx, dwt && (d.n == 0 || (g && x)), "nk_convnd_bwd_kernel: NULL pointer");
+  const int64_t no_pad[3] = {0, 0, 0};
+  if (d.n > 0 && nk_conv_tf32_on(ctx, dtype, groups))
+    return nk_conv_tf32_bwd_kernel(ctx, dwt, dw_dtype, g, x, nsp, n, cin, in_sp, cout, k, stride, dilation, no_pad,
+                                   NK_PAD_CONSTANT, 0.f, beta, true);
   float* scratch;
   rc = nk_workspace(ctx, size_t(welems) * sizeof(float), (void**)&scratch);
   if (rc) return rc;
@@ -312,8 +324,9 @@ int nk_convnd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, co
   return NK_OK;
 }
 
-// The layers pick the engine as nk_conv2d_* do: the tensor cores for bf16 shapes the im2col engine takes (unless
-// nk_conv_config(DIRECT)); otherwise the padded input in a temporary and the CUDA-core kernels above, i.e. the calls of
+// The layers pick the engine as nk_conv2d_* do: the tensor cores for bf16 shapes the im2col engine takes and, in the
+// TF32 / TF32X3 modes of nk_conv_f32_config, for every f32 call (nk_conv_tf32.cu; unless nk_conv_config(DIRECT));
+// otherwise the padded input in a temporary and the CUDA-core kernels above, i.e. the calls of
 // the composed graph pad -> convolution -> + bias, with the same results.
 int nk_conv_layer_nd_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int nsp, int64_t n, int64_t cin,
                          const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* stride,
@@ -325,6 +338,9 @@ int nk_conv_layer_nd_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, con
   if (rc) return rc;
   if (ld.d.n * ld.d.cout * ld.d.out[0] * ld.d.out[1] * ld.d.out[2] == 0) return NK_OK;
   NK_REQUIRE(ctx, y && x && w, "nk_conv_layer_nd_fwd: NULL pointer");
+  if (nk_conv_tf32_on(ctx, dtype, 1))
+    return nk_conv_tf32_fwd(ctx, y, x, w, bias, 0, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, pad_value,
+                            true);
   if (dtype == NK_BF16 && ctx->conv_engine != NK_CONV_DIRECT) {
     rc = nk_conv_gemm_nd_fwd(ctx, y, x, w, bias, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, pad_value);
     if (rc != NK_ERR_UNSUPPORTED) return rc;
@@ -354,6 +370,8 @@ int nk_conv_layer_nd_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void*
   for (int a = 0; a < nsp; ++a) total *= in_sp[a];
   if (total == 0) return NK_OK;
   NK_REQUIRE(ctx, dx && g && w, "nk_conv_layer_nd_bwd_input: NULL pointer");
+  if (nk_conv_tf32_on(ctx, dtype, 1))
+    return nk_conv_tf32_bwd_input(ctx, dx, g, w, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, beta, true);
   if (dtype == NK_BF16 && ctx->conv_engine != NK_CONV_DIRECT) {
     rc = nk_conv_gemm_nd_bwd_input(ctx, dx, g, w, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode, beta);
     if (rc != NK_ERR_UNSUPPORTED) return rc;
@@ -389,6 +407,9 @@ int nk_conv_layer_nd_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, void* dbia
     rc = nk_unbroadcast_acc(ctx, dbias, dw_dtype, nsp + 1, bshape, g, dtype, nsp + 2, gshape, beta);
     if (rc) return rc;
   }
+  if (n > 0 && nk_conv_tf32_on(ctx, dtype, 1))
+    return nk_conv_tf32_bwd_kernel(ctx, dwt, dw_dtype, g, x, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode,
+                                   pad_value, beta, true);
   if (n > 0 && dtype == NK_BF16 && ctx->conv_engine != NK_CONV_DIRECT) {
     rc = nk_conv_gemm_nd_bwd_kernel(ctx, dwt, dw_dtype, g, x, nsp, n, cin, in_sp, cout, k, stride, dilation, pad, pad_mode,
                                     pad_value, beta);

@@ -191,6 +191,12 @@ int nk_conv_config(nk_ctx* ctx, int engine) {
   ctx->conv_engine = engine;
   return NK_OK;
 }
+int nk_conv_f32_config(nk_ctx* ctx, int mode) {
+  if (!ctx) return NK_ERR_INVALID_ARG;
+  NK_REQUIRE(ctx, mode >= NK_F32_GEMM_IEEE && mode <= NK_F32_GEMM_TF32X3, "nk_conv_f32_config: bad mode %d", mode);
+  ctx->f32_conv = mode;
+  return NK_OK;
+}
 const char* nk_last_gemm_kernel(nk_ctx* ctx) { return ctx ? ctx->last_gemm_kernel : "none"; }
 const char* nk_last_conv_kernel(nk_ctx* ctx) { return ctx ? ctx->last_conv_kernel : "none"; }
 

@@ -25,7 +25,10 @@
 // accumulator, which the warpgroup adds to the tile's accumulator with ordinary f32 adds once its group is done: the
 // tensor cores never sum more than 32 products.  Two accumulators per thread limit 3xTF32 tiles to 128 columns.
 // No split-K: every output element is one accumulator's sum in a fixed order, so repeated calls give the same bits.
-#include "nk_internal.cuh"
+// nk_gemm_tf32_packed (nk_tf32.cuh) is the same kernel on operands the caller packed: a batch index is the slowest index
+// of the tile order (A shared or batched, row / reduction-column / C offsets per batch entry) and the bias may be per
+// row; the f32 convolution engine (nk_conv_tf32.cu) runs its three products on it.
+#include "nk_tf32.cuh"
 #include "nk_ptx.cuh"
 
 namespace {
@@ -42,8 +45,13 @@ struct Tf32Params {
   void* C;
   const void* bias;
   float alpha, beta;
-  int bias_bf16, relu;
+  int bias_bf16, relu, row_bias;
   int num_m_blocks, num_n_blocks, num_k_blocks;
+  int k_blocks_total;   // of the packed operands: a batch entry's k-blocks stop there
+  // batch entry b (the slowest index of the tile order): operand rows from b * a_bstride / b * b_bstride, reduction
+  // columns from b * k_bstride, output at C + b * c_bstride
+  int batch, a_bstride, b_bstride, k_bstride;
+  int64_t c_bstride;
 };
 
 template <int BLOCK_N>
@@ -56,7 +64,10 @@ struct Tf32Cfg {
   static constexpr uint32_t SMEM_BYTES = kStages * STAGE_BYTES + 2048;  // + alignment slack + barriers
 };
 
-__device__ __forceinline__ void tile_coords(const Tf32Params& p, int tile, int& m_blk, int& n_blk) {
+__device__ __forceinline__ void tile_coords(const Tf32Params& p, int tile, int& b, int& m_blk, int& n_blk) {
+  const int per_batch = p.num_m_blocks * p.num_n_blocks;
+  b = tile / per_batch;
+  tile -= b * per_batch;
   const int group_size = kGroupM * p.num_n_blocks;
   const int group = tile / group_size, in_group = tile - group * group_size;
   const int first_m = group * kGroupM;
@@ -65,55 +76,51 @@ __device__ __forceinline__ void tile_coords(const Tf32Params& p, int tile, int& 
   n_blk = in_group / gm;
 }
 
-__device__ __forceinline__ float tf32_rna(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
 // One 32 (rows) x 32 (k) tile of op(X) per block of 32 x 8 threads, through shared memory so that both the read of an
-// MN-major operand (along rows) and the write (along k) are coalesced.  dst row r holds, in segment s of K columns,
-// hi for s != lo_seg and lo for s == lo_seg; segments = 1 (TF32, lo_seg = -1) or 3 (3xTF32).
+// MN-major operand (along rows) and the write (along k) are coalesced; every element written by tf32_put.  grid.y
+// steps through the k tiles and grid.z through the batch entries, so K and the batch have no grid limit.
 template <bool MN>
 __global__ void __launch_bounds__(256) tf32_pack_kernel(const float* __restrict__ src, int64_t ld, int64_t R, int64_t K,
-                                                       float* __restrict__ dst, int64_t ldp, int segments, int lo_seg) {
+                                                       float* __restrict__ dst, int64_t ldp, int segments, int lo_seg,
+                                                       int64_t batch, int64_t src_bstride, int64_t dst_bstride,
+                                                       int64_t seg_len) {
   __shared__ float tile[32][33];
-  const int64_t r0 = int64_t(blockIdx.x) * 32, k0 = int64_t(blockIdx.y) * 32;
+  const int64_t r0 = int64_t(blockIdx.x) * 32, k_tiles = (K + 31) / 32;
   const int tx = threadIdx.x, ty = threadIdx.y;
+  bool first = true;
+  for (int64_t b = blockIdx.z; b < batch; b += gridDim.z) {
+    const float* sb = src + b * src_bstride;
+    for (int64_t kt = blockIdx.y; kt < k_tiles; kt += gridDim.y) {
+      const int64_t k0 = kt * 32;
+      if (!first) __syncthreads();   // the previous tile has been read
+      first = false;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int yy = ty + 8 * i;
-    if (MN) {   // element (r, k) at src[k * ld + r]: lanes along r
-      const int64_t r = r0 + tx, k = k0 + yy;
-      if (r < R && k < K) tile[tx][yy] = src[k * ld + r];
-    } else {    // element (r, k) at src[r * ld + k]: lanes along k
-      const int64_t r = r0 + yy, k = k0 + tx;
-      if (r < R && k < K) tile[yy][tx] = src[r * ld + k];
-    }
-  }
-  __syncthreads();
+      for (int i = 0; i < 4; ++i) {
+        const int yy = ty + 8 * i;
+        if (MN) {   // element (r, k) at src[k * ld + r]: lanes along r
+          const int64_t r = r0 + tx, k = k0 + yy;
+          if (r < R && k < K) tile[tx][yy] = sb[k * ld + r];
+        } else {    // element (r, k) at src[r * ld + k]: lanes along k
+          const int64_t r = r0 + yy, k = k0 + tx;
+          if (r < R && k < K) tile[yy][tx] = sb[r * ld + k];
+        }
+      }
+      __syncthreads();
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int yy = ty + 8 * i;
-    const int64_t r = r0 + yy, k = k0 + tx;
-    if (r < R && k < K) {
-      const float x = tile[yy][tx];
-      const float hi = tf32_rna(x);
-      float* d = dst + r * ldp + k;
-      if (segments == 1) {
-        d[0] = hi;
-      } else {
-        const float lo = tf32_rna(__fsub_rn(x, hi));
-        for (int s = 0; s < segments; ++s) d[s * K] = s == lo_seg ? lo : hi;
+      for (int i = 0; i < 4; ++i) {
+        const int yy = ty + 8 * i;
+        const int64_t r = r0 + yy, k = k0 + tx;
+        if (r < R && k < K) tf32_put(dst + b * dst_bstride + r * ldp + k, tile[yy][tx], segments, lo_seg, seg_len);
       }
     }
   }
 }
 
 template <typename TC>
-__device__ __forceinline__ void store_pair(const Tf32Params& p, int64_t row, int64_t col, float a0, float a1, bool pair_ok) {
+__device__ __forceinline__ void store_pair(const Tf32Params& p, TC* cb, int64_t row, int64_t col, float a0, float a1,
+                                           bool pair_ok) {
   if (row >= p.M || col >= p.N) return;
-  TC* c = static_cast<TC*>(p.C) + row * p.ldc + col;
+  TC* c = cb + row * p.ldc + col;
   float v[2] = {a0, a1};
   const int n = col + 1 < p.N ? 2 : 1;
   // nk_gemm_simt.cu store_out: alpha, beta.C, bias, ReLU, rounding to C's type
@@ -122,9 +129,11 @@ __device__ __forceinline__ void store_pair(const Tf32Params& p, int64_t row, int
     if (e >= n) break;
     float x = p.alpha * v[e];
     if (p.beta != 0.f) x += p.beta * nk_to_f32<TC>(c[e]);
-    if (p.bias)
-      x += p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[col + e])
-                       : static_cast<const float*>(p.bias)[col + e];
+    if (p.bias) {
+      const int64_t bi = p.row_bias ? row : col + e;
+      x += p.bias_bf16 ? __bfloat162float(static_cast<const __nv_bfloat16*>(p.bias)[bi])
+                       : static_cast<const float*>(p.bias)[bi];
+    }
     if (p.relu) x = x > 0.f ? x : 0.f;
     v[e] = x;
   }
@@ -163,7 +172,7 @@ tf32_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     ptx::fence_barrier_init();
   }
   __syncthreads();
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  const int num_tiles = p.batch * p.num_m_blocks * p.num_n_blocks;
 
   if (wg == 0) {
     // ===================================================== TMA producer
@@ -172,13 +181,16 @@ tf32_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int m_blk, n_blk;
-        tile_coords(p, tile, m_blk, n_blk);
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+        int b, m_blk, n_blk;
+        tile_coords(p, tile, b, m_blk, n_blk);
+        const int a_row = b * p.a_bstride + m_blk * BLOCK_M, b_row = b * p.b_bstride + n_blk * BLOCK_N;
+        const int k0 = b * p.k_bstride;
+        const int nkb = min(p.num_k_blocks, p.k_blocks_total - k0 / BLOCK_K);
+        for (int kb = 0; kb < nkb; ++kb) {
           ptx::mbar_wait_spin(empty_bar(stage), phase ^ 1u);
           ptx::mbar_expect_tx(full_bar(stage), C_::STAGE_BYTES);
-          ptx::tma_load_2d(smem_a0 + stage * C_::A_BYTES, &tmap_a, full_bar(stage), kb * BLOCK_K, m_blk * BLOCK_M);
-          ptx::tma_load_2d(smem_b0 + stage * C_::B_BYTES, &tmap_b, full_bar(stage), kb * BLOCK_K, n_blk * BLOCK_N);
+          ptx::tma_load_2d(smem_a0 + stage * C_::A_BYTES, &tmap_a, full_bar(stage), k0 + kb * BLOCK_K, a_row);
+          ptx::tma_load_2d(smem_b0 + stage * C_::B_BYTES, &tmap_b, full_bar(stage), k0 + kb * BLOCK_K, b_row);
           if (++stage == kStages) {
             stage = 0;
             phase ^= 1u;
@@ -194,17 +206,17 @@ tf32_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int cw = wg - 1;
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
-  const bool pair_ok = (p.ldc % 2 == 0) && (reinterpret_cast<uintptr_t>(p.C) % (2 * sizeof(TC)) == 0);
   const uint32_t a_off = uint32_t(cw) * (64 * BLOCK_K * 4);   // 64 K-major rows of 128 B
   float acc[BLOCK_N / 2];
   float part[kSplitAcc ? BLOCK_N / 2 : 1];   // kSplitAcc: the current k-block's product
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    int m_blk, n_blk;
-    tile_coords(p, tile, m_blk, n_blk);
+    int b, m_blk, n_blk;
+    tile_coords(p, tile, b, m_blk, n_blk);
     int prev_stage = 0;
-    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+    const int nkb = min(p.num_k_blocks, p.k_blocks_total - b * p.k_bstride / BLOCK_K);
+    for (int kb = 0; kb < nkb; ++kb) {
       ptx::mbar_wait_spin(full_bar(stage), phase);
       // K-major SW128: 8-row groups 1024 B apart (SBO), +32 B per k8 step inside the swizzle row
       const uint64_t adesc = ptx::make_smem_desc_sw128(smem_a0 + stage * C_::A_BYTES + a_off, 16, 1024);
@@ -253,10 +265,12 @@ tf32_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     // ---- drain: thread holds rows r, r + 8 (r = 16 warp + lane / 4) and columns 8j + 2 (lane % 4) + {0, 1}
     const int64_t row = int64_t(m_blk) * BLOCK_M + cw * 64 + warp * 16 + (lane >> 2);
     const int64_t col = int64_t(n_blk) * BLOCK_N + 2 * (lane & 3);
+    TC* cb = static_cast<TC*>(p.C) + b * p.c_bstride;
+    const bool pair_ok = (p.ldc % 2 == 0) && (reinterpret_cast<uintptr_t>(cb) % (2 * sizeof(TC)) == 0);
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
-      store_pair<TC>(p, row, col + 8 * j, acc[4 * j], acc[4 * j + 1], pair_ok);
-      store_pair<TC>(p, row + 8, col + 8 * j, acc[4 * j + 2], acc[4 * j + 3], pair_ok);
+      store_pair<TC>(p, cb, row, col + 8 * j, acc[4 * j], acc[4 * j + 1], pair_ok);
+      store_pair<TC>(p, cb, row + 8, col + 8 * j, acc[4 * j + 2], acc[4 * j + 3], pair_ok);
     }
   }
 }
@@ -272,7 +286,7 @@ int launch_tf32(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, Tf32P
     attr_done[ctx->device & 63] = true;
   }
   p.num_n_blocks = int((p.N + BLOCK_N - 1) / BLOCK_N);
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  const int num_tiles = p.batch * p.num_m_blocks * p.num_n_blocks;
   const int waves = (num_tiles + ctx->sm_count - 1) / ctx->sm_count;
   const int grid = (num_tiles + waves - 1) / waves;
   kern<<<grid, kNumThreads, C_::SMEM_BYTES, ctx->stream>>>(ta, tb, p);
@@ -280,19 +294,56 @@ int launch_tf32(nk_ctx* ctx, const CUtensorMap& ta, const CUtensorMap& tb, Tf32P
   return NK_OK;
 }
 
-// op(X) (R x K; MN: stored (K, R)) -> dst, K-major with leading dimension ldp
-int pack(nk_ctx* ctx, const float* src, int64_t ld, bool mn, int64_t R, int64_t K, float* dst, int64_t ldp, int segments,
-         int lo_seg) {
-  const dim3 grid(unsigned((R + 31) / 32), unsigned((K + 31) / 32)), block(32, 8);
+}  // namespace
+
+int nk_tf32_pack(nk_ctx* ctx, const float* src, int64_t ld, bool mn, int64_t R, int64_t K, float* dst, int64_t ldp,
+                 int segments, int lo_seg, int64_t batch, int64_t src_bstride, int64_t dst_bstride, int64_t seg_len) {
+  NK_REQUIRE(ctx, (R + 31) / 32 < (int64_t(1) << 31), "tf32 pack: operand too large (R=%lld K=%lld)", (long long)R,
+             (long long)K);
+  const int64_t k_tiles = (K + 31) / 32;
+  const dim3 grid(unsigned((R + 31) / 32), unsigned(k_tiles < 65535 ? k_tiles : 65535), unsigned(batch < 65535 ? batch : 65535)),
+      block(32, 8);
+  if (seg_len < 0) seg_len = K;
   if (mn)
-    tf32_pack_kernel<true><<<grid, block, 0, ctx->stream>>>(src, ld, R, K, dst, ldp, segments, lo_seg);
+    tf32_pack_kernel<true><<<grid, block, 0, ctx->stream>>>(src, ld, R, K, dst, ldp, segments, lo_seg, batch, src_bstride,
+                                                            dst_bstride, seg_len);
   else
-    tf32_pack_kernel<false><<<grid, block, 0, ctx->stream>>>(src, ld, R, K, dst, ldp, segments, lo_seg);
+    tf32_pack_kernel<false><<<grid, block, 0, ctx->stream>>>(src, ld, R, K, dst, ldp, segments, lo_seg, batch, src_bstride,
+                                                             dst_bstride, seg_len);
   NK_LAUNCHED(ctx, "tf32_pack");
   return NK_OK;
 }
 
-}  // namespace
+int nk_gemm_tf32_packed(nk_ctx* ctx, const NkTf32Gemm& g) {
+  const int block_n = nk_tf32_block_n(g.N, g.x3);
+  const int64_t m_blocks = (g.M + BLOCK_M - 1) / BLOCK_M, n_blocks = (g.N + block_n - 1) / block_n;
+  NK_REQUIRE(ctx, g.batch >= 1 && g.batch * m_blocks * n_blocks < (int64_t(1) << 31) && g.a_rows < (int64_t(1) << 31) &&
+                  g.b_rows < (int64_t(1) << 31) && g.kp < (int64_t(1) << 31) &&
+                  (g.batch - 1) * (g.a_bstride + g.b_bstride + g.k_bstride) < (int64_t(1) << 31),
+             "tf32 gemm: shape too large (M=%lld N=%lld K=%lld batch=%lld)", (long long)g.M, (long long)g.N,
+             (long long)g.kp, (long long)g.batch);
+  CUtensorMap ta, tb;
+  int rc = make_tmap_2d(ctx, &ta, g.A, g.a_rows, g.kp, g.lda, BLOCK_K, BLOCK_M, NK_F32);
+  if (!rc) rc = make_tmap_2d(ctx, &tb, g.B, g.b_rows, g.kp, g.ldb, BLOCK_K, uint32_t(block_n), NK_F32);
+  if (rc) return rc;
+  Tf32Params p;
+  p.M = g.M, p.N = g.N, p.ldc = g.ldc, p.C = g.C, p.bias = g.bias, p.alpha = g.alpha, p.beta = g.beta;
+  p.bias_bf16 = g.bias_dtype == NK_BF16, p.relu = g.relu, p.row_bias = g.row_bias;
+  p.num_m_blocks = int(m_blocks);
+  p.num_n_blocks = 0;
+  p.num_k_blocks = int((g.k_len + BLOCK_K - 1) / BLOCK_K);
+  p.k_blocks_total = int((g.kp + BLOCK_K - 1) / BLOCK_K);
+  p.batch = int(g.batch), p.a_bstride = int(g.a_bstride), p.b_bstride = int(g.b_bstride), p.k_bstride = int(g.k_bstride);
+  p.c_bstride = g.c_bstride;
+  const bool cb = g.c_dtype == NK_BF16;
+#define NK_TF32(BN, SPLIT) (cb ? launch_tf32<BN, __nv_bfloat16, SPLIT>(ctx, ta, tb, p) : launch_tf32<BN, float, SPLIT>(ctx, ta, tb, p))
+  if (g.x3)
+    rc = block_n == 128 ? NK_TF32(128, true) : NK_TF32(64, true);
+  else
+    rc = block_n == 256 ? NK_TF32(256, false) : block_n == 128 ? NK_TF32(128, false) : NK_TF32(64, false);
+#undef NK_TF32
+  return rc;
+}
 
 int nk_gemm_tf32(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
                  int64_t lda, const void* B, int64_t ldb, float beta, void* C, int64_t ldc, int c_dtype, const void* bias,
@@ -304,8 +355,7 @@ int nk_gemm_tf32(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int6
   NK_REQUIRE(ctx, (M + 31) / 32 < (int64_t(1) << 31) && (N + 31) / 32 < (int64_t(1) << 31) && (K + 31) / 32 <= 65535 &&
                   (M + BLOCK_M - 1) / BLOCK_M * ((N + 63) / 64) < (int64_t(1) << 31),
              "nk_gemm (tf32): shape too large (M=%lld N=%lld K=%lld)", (long long)M, (long long)N, (long long)K);
-  // tile width: the widest that does not leave most of a tile empty (3xTF32: at most 128, see kSplitAcc)
-  const int block_n = N <= 64 ? 64 : (N <= 128 || x3) ? 128 : 256;
+  const int block_n = nk_tf32_block_n(N, x3);
 
   void* pa = nullptr;
   void* pb = nullptr;
@@ -317,18 +367,9 @@ int nk_gemm_tf32(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int6
     return rc;
   }
   // A' = [A_hi | A_hi | A_lo], B' = [B_hi | B_lo | B_hi]
-  rc = pack(ctx, static_cast<const float*>(A), lda, transA != 0, M, K, static_cast<float*>(pa), ldp, segments, 2);
-  if (!rc) rc = pack(ctx, static_cast<const float*>(B), ldb, transB == 0, N, K, static_cast<float*>(pb), ldp, segments, 1);
-  CUtensorMap ta, tb;
-  if (!rc) rc = make_tmap_2d(ctx, &ta, pa, M, kp, ldp, BLOCK_K, BLOCK_M, NK_F32);
-  if (!rc) rc = make_tmap_2d(ctx, &tb, pb, N, kp, ldp, BLOCK_K, uint32_t(block_n), NK_F32);
+  rc = nk_tf32_pack(ctx, static_cast<const float*>(A), lda, transA != 0, M, K, static_cast<float*>(pa), ldp, segments, 2);
+  if (!rc) rc = nk_tf32_pack(ctx, static_cast<const float*>(B), ldb, transB == 0, N, K, static_cast<float*>(pb), ldp, segments, 1);
   if (!rc) {
-    Tf32Params p;
-    p.M = M, p.N = N, p.ldc = ldc, p.C = C, p.bias = bias, p.alpha = alpha, p.beta = beta;
-    p.bias_bf16 = bias_dtype == NK_BF16, p.relu = relu;
-    p.num_m_blocks = int((M + BLOCK_M - 1) / BLOCK_M);
-    p.num_n_blocks = 0;
-    p.num_k_blocks = int((kp + BLOCK_K - 1) / BLOCK_K);
     static const char* names[2][2][2][3] = {
         {{{"tf32_nn_128x256", "tf32_nn_128x128", "tf32_nn_128x64"}, {"tf32_nt_128x256", "tf32_nt_128x128", "tf32_nt_128x64"}},
          {{"tf32_tn_128x256", "tf32_tn_128x128", "tf32_tn_128x64"}, {"tf32_tt_128x256", "tf32_tt_128x128", "tf32_tt_128x64"}}},
@@ -337,13 +378,14 @@ int nk_gemm_tf32(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int6
          {{"tf32x3_tn_128x256", "tf32x3_tn_128x128", "tf32x3_tn_128x64"},
           {"tf32x3_tt_128x256", "tf32x3_tt_128x128", "tf32x3_tt_128x64"}}}};
     ctx->last_gemm_kernel = names[x3][transA != 0][transB != 0][block_n == 256 ? 0 : block_n == 128 ? 1 : 2];
-    const bool cb = c_dtype == NK_BF16;
-#define NK_TF32(BN, SPLIT) (cb ? launch_tf32<BN, __nv_bfloat16, SPLIT>(ctx, ta, tb, p) : launch_tf32<BN, float, SPLIT>(ctx, ta, tb, p))
-    if (x3)
-      rc = block_n == 128 ? NK_TF32(128, true) : NK_TF32(64, true);
-    else
-      rc = block_n == 256 ? NK_TF32(256, false) : block_n == 128 ? NK_TF32(128, false) : NK_TF32(64, false);
-#undef NK_TF32
+    NkTf32Gemm g;
+    g.x3 = x3, g.M = M, g.N = N;
+    g.A = static_cast<const float*>(pa), g.lda = ldp, g.a_rows = M;
+    g.B = static_cast<const float*>(pb), g.ldb = ldp, g.b_rows = N;
+    g.kp = kp, g.k_len = kp;
+    g.C = C, g.ldc = ldc, g.c_dtype = c_dtype, g.alpha = alpha, g.beta = beta;
+    g.bias = bias, g.bias_dtype = bias_dtype, g.relu = relu;
+    rc = nk_gemm_tf32_packed(ctx, g);
   }
   nk_free(ctx, pa);
   nk_free(ctx, pb);

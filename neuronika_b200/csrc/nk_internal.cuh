@@ -36,6 +36,7 @@ struct nk_ctx {
   int gemm_engine = NK_GEMM_AUTO;
   int f32_gemm = NK_F32_GEMM_IEEE;   // nk_gemm_f32_config: how f32 products use the tensor cores
   int conv_engine = NK_CONV_AUTO;
+  int f32_conv = NK_F32_GEMM_IEEE;   // nk_conv_f32_config: how f32 convolutions use the tensor cores
   const char* last_gemm_kernel = "none";
   const char* last_conv_kernel = "none";
   void* encode_tiled = nullptr;  // cuTensorMapEncodeTiled, fetched through the runtime
@@ -178,5 +179,21 @@ int make_tmap_2d(nk_ctx* ctx, CUtensorMap* tm, const void* base, int64_t rows, i
 int nk_gemm_tf32(nk_ctx* ctx, int transA, int transB, int64_t M, int64_t N, int64_t K, float alpha, const void* A,
                  int64_t lda, const void* B, int64_t ldb, float beta, void* C, int64_t ldc, int c_dtype, const void* bias,
                  int bias_dtype, int relu);
+// f32 convolution on the tensor cores (nk_conv_tf32.cu): every f32, groups = 1 call with a non-empty batch once
+// nk_conv_f32_config has set TF32 or TF32X3, unless nk_conv_config(DIRECT).  Arguments checked by the caller; the
+// convolution of x padded by `pad` (nk_pad_mode `mode`, fill `value`) with nsp sample dims; `nd` picks the kernel names
+// of the 1-D / 3-D entry points ("tf32_im2col_nd_*") over the 2-D ones ("tf32_im2col_*").
+static inline bool nk_conv_tf32_on(const nk_ctx* ctx, int dtype, int64_t groups) {
+  return dtype == NK_F32 && groups == 1 && ctx->f32_conv != NK_F32_GEMM_IEEE && ctx->conv_engine != NK_CONV_DIRECT;
+}
+int nk_conv_tf32_fwd(nk_ctx* ctx, void* y, const void* x, const void* w, const void* bias, int relu, int nsp, int64_t n,
+                     int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s, const int64_t* dil,
+                     const int64_t* pad, int mode, float value, bool nd);
+int nk_conv_tf32_bwd_input(nk_ctx* ctx, void* dx, const void* g, const void* w, int nsp, int64_t n, int64_t cin,
+                           const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s, const int64_t* dil,
+                           const int64_t* pad, int mode, float beta, bool nd);
+int nk_conv_tf32_bwd_kernel(nk_ctx* ctx, void* dwt, int dw_dtype, const void* g, const void* x, int nsp, int64_t n,
+                            int64_t cin, const int64_t* in_sp, int64_t cout, const int64_t* k, const int64_t* s,
+                            const int64_t* dil, const int64_t* pad, int mode, float value, float beta, bool nd);
 bool nk_gemm_wgmma_supported(int transA, int transB, int64_t M, int64_t N, int64_t K,
                              const void* A, int64_t lda, const void* B, int64_t ldb);

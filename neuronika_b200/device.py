@@ -72,6 +72,17 @@ class Device:
             raise ValueError(f"f32_matmul: mode must be one of {sorted(self.F32_MATMUL_MODES)}, got {mode!r}")
         L.check(L.lib.nk_gemm_f32_config(self.ctx, self.F32_MATMUL_MODES[mode]), self.ctx)
 
+    def f32_conv(self, mode: str) -> None:
+        """How f32 convolutions use the tensor cores (off by default, like torch's cudnn.allow_tf32), separately from
+        f32_matmul: "ieee": the CUDA-core kernels in full f32; "tf32" / "tf32x3": im2col + the TF32 / 3xTF32 wgmma GEMM
+        (operands rounded as f32_matmul describes) for every f32, groups = 1 convolution -- Var.convolution in 1-D,
+        2-D and 3-D and the Conv1d / Conv2d / Conv3d layers, forward and backward.  Grouped convolutions stay on the
+        CUDA cores, and conv_engine("direct") keeps every convolution there.  The mode is read when a convolution is
+        launched: a captured step replays with the mode it was captured with."""
+        if mode not in self.F32_MATMUL_MODES:
+            raise ValueError(f"f32_conv: mode must be one of {sorted(self.F32_MATMUL_MODES)}, got {mode!r}")
+        L.check(L.lib.nk_conv_f32_config(self.ctx, self.F32_MATMUL_MODES[mode]), self.ctx)
+
     def conv_engine(self, engine: str) -> None:
         """"auto": tensor-core kernels wherever they apply; "direct": CUDA-core kernels only"""
         L.check(L.lib.nk_conv_config(self.ctx, {"auto": 0, "direct": 1}[engine]), self.ctx)
