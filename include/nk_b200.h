@@ -282,6 +282,37 @@ int nk_padnd_fwd(nk_ctx* ctx, void* y, const void* x, int64_t planes, int nsp, c
 int nk_padnd_bwd(nk_ctx* ctx, void* dx, const void* g, int64_t planes, int nsp, const int64_t* in_sp,
                  const int64_t* pad, int dtype, float beta);
 
+/* ---- pooling over the last nsp (1..3) dims of (planes, s...), torch's semantics (csrc/nk_pool.cu) ----
+ * in_sp / out_sp / k / stride / pad / dilation are host arrays of nsp entries.  Per axis out_sp must be torch's extent
+ * floor((L + 2p - d(k-1) - 1)/s) + 1 or its ceil_mode value (the last window dropped when it would start in the right
+ * padding); k, s, d >= 1, 0 <= p <= k/2.  Anything else is NK_ERR_INVALID_ARG and launches nothing; more than 2^31 - 1
+ * elements in one plane is NK_ERR_UNSUPPORTED.  planes = 0 launches nothing.
+ * max: padded positions are never candidates; each window is scanned in row-major order from -inf, an element replacing
+ *   the maximum when it is greater or NaN (the first of equal maxima, the last NaN); idx (int32, may be NULL) gets the
+ *   in-plane flat index of the winner.  Bit exact.
+ * avg: the f32 sum of the in-bounds elements divided once by prod(e - a) (count_include_pad, a = o*s - p,
+ *   e = min(a + k, L + p)) or by the number of in-bounds elements; adaptive: window [floor(iL/O), ceil((i+1)L/O)) per
+ *   axis, divided by its element count.
+ * Backward: dx = beta*dx + sum, the sum gathered per input element in f32 and ascending output order (max: g[o] where
+ *   idx[o] is the element; averages: g[o] / divisor), the product and the add rounded separately; no atomics, so
+ *   repeated calls are bitwise equal.  dx and g are each f32 or bf16 (dx_dtype, g_dtype). */
+int nk_max_pool_nd_fwd(nk_ctx* ctx, void* y, int32_t* idx, const void* x, int64_t planes, int nsp, const int64_t* in_sp,
+                       const int64_t* out_sp, const int64_t* k, const int64_t* stride, const int64_t* pad,
+                       const int64_t* dilation, int dtype);
+int nk_max_pool_nd_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* g, int g_dtype, const int32_t* idx,
+                       int64_t planes, int nsp, const int64_t* in_sp, const int64_t* out_sp, const int64_t* k,
+                       const int64_t* stride, const int64_t* pad, const int64_t* dilation, float beta);
+int nk_avg_pool_nd_fwd(nk_ctx* ctx, void* y, const void* x, int64_t planes, int nsp, const int64_t* in_sp,
+                       const int64_t* out_sp, const int64_t* k, const int64_t* stride, const int64_t* pad,
+                       int count_include_pad, int dtype);
+int nk_avg_pool_nd_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* g, int g_dtype, int64_t planes, int nsp,
+                       const int64_t* in_sp, const int64_t* out_sp, const int64_t* k, const int64_t* stride,
+                       const int64_t* pad, int count_include_pad, float beta);
+int nk_adaptive_avg_pool_nd_fwd(nk_ctx* ctx, void* y, const void* x, int64_t planes, int nsp, const int64_t* in_sp,
+                                const int64_t* out_sp, int dtype);
+int nk_adaptive_avg_pool_nd_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* g, int g_dtype, int64_t planes,
+                                int nsp, const int64_t* in_sp, const int64_t* out_sp, float beta);
+
 /* ---- matrix-vector / vector-matrix / vector-vector products (8-f rank 3; csrc/nk_gemv.cu) ----
  * A is (rows, cols) row-major.  trans = 0: y[rows] = beta*y + A.x[cols] (MatrixVectorMul::forward,
  * matrix_vector_mul/mod.rs:32-40; vm dv, vector_matrix_mul/mod.rs:64-72); trans = 1: y[cols] = beta*y +

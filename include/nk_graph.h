@@ -108,6 +108,15 @@ int nkg_pow(nkg_var* a, int exp, nkg_var** out);
 int nkg_transpose(nkg_var* a, nkg_var** out);
 /* pad the nsp (1..3) sample dims of (N, C, ...) with an nk_pad_mode (pad/mod.rs:20-182) */
 int nkg_pad_mode(nkg_var* a, int nsp, const int64_t* padding, int mode, float value, nkg_var** out);
+/* Pooling of the nsp (1..3) sample dims of (N, C, ...), torch's semantics (nk_b200.h nk_*_pool_nd_*), one forward and
+ * one backward node each.  kernel / stride / padding / dilation / output_size: nsp entries; ceil_mode as in torch.  The
+ * max pool of a differentiable operand keeps the winners' int32 indices (numel(out) * 4 bytes, allocated when the node
+ * is built) for its backward.  Invalid arguments fail with NK_ERR_INVALID_ARG and record nothing. */
+int nkg_max_pool(nkg_var* a, int nsp, const int64_t* kernel, const int64_t* stride, const int64_t* padding,
+                 const int64_t* dilation, int ceil_mode, nkg_var** out);
+int nkg_avg_pool(nkg_var* a, int nsp, const int64_t* kernel, const int64_t* stride, const int64_t* padding,
+                 int ceil_mode, int count_include_pad, nkg_var** out);
+int nkg_adaptive_avg_pool(nkg_var* a, int nsp, const int64_t* output_size, nkg_var** out);
 int nkg_mv(nkg_var* matrix, nkg_var* vector, nkg_var** out);   /* matrix_vector_mul/mod.rs */
 int nkg_vm(nkg_var* vector, nkg_var* matrix, nkg_var** out);   /* vector_matrix_mul/mod.rs */
 int nkg_vv(nkg_var* a, nkg_var* b, nkg_var** out);             /* vector_vector_mul/mod.rs: 0-d result */

@@ -138,6 +138,12 @@ _PROTOS = {
     "nk_transpose": (i32, [vp, vp, i32, vp, i32, i32, pi64, f32]),
     "nk_padnd_fwd": (i32, [vp, vp, vp, i64, i32, pi64, pi64, i32, f32, i32]),
     "nk_padnd_bwd": (i32, [vp, vp, vp, i64, i32, pi64, pi64, i32, f32]),
+    "nk_max_pool_nd_fwd": (i32, [vp, vp, vp, vp, i64, i32, pi64, pi64, pi64, pi64, pi64, pi64, i32]),
+    "nk_max_pool_nd_bwd": (i32, [vp, vp, i32, vp, i32, vp, i64, i32, pi64, pi64, pi64, pi64, pi64, pi64, f32]),
+    "nk_avg_pool_nd_fwd": (i32, [vp, vp, vp, i64, i32, pi64, pi64, pi64, pi64, pi64, i32, i32]),
+    "nk_avg_pool_nd_bwd": (i32, [vp, vp, i32, vp, i32, i64, i32, pi64, pi64, pi64, pi64, pi64, i32, f32]),
+    "nk_adaptive_avg_pool_nd_fwd": (i32, [vp, vp, vp, i64, i32, pi64, pi64, i32]),
+    "nk_adaptive_avg_pool_nd_bwd": (i32, [vp, vp, i32, vp, i32, i64, i32, pi64, pi64, f32]),
     "nk_gemv": (i32, [vp, i32, i64, i64, vp, vp, f32, vp, i32, i32]),
     "nk_outer_acc": (i32, [vp, vp, i32, vp, vp, i64, i64, i32, f32]),
     "nk_dot": (i32, [vp, vp, vp, vp, sz, i32]),

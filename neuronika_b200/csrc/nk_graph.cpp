@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "nk_graph.h"
+#include "nk_pool.h"
 
 namespace nkg {
 
@@ -923,6 +924,67 @@ struct PadNdBackward : Backward {
     const void* g = gradient->get();
     accumulate(ctx, operand_grad, gradient->dtype, [&](void* d, float beta) {
       ck(ctx, nk_padnd_bwd(ctx, d, g, s[0] * s[1], nsp, s.data() + 2, pad, gradient->dtype, beta));
+    });
+    grad_written(operand_grad);
+  }
+};
+
+// ------------------------------------------------------------------------------- pooling (nk_pool.cu)
+// Max / average / adaptive average pooling of the nsp sample dims of (N, C, ...), torch's semantics.  The max pool's
+// int32 winner indices (idx, allocated when the node is built, only for a differentiable operand) carry the forward's
+// choice to the backward.
+enum PoolOp { kPoolMax, kPoolAvg, kPoolAdaptive };
+struct PoolArgs {
+  int op, nsp, include_pad;
+  int64_t k[3], s[3], p[3], d[3];
+};
+static int pool_fwd(nk_ctx* ctx, const PoolArgs& a, void* y, int32_t* idx, const void* x, const Shape& xs,
+                    const Shape& ys, int dtype) {
+  const int64_t planes = xs[0] * xs[1];
+  if (a.op == kPoolMax)
+    return nk_max_pool_nd_fwd(ctx, y, idx, x, planes, a.nsp, xs.data() + 2, ys.data() + 2, a.k, a.s, a.p, a.d, dtype);
+  if (a.op == kPoolAvg)
+    return nk_avg_pool_nd_fwd(ctx, y, x, planes, a.nsp, xs.data() + 2, ys.data() + 2, a.k, a.s, a.p, a.include_pad,
+                              dtype);
+  return nk_adaptive_avg_pool_nd_fwd(ctx, y, x, planes, a.nsp, xs.data() + 2, ys.data() + 2, dtype);
+}
+struct Pool : Forward {
+  TensorP operand, data, idx;
+  PoolArgs a;
+  Pool(nk_ctx* c, TensorP x, TensorP d, TensorP i, const PoolArgs& pa)
+      : Forward(c), operand(std::move(x)), data(std::move(d)), idx(std::move(i)), a(pa) {}
+  const char* name() const override {
+    return a.op == kPoolMax ? "MaxPool" : a.op == kPoolAvg ? "AvgPool" : "AdaptiveAvgPool";
+  }
+  void forward() override {
+    ck(ctx, pool_fwd(ctx, a, data->wptr(), idx ? (int32_t*)idx->wptr() : nullptr, operand->rptr(), operand->shape,
+                     data->shape, data->dtype));
+  }
+};
+struct PoolBackward : Backward {
+  GradientP operand_grad;
+  TensorP idx;
+  PoolArgs a;
+  PoolBackward(nk_ctx* c, GradientP g, GradientP xg, TensorP i, const PoolArgs& pa)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), idx(std::move(i)), a(pa) {}
+  const char* name() const override {
+    return a.op == kPoolMax ? "MaxPoolBackward" : a.op == kPoolAvg ? "AvgPoolBackward" : "AdaptiveAvgPoolBackward";
+  }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad}); }
+  void backward() override {
+    const Shape &xs = operand_grad->shape, &ys = gradient->shape;
+    const void* g = gradient->get();
+    const int64_t planes = xs[0] * xs[1];
+    accumulate(ctx, operand_grad, [&](void* d, float beta) {  // one launch for every (dx, g) dtype pair
+      const int dt = operand_grad->dtype, gt = gradient->dtype;
+      if (a.op == kPoolMax)
+        ck(ctx, nk_max_pool_nd_bwd(ctx, d, dt, g, gt, (const int32_t*)idx->rptr(), planes, a.nsp, xs.data() + 2,
+                                   ys.data() + 2, a.k, a.s, a.p, a.d, beta));
+      else if (a.op == kPoolAvg)
+        ck(ctx, nk_avg_pool_nd_bwd(ctx, d, dt, g, gt, planes, a.nsp, xs.data() + 2, ys.data() + 2, a.k, a.s, a.p,
+                                   a.include_pad, beta));
+      else
+        ck(ctx, nk_adaptive_avg_pool_nd_bwd(ctx, d, dt, g, gt, planes, a.nsp, xs.data() + 2, ys.data() + 2, beta));
     });
     grad_written(operand_grad);
   }
@@ -2329,6 +2391,68 @@ int nkg_pad_mode(nkg_var* a, int nsp, const int64_t* padding, int mode, float va
         [&](const TensorP& d) { return std::make_shared<PadNd>(a->ctx, a->data, d, nsp, pad, mode, value); },
         [&](const TensorP&, const GradientP& g) { return std::make_shared<PadNdBackward>(a->ctx, g, a->grad, nsp, pad); });
   });
+}
+
+// checks the operand and the per-axis arguments of a pooling op, then records it; nothing is recorded on an error
+static int pool_record(int op, nkg_var* a, int nsp, const int64_t* kernel, const int64_t* stride,
+                       const int64_t* padding, const int64_t* dilation, const int64_t* out_size, bool ceil_mode,
+                       bool include_pad, nkg_var** out) {
+  static const char* const who[] = {"max_pool", "avg_pool", "adaptive_avg_pool"};
+  const char* name = who[op];
+  return guard([&] {
+    not_null({a, out}, name);
+    if (op == kPoolAdaptive)
+      not_null({out_size}, name);
+    else
+      not_null({kernel, stride, padding, op == kPoolMax ? dilation : kernel}, name);
+    const Shape& s = a->data->shape;
+    if (nsp < 1 || nsp > 3 || (int)s.size() != nsp + 2)
+      fail(NK_ERR_INVALID_ARG, "%s: expects a (N, C, ...) operand with %d sample dimensions (1 to 3), got %d dimensions",
+           name, nsp, (int)s.size());
+    PoolArgs pa{op, nsp, include_pad, {1, 1, 1}, {1, 1, 1}, {0, 0, 0}, {1, 1, 1}};
+    Shape os = s;
+    for (int i = 0; i < nsp; ++i) {
+      const int64_t L = s[2 + i];
+      if (op == kPoolAdaptive) {
+        if (out_size[i] < 1 || L < 1)
+          fail(NK_ERR_INVALID_ARG, "%s: input and output sizes must be >= 1 (axis %d: %lld, %lld)", name, i,
+               (long long)L, (long long)out_size[i]);
+        os[2 + i] = out_size[i];
+        continue;
+      }
+      pa.k[i] = kernel[i], pa.s[i] = stride[i], pa.p[i] = padding[i], pa.d[i] = op == kPoolMax ? dilation[i] : 1;
+      char msg[160];
+      if (nk_pool_check_axis(name, i, L, pa.k[i], pa.s[i], pa.p[i], pa.d[i], msg, sizeof msg))
+        fail(NK_ERR_INVALID_ARG, "%s", msg);
+      os[2 + i] = nk_pool_out_extent(L, pa.k[i], pa.s[i], pa.p[i], pa.d[i], ceil_mode);
+      if (os[2 + i] < 1)
+        fail(NK_ERR_INVALID_ARG, "%s: output size would be %lld (axis %d, input %lld)", name, (long long)os[2 + i], i,
+             (long long)L);
+    }
+    TensorP idx;
+    if (op == kPoolMax && a->diff()) {
+      idx = std::make_shared<Tensor>(a->ctx, os, NK_F32);  // int32 words
+      idx->wptr();
+    }
+    *out = record(
+        {a}, os, a->data->dtype, [&](const TensorP& d) { return std::make_shared<Pool>(a->ctx, a->data, d, idx, pa); },
+        [&](const TensorP&, const GradientP& g) { return std::make_shared<PoolBackward>(a->ctx, g, a->grad, idx, pa); });
+  });
+}
+
+int nkg_max_pool(nkg_var* a, int nsp, const int64_t* kernel, const int64_t* stride, const int64_t* padding,
+                 const int64_t* dilation, int ceil_mode, nkg_var** out) {
+  return pool_record(kPoolMax, a, nsp, kernel, stride, padding, dilation, nullptr, ceil_mode != 0, true, out);
+}
+
+int nkg_avg_pool(nkg_var* a, int nsp, const int64_t* kernel, const int64_t* stride, const int64_t* padding,
+                 int ceil_mode, int count_include_pad, nkg_var** out) {
+  return pool_record(kPoolAvg, a, nsp, kernel, stride, padding, nullptr, nullptr, ceil_mode != 0,
+                     count_include_pad != 0, out);
+}
+
+int nkg_adaptive_avg_pool(nkg_var* a, int nsp, const int64_t* output_size, nkg_var** out) {
+  return pool_record(kPoolAdaptive, a, nsp, nullptr, nullptr, nullptr, nullptr, output_size, false, false, out);
 }
 
 static int matvec_impl(nkg_var* mat, nkg_var* vec, bool vm, nkg_var** out) {

@@ -1,5 +1,6 @@
 """Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell, Conv1d, Conv2d and Conv3d (neuronika-nn/src/lib.rs:
-406-916), and the sequence layers LSTM and GRU over them (stacked and bidirectional like torch.nn.LSTM / GRU)."""
+406-916), the sequence layers LSTM and GRU over them (stacked and bidirectional like torch.nn.LSTM / GRU), and torch's
+max, average and adaptive average pooling layers."""
 from __future__ import annotations
 
 import math
@@ -300,6 +301,94 @@ class Dropout:
 
     def parameters(self):
         return []
+
+
+class _Pool:
+    """The pooling layers: no parameters; `forward` is one graph node (Var.max_pool / avg_pool / adaptive_avg_pool)
+    over an input with `nsp` sample dimensions after (N, C)."""
+
+    nsp = 0
+
+    def _check(self, input: V.Var) -> None:
+        if len(input.shape) != self.nsp + 2:
+            raise ValueError(f"{type(self).__name__} expects a {self.nsp + 2}-d (N, C, ...) input, got shape {input.shape}")
+
+    def parameters(self):
+        return []
+
+
+class _MaxPoolNd(_Pool):
+    def __init__(self, kernel_size, stride=None, padding=0, dilation=1, ceil_mode: bool = False):
+        self.kernel_size, self.stride, self.padding = kernel_size, stride, padding
+        self.dilation, self.ceil_mode = dilation, bool(ceil_mode)
+
+    def forward(self, input: V.Var) -> V.Var:
+        self._check(input)
+        return input.max_pool(self.kernel_size, self.stride, self.padding, self.dilation, self.ceil_mode)
+
+
+class _AvgPoolNd(_Pool):
+    def __init__(self, kernel_size, stride=None, padding=0, ceil_mode: bool = False, count_include_pad: bool = True):
+        self.kernel_size, self.stride, self.padding = kernel_size, stride, padding
+        self.ceil_mode, self.count_include_pad = bool(ceil_mode), bool(count_include_pad)
+
+    def forward(self, input: V.Var) -> V.Var:
+        self._check(input)
+        return input.avg_pool(self.kernel_size, self.stride, self.padding, self.ceil_mode, self.count_include_pad)
+
+
+class _AdaptiveAvgPoolNd(_Pool):
+    def __init__(self, output_size):
+        self.output_size = output_size
+
+    def forward(self, input: V.Var) -> V.Var:
+        self._check(input)
+        return input.adaptive_avg_pool(self.output_size)
+
+
+class MaxPool1d(_MaxPoolNd):
+    """torch.nn.MaxPool1d over (N, C, L)."""
+    nsp = 1
+
+
+class MaxPool2d(_MaxPoolNd):
+    """torch.nn.MaxPool2d over (N, C, H, W)."""
+    nsp = 2
+
+
+class MaxPool3d(_MaxPoolNd):
+    """torch.nn.MaxPool3d over (N, C, D, H, W)."""
+    nsp = 3
+
+
+class AvgPool1d(_AvgPoolNd):
+    """torch.nn.AvgPool1d over (N, C, L)."""
+    nsp = 1
+
+
+class AvgPool2d(_AvgPoolNd):
+    """torch.nn.AvgPool2d over (N, C, H, W)."""
+    nsp = 2
+
+
+class AvgPool3d(_AvgPoolNd):
+    """torch.nn.AvgPool3d over (N, C, D, H, W)."""
+    nsp = 3
+
+
+class AdaptiveAvgPool1d(_AdaptiveAvgPoolNd):
+    """torch.nn.AdaptiveAvgPool1d over (N, C, L)."""
+    nsp = 1
+
+
+class AdaptiveAvgPool2d(_AdaptiveAvgPoolNd):
+    """torch.nn.AdaptiveAvgPool2d over (N, C, H, W); AdaptiveAvgPool2d(1) is global average pooling."""
+    nsp = 2
+
+
+class AdaptiveAvgPool3d(_AdaptiveAvgPoolNd):
+    """torch.nn.AdaptiveAvgPool3d over (N, C, D, H, W)."""
+    nsp = 3
 
 
 class GRUCell:

@@ -334,6 +334,94 @@ def pad_nd_bwd(dx: CuArray, g: CuArray, padding, beta=1.0) -> CuArray:
     return dx
 
 
+# ---------------------------------------------------------------- pooling over 1..3 sample dims (csrc/nk_pool.cu)
+def pool_out_extent(length, k, stride, pad, dilation=1, ceil_mode=False) -> int:
+    """torch's pooling output extent along one axis (the value nk_*_pool_nd_* check out_sp against)."""
+    if stride < 1:
+        return 0                            # nk_*_pool_nd_* reject the stride
+    num = length + 2 * pad - dilation * (k - 1) - 1
+    o = (num + (stride - 1 if ceil_mode else 0)) // stride + 1
+    if ceil_mode and (o - 1) * stride >= length + pad:
+        o -= 1
+    return o
+
+
+def _pool_geom(x_shape, out_sp, *per_axis):
+    nsp = len(out_sp)
+    planes = int(np.prod(x_shape[:len(x_shape) - nsp]))
+    return [planes, nsp, L.shape_arr(x_shape[len(x_shape) - nsp:]), L.shape_arr(out_sp)] + [L.shape_arr(a) for a in per_axis]
+
+
+def _pool_out(x: CuArray, k, stride, padding, dilation, ceil_mode):
+    sp = x.shape[x.ndim - len(k):]
+    return tuple(pool_out_extent(*a, ceil_mode) for a in zip(sp, k, stride, padding, dilation))
+
+
+def max_pool_nd(x: CuArray, k, stride=None, padding=None, dilation=None, ceil_mode=False, out=None,
+                idx: CuArray | None = None, out_sp=None) -> CuArray:
+    """y = max pool of the last len(k) dims of x (nk_max_pool_nd_fwd); idx (int32 as F32-sized elements, y's shape) gets
+    the winners' in-plane flat indices when given."""
+    nsp = len(k)
+    stride, padding, dilation = stride or k, padding or (0,) * nsp, dilation or (1,) * nsp
+    out_sp = out_sp or _pool_out(x, k, stride, padding, dilation, ceil_mode)
+    out = out or CuArray(x.device, x.shape[:x.ndim - nsp] + tuple(out_sp), x.dtype)
+    _ck(lib.nk_max_pool_nd_fwd(x.device.ctx, out.ptr, _ptr(idx), x.ptr,
+                               *_pool_geom(x.shape, out_sp, k, stride, padding, dilation), x.dtype), x.device)
+    return out
+
+
+def max_pool_nd_bwd(dx: CuArray, g: CuArray, idx: CuArray, k, stride=None, padding=None, dilation=None,
+                    beta=1.0) -> CuArray:
+    """dx = beta*dx + the gradient gathered through the saved indices (nk_max_pool_nd_bwd)."""
+    nsp = len(k)
+    stride, padding, dilation = stride or k, padding or (0,) * nsp, dilation or (1,) * nsp
+    _ck(lib.nk_max_pool_nd_bwd(dx.device.ctx, dx.ptr, dx.dtype, g.ptr, g.dtype, idx.ptr,
+                               *_pool_geom(dx.shape, g.shape[g.ndim - nsp:], k, stride, padding, dilation),
+                               float(beta)), dx.device)
+    return dx
+
+
+def avg_pool_nd(x: CuArray, k, stride=None, padding=None, ceil_mode=False, count_include_pad=True, out=None,
+                out_sp=None) -> CuArray:
+    """y = average pool of the last len(k) dims of x (nk_avg_pool_nd_fwd)."""
+    nsp = len(k)
+    stride, padding = stride or k, padding or (0,) * nsp
+    out_sp = out_sp or _pool_out(x, k, stride, padding, (1,) * nsp, ceil_mode)
+    out = out or CuArray(x.device, x.shape[:x.ndim - nsp] + tuple(out_sp), x.dtype)
+    _ck(lib.nk_avg_pool_nd_fwd(x.device.ctx, out.ptr, x.ptr, *_pool_geom(x.shape, out_sp, k, stride, padding),
+                               int(bool(count_include_pad)), x.dtype), x.device)
+    return out
+
+
+def avg_pool_nd_bwd(dx: CuArray, g: CuArray, k, stride=None, padding=None, count_include_pad=True,
+                    beta=1.0) -> CuArray:
+    """dx = beta*dx + the average pool's input gradient (nk_avg_pool_nd_bwd)."""
+    nsp = len(k)
+    stride, padding = stride or k, padding or (0,) * nsp
+    _ck(lib.nk_avg_pool_nd_bwd(dx.device.ctx, dx.ptr, dx.dtype, g.ptr, g.dtype,
+                               *_pool_geom(dx.shape, g.shape[g.ndim - nsp:], k, stride, padding),
+                               int(bool(count_include_pad)), float(beta)), dx.device)
+    return dx
+
+
+def adaptive_avg_pool_nd(x: CuArray, output_size, out=None) -> CuArray:
+    """y = adaptive average pool of the last len(output_size) dims of x to output_size (nk_adaptive_avg_pool_nd_fwd)."""
+    nsp = len(output_size)
+    out = out or CuArray(x.device, x.shape[:x.ndim - nsp] + tuple(output_size), x.dtype)
+    _ck(lib.nk_adaptive_avg_pool_nd_fwd(x.device.ctx, out.ptr, x.ptr, *_pool_geom(x.shape, output_size), x.dtype),
+        x.device)
+    return out
+
+
+def adaptive_avg_pool_nd_bwd(dx: CuArray, g: CuArray, beta=1.0, nsp=None) -> CuArray:
+    """dx = beta*dx + the adaptive average pool's input gradient (nk_adaptive_avg_pool_nd_bwd); nsp defaults to
+    dx.ndim - 2."""
+    nsp = nsp or dx.ndim - 2
+    _ck(lib.nk_adaptive_avg_pool_nd_bwd(dx.device.ctx, dx.ptr, dx.dtype, g.ptr, g.dtype,
+                                        *_pool_geom(dx.shape, g.shape[g.ndim - nsp:]), float(beta)), dx.device)
+    return dx
+
+
 # ---------------------------------------------------------------- 8-f: mv / vm / vv
 def gemv(a: CuArray, x: CuArray, y: CuArray | None = None, trans=False, beta=0.0) -> CuArray:
     rows, cols = a.shape

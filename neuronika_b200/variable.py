@@ -102,6 +102,9 @@ _G = {
     "nkg_status_get": (i32, [vp]),
     "nkg_status_release": (i32, [vp]),
     "nkg_dropout": (i32, [vp, C.c_double, vp, pvp]),
+    "nkg_max_pool": (i32, [vp, i32, pi64, pi64, pi64, pi64, i32, pvp]),
+    "nkg_avg_pool": (i32, [vp, i32, pi64, pi64, pi64, i32, i32, pvp]),
+    "nkg_adaptive_avg_pool": (i32, [vp, i32, pi64, pvp]),
 }
 for _n, (_r, _a) in _G.items():
     _f = getattr(lib, _n)
@@ -289,6 +292,36 @@ class Var:
         return self._unary(lib.nkg_dropout, float(p), (status or Status())._h)
 
     def flatten(self): return self._unary(lib.nkg_flatten)
+
+    def _nsp_tuple(self, v, name):
+        nsp = len(self.shape) - 2
+        t = (int(v),) * nsp if np.isscalar(v) else tuple(int(x) for x in v)
+        if len(t) != nsp or not 1 <= nsp <= 3:
+            raise L.NkError(-1, f"Invalid {name} {list(t)} for a pool over {nsp} sample dimensions.")
+        return t
+
+    def max_pool(self, kernel_size, stride=None, padding=0, dilation=1, ceil_mode: bool = False):
+        """torch's max_pool{1,2,3}d over the sample dims of a (N, C, ...) operand, as one node; ints broadcast to every
+        sample dim and stride defaults to kernel_size.  The backward sends each output's gradient to its window's first
+        maximum (the last NaN), through int32 indices the node keeps when the operand is differentiable."""
+        k = self._nsp_tuple(kernel_size, "kernel_size")
+        s = self._nsp_tuple(kernel_size if stride is None else stride, "stride")
+        p, d = self._nsp_tuple(padding, "padding"), self._nsp_tuple(dilation, "dilation")
+        return self._unary(lib.nkg_max_pool, len(k), *(L.shape_arr(t) for t in (k, s, p, d)), int(bool(ceil_mode)))
+
+    def avg_pool(self, kernel_size, stride=None, padding=0, ceil_mode: bool = False, count_include_pad: bool = True):
+        """torch's avg_pool{1,2,3}d over the sample dims of a (N, C, ...) operand, as one node."""
+        k = self._nsp_tuple(kernel_size, "kernel_size")
+        s = self._nsp_tuple(kernel_size if stride is None else stride, "stride")
+        p = self._nsp_tuple(padding, "padding")
+        return self._unary(lib.nkg_avg_pool, len(k), *(L.shape_arr(t) for t in (k, s, p)), int(bool(ceil_mode)),
+                           int(bool(count_include_pad)))
+
+    def adaptive_avg_pool(self, output_size):
+        """torch's adaptive_avg_pool{1,2,3}d over the sample dims of a (N, C, ...) operand, as one node: window i of an
+        axis is [floor(i*L/O), ceil((i+1)*L/O))."""
+        o = self._nsp_tuple(output_size, "output_size")
+        return self._unary(lib.nkg_adaptive_avg_pool, len(o), L.shape_arr(o))
 
     def pad(self, padding, value: float = 0.0, mode: str = "constant"):
         """`pad(padding, mode)` (var.rs:726-737): Zero / Constant(value) / Reflective / Replicative over the 1..3
