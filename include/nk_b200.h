@@ -313,6 +313,37 @@ int nk_adaptive_avg_pool_nd_fwd(nk_ctx* ctx, void* y, const void* x, int64_t pla
 int nk_adaptive_avg_pool_nd_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* g, int g_dtype, int64_t planes,
                                 int nsp, const int64_t* in_sp, const int64_t* out_sp, float beta);
 
+/* ---- batch norm over (N, C, S) and layer norm over (rows, cols), torch's semantics (csrc/nk_norm.cu) ----
+ * x / y are f32 or bf16 (dtype); w and b (may be NULL: 1 and 0) have x's dtype; every statistic is f32.
+ * Batch norm, S = product of the sample dims (1 for (N, C)), M = N*S per channel:
+ *   batch statistics when training or running_mean is NULL: y = (x - mean) * rstd * w + b, mean and the biased var of
+ *   the channel, rstd = 1/sqrt(var + eps), saved to save_mean / save_rstd (C floats each); when training with running
+ *   stats, rm = (1 - momentum) rm + momentum mean, rv = (1 - momentum) rv + momentum var M/(M - 1).  Otherwise the
+ *   running statistics normalize, and save_mean = rm, save_rstd = 1/sqrt(rv + eps).  M = 1 with batch statistics is
+ *   NK_ERR_INVALID_ARG (torch's message); N = 0 launches nothing.  Training: 3 launches (partial statistics, per-channel
+ *   finalize, apply); running statistics: 1.
+ *   Backward with the saved statistics, xhat = (x - save_mean) * save_rstd: db = sum g, dw = sum g*xhat per channel;
+ *   dx = w*rstd/M * (M g - sum g - xhat sum g*xhat) when batch_stats, else g*w*rstd.  Each of dx / dw / db may be NULL
+ *   (not computed), has its own dtype and is accumulated as d = beta*d + value.  Launches: partial sums and finalize
+ *   when dw, db or a batch-statistics dx is wanted, then dx.
+ * Layer norm: each of `rows` rows of `cols` elements is normalized by its own mean and biased variance, then w and b
+ *   (cols elements) apply elementwise; save_mean / save_rstd hold `rows` floats.  One launch.  Backward, g' = g*w:
+ *   dx = rstd/D * (D g' - sum g' - xhat sum g'*xhat) over the row (D = cols), dw / db = the column sums of g*xhat / g;
+ *   at most 2 launches (column partials, then dx and the column finalize).
+ * Every reduction runs in a fixed order without atomics: repeated calls give identical bits for every output. */
+int nk_batch_norm_fwd(nk_ctx* ctx, void* y, const void* x, int dtype, int64_t n, int64_t c, int64_t s, const void* w,
+                      const void* b, float* running_mean, float* running_var, float* save_mean, float* save_rstd,
+                      int training, float momentum, float eps);
+int nk_batch_norm_bwd(nk_ctx* ctx, void* dx, int dx_dtype, float dx_beta, void* dw, int dw_dtype, float dw_beta,
+                      void* db, int db_dtype, float db_beta, const void* g, int g_dtype, const void* x, int dtype,
+                      int64_t n, int64_t c, int64_t s, const void* w, const float* save_mean, const float* save_rstd,
+                      int batch_stats);
+int nk_layer_norm_fwd(nk_ctx* ctx, void* y, const void* x, int dtype, int64_t rows, int64_t cols, const void* w,
+                      const void* b, float* save_mean, float* save_rstd, float eps);
+int nk_layer_norm_bwd(nk_ctx* ctx, void* dx, int dx_dtype, float dx_beta, void* dw, int dw_dtype, float dw_beta,
+                      void* db, int db_dtype, float db_beta, const void* g, int g_dtype, const void* x, int dtype,
+                      int64_t rows, int64_t cols, const void* w, const float* save_mean, const float* save_rstd);
+
 /* ---- matrix-vector / vector-matrix / vector-vector products (8-f rank 3; csrc/nk_gemv.cu) ----
  * A is (rows, cols) row-major.  trans = 0: y[rows] = beta*y + A.x[cols] (MatrixVectorMul::forward,
  * matrix_vector_mul/mod.rs:32-40; vm dv, vector_matrix_mul/mod.rs:64-72); trans = 1: y[cols] = beta*y +

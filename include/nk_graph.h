@@ -205,6 +205,17 @@ int nkg_status_set(nkg_status* status, int train);
 int nkg_status_get(nkg_status* status);   /* 1 train, 0 eval */
 int nkg_status_release(nkg_status* status);
 int nkg_dropout(nkg_var* a, double p, nkg_status* status, nkg_var** out);
+/* Batch norm of an (N, C, ...) operand over N and the sample dims, torch's semantics (nk_b200.h nk_batch_norm_*), one
+ * node.  weight / bias: (C,) of the operand's dtype, or NULL; running_mean / running_var: non-differentiable f32 (C,)
+ * leaves updated in place by every training forward, or both NULL (batch statistics in both modes).  `status` is read
+ * on each forward() (train: batch statistics); the backward follows what the last forward did.  The node's (C,) f32
+ * saved statistics are allocated when it is built.  Invalid arguments fail with NK_ERR_INVALID_ARG and record
+ * nothing, batch statistics of one value per channel with torch's message. */
+int nkg_batch_norm(nkg_var* x, nkg_var* weight, nkg_var* bias, nkg_var* running_mean, nkg_var* running_var,
+                   nkg_status* status, float momentum, float eps, nkg_var** out);
+/* Layer norm over the last k dims of the operand (torch's normalized_shape = those dims), one node; weight / bias have
+ * that shape and the operand's dtype, or are NULL. */
+int nkg_layer_norm(nkg_var* x, int k, nkg_var* weight, nkg_var* bias, float eps, nkg_var** out);
 
 /* ---- gradient-ready hook (data parallel overlap): `cb(user, begin, end)` is called from inside nkg_backward(), on
  * the calling thread, right after the LAST kernel that accumulates into elements [begin, end) of this leaf's gradient

@@ -990,6 +990,125 @@ struct PoolBackward : Backward {
   }
 };
 
+// ------------------------------------------------------------------------------- batch norm / layer norm (nk_norm.cu)
+// Which statistics the last BatchNorm forward normalized with; its backward applies exactly that, whatever the status
+// says by then (as DropoutState).
+struct BatchNormState {
+  bool batch = true;
+};
+// (N, C, S) view of a batch-norm operand: S = product of the sample dims
+static void bn_dims(const Shape& s, int64_t& n, int64_t& c, int64_t& sp) {
+  n = s[0], c = s[1], sp = 1;
+  for (size_t i = 2; i < s.size(); ++i) sp *= s[i];
+}
+static void* opt_r(const TensorP& t) { return t ? t->rptr() : nullptr; }
+
+// the size as torch prints it in its messages: torch.Size([2, 3])
+static std::string torch_size(const Shape& s) {
+  std::string out = "torch.Size([";
+  for (size_t i = 0; i < s.size(); ++i) out += (i ? ", " : "") + std::to_string(s[i]);
+  return out + "])";
+}
+// batch statistics need two values per channel (torch's _verify_batch_size): checked when the node is built and again
+// on every forward, since the status may have turned to training in between
+static void bn_check_batch(const Shape& s, bool batch) {
+  int64_t n, c, sp;
+  bn_dims(s, n, c, sp);
+  if (batch && n * sp == 1)
+    fail(NK_ERR_INVALID_ARG, "Expected more than 1 value per channel when training, got input size %s",
+         torch_size(s).c_str());
+}
+
+struct BatchNorm : Forward {
+  TensorP operand, weight, bias, running_mean, running_var, data, save_mean, save_rstd;
+  std::shared_ptr<bool> train;
+  std::shared_ptr<BatchNormState> state;
+  float momentum, eps;
+  BatchNorm(nk_ctx* c, TensorP x, TensorP w, TensorP b, TensorP rm, TensorP rv, TensorP d, TensorP sm, TensorP sr,
+            std::shared_ptr<bool> st, std::shared_ptr<BatchNormState> s, float mom, float e)
+      : Forward(c), operand(std::move(x)), weight(std::move(w)), bias(std::move(b)), running_mean(std::move(rm)),
+        running_var(std::move(rv)), data(std::move(d)), save_mean(std::move(sm)), save_rstd(std::move(sr)),
+        train(std::move(st)), state(std::move(s)), momentum(mom), eps(e) {}
+  const char* name() const override { return "BatchNorm"; }
+  void forward() override {
+    bn_check_batch(operand->shape, *train || !running_mean);
+    int64_t n, c, sp;
+    bn_dims(operand->shape, n, c, sp);
+    ck(ctx, nk_batch_norm_fwd(ctx, data->wptr(), operand->rptr(), data->dtype, n, c, sp, opt_r(weight), opt_r(bias),
+                              (float*)opt_r(running_mean), (float*)opt_r(running_var), (float*)save_mean->wptr(),
+                              (float*)save_rstd->wptr(), *train ? 1 : 0, momentum, eps));
+    state->batch = *train || !running_mean;
+  }
+};
+struct BatchNormBackward : Backward {
+  GradientP operand_grad, weight_grad, bias_grad;
+  TensorP operand, weight, save_mean, save_rstd;
+  std::shared_ptr<BatchNormState> state;
+  BatchNormBackward(nk_ctx* c, GradientP g, GradientP xg, GradientP wg, GradientP bg, TensorP x, TensorP w, TensorP sm,
+                    TensorP sr, std::shared_ptr<BatchNormState> s)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), weight_grad(std::move(wg)), bias_grad(std::move(bg)),
+        operand(std::move(x)), weight(std::move(w)), save_mean(std::move(sm)), save_rstd(std::move(sr)),
+        state(std::move(s)) {}
+  const char* name() const override { return "BatchNormBackward"; }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad, &weight_grad, &bias_grad}); }
+  void backward() override {
+    int64_t n, c, sp;
+    bn_dims(operand->shape, n, c, sp);
+    const void* g = gradient->get();
+    float bx = 0.f, bw = 0.f, bb = 0.f;  // one launch sequence writes all three, each with its own dtype and beta
+    void* dx = operand_grad ? operand_grad->acc(&bx) : nullptr;
+    void* dw = weight_grad ? weight_grad->acc(&bw) : nullptr;
+    void* db = bias_grad ? bias_grad->acc(&bb) : nullptr;
+    ck(ctx, nk_batch_norm_bwd(ctx, dx, operand_grad ? operand_grad->dtype : NK_F32, bx, dw,
+                              weight_grad ? weight_grad->dtype : NK_F32, bw, db, bias_grad ? bias_grad->dtype : NK_F32,
+                              bb, g, gradient->dtype, operand->rptr(), operand->dtype, n, c, sp, opt_r(weight),
+                              (const float*)save_mean->rptr(), (const float*)save_rstd->rptr(), state->batch ? 1 : 0));
+    grad_written(operand_grad);
+    grad_written(weight_grad);
+    grad_written(bias_grad);
+  }
+};
+
+// the last k dims of the operand are one row
+struct LayerNorm : Forward {
+  TensorP operand, weight, bias, data, save_mean, save_rstd;
+  int64_t cols;
+  float eps;
+  LayerNorm(nk_ctx* c, TensorP x, TensorP w, TensorP b, TensorP d, TensorP sm, TensorP sr, int64_t cl, float e)
+      : Forward(c), operand(std::move(x)), weight(std::move(w)), bias(std::move(b)), data(std::move(d)),
+        save_mean(std::move(sm)), save_rstd(std::move(sr)), cols(cl), eps(e) {}
+  const char* name() const override { return "LayerNorm"; }
+  void forward() override {
+    ck(ctx, nk_layer_norm_fwd(ctx, data->wptr(), operand->rptr(), data->dtype, operand->n() / cols, cols, opt_r(weight),
+                              opt_r(bias), (float*)save_mean->wptr(), (float*)save_rstd->wptr(), eps));
+  }
+};
+struct LayerNormBackward : Backward {
+  GradientP operand_grad, weight_grad, bias_grad;
+  TensorP operand, weight, save_mean, save_rstd;
+  int64_t cols;
+  LayerNormBackward(nk_ctx* c, GradientP g, GradientP xg, GradientP wg, GradientP bg, TensorP x, TensorP w, TensorP sm,
+                    TensorP sr, int64_t cl)
+      : Backward(c, std::move(g)), operand_grad(std::move(xg)), weight_grad(std::move(wg)), bias_grad(std::move(bg)),
+        operand(std::move(x)), weight(std::move(w)), save_mean(std::move(sm)), save_rstd(std::move(sr)), cols(cl) {}
+  const char* name() const override { return "LayerNormBackward"; }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&operand_grad, &weight_grad, &bias_grad}); }
+  void backward() override {
+    const void* g = gradient->get();
+    float bx = 0.f, bw = 0.f, bb = 0.f;
+    void* dx = operand_grad ? operand_grad->acc(&bx) : nullptr;
+    void* dw = weight_grad ? weight_grad->acc(&bw) : nullptr;
+    void* db = bias_grad ? bias_grad->acc(&bb) : nullptr;
+    ck(ctx, nk_layer_norm_bwd(ctx, dx, operand_grad ? operand_grad->dtype : NK_F32, bx, dw,
+                              weight_grad ? weight_grad->dtype : NK_F32, bw, db, bias_grad ? bias_grad->dtype : NK_F32,
+                              bb, g, gradient->dtype, operand->rptr(), operand->dtype, operand->n() / cols, cols,
+                              opt_r(weight), (const float*)save_mean->rptr(), (const float*)save_rstd->rptr()));
+    grad_written(operand_grad);
+    grad_written(weight_grad);
+    grad_written(bias_grad);
+  }
+};
+
 // ------------------------------------------------------------------------------- mv / vm / vv
 // matrix_vector_mul/mod.rs:11-129, vector_matrix_mul/mod.rs:11-129, vector_vector_mul/mod.rs:11-91
 struct MatVec : Forward {
@@ -2453,6 +2572,94 @@ int nkg_avg_pool(nkg_var* a, int nsp, const int64_t* kernel, const int64_t* stri
 
 int nkg_adaptive_avg_pool(nkg_var* a, int nsp, const int64_t* output_size, nkg_var** out) {
   return pool_record(kPoolAdaptive, a, nsp, nullptr, nullptr, nullptr, nullptr, output_size, false, false, out);
+}
+
+// a (C,) operand of a normalization: w / b of the operand's dtype, or a running statistic: a non-differentiable f32
+// leaf
+static void norm_param(nkg_var* p, nkg_var* x, const Shape& want, const char* who, const char* what, bool stat) {
+  if (!p) return;
+  if (p->ctx != x->ctx) fail(NK_ERR_INVALID_ARG, "%s: %s lives on another device", who, what);
+  if (p->data->shape != want)
+    fail(NK_ERR_INVALID_ARG, "%s: %s must have shape %s, got %s", who, what, shape_str(want).c_str(),
+         shape_str(p->data->shape).c_str());
+  if (stat) {
+    if (p->data->dtype != NK_F32) fail(NK_ERR_INVALID_ARG, "%s: %s must be f32", who, what);
+    if (p->diff()) fail(NK_ERR_INVALID_ARG, "%s: %s must not be differentiable", who, what);
+    // the forward writes it in place: only a leaf's buffer is the caller's alone, never another node's output
+    if (!p->fwd.empty()) fail(NK_ERR_INVALID_ARG, "%s: %s must be a leaf", who, what);
+  } else {
+    require_same_dtype(p, x, who);
+  }
+}
+
+int nkg_batch_norm(nkg_var* x, nkg_var* weight, nkg_var* bias, nkg_var* running_mean, nkg_var* running_var,
+                   nkg_status* status, float momentum, float eps, nkg_var** out) {
+  return guard([&] {
+    static const char* who = "batch_norm";
+    not_null({x, status, out}, who);
+    const Shape& s = x->data->shape;
+    if (s.size() < 2) fail(NK_ERR_INVALID_ARG, "%s: expects an (N, C, ...) operand, got %d dimensions", who, (int)s.size());
+    if (s[1] < 1) fail(NK_ERR_INVALID_ARG, "%s: no channels", who);
+    if (!running_mean != !running_var)
+      fail(NK_ERR_INVALID_ARG, "%s: running_mean and running_var are both given or both NULL", who);
+    if (!(eps >= 0.f)) fail(NK_ERR_INVALID_ARG, "%s: eps must be >= 0, got %g", who, eps);
+    const Shape cs{s[1]};
+    norm_param(weight, x, cs, who, "weight", false);
+    norm_param(bias, x, cs, who, "bias", false);
+    norm_param(running_mean, x, cs, who, "running_mean", true);
+    norm_param(running_var, x, cs, who, "running_var", true);
+    bn_check_batch(s, *status->train || !running_mean);
+    auto sm = std::make_shared<Tensor>(x->ctx, cs, NK_F32), sr = std::make_shared<Tensor>(x->ctx, cs, NK_F32);
+    sm->wptr();
+    sr->wptr();
+    auto state = std::make_shared<BatchNormState>();
+    TensorP w = weight ? weight->data : nullptr, b = bias ? bias->data : nullptr;
+    TensorP rm = running_mean ? running_mean->data : nullptr, rv = running_var ? running_var->data : nullptr;
+    std::vector<nkg_var*> operands{x};
+    if (weight) operands.push_back(weight);
+    if (bias) operands.push_back(bias);
+    *out = record(
+        operands, s, x->data->dtype,
+        [&](const TensorP& d) {
+          return std::make_shared<BatchNorm>(x->ctx, x->data, w, b, rm, rv, d, sm, sr, status->train, state, momentum,
+                                             eps);
+        },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<BatchNormBackward>(x->ctx, g, x->grad, weight ? weight->grad : nullptr,
+                                                     bias ? bias->grad : nullptr, x->data, w, sm, sr, state);
+        });
+  });
+}
+
+int nkg_layer_norm(nkg_var* x, int k, nkg_var* weight, nkg_var* bias, float eps, nkg_var** out) {
+  return guard([&] {
+    static const char* who = "layer_norm";
+    not_null({x, out}, who);
+    const Shape& s = x->data->shape;
+    if (k < 1 || k > (int)s.size())
+      fail(NK_ERR_INVALID_ARG, "%s: normalized_shape has %d dimensions, the input %d", who, k, (int)s.size());
+    if (!(eps >= 0.f)) fail(NK_ERR_INVALID_ARG, "%s: eps must be >= 0, got %g", who, eps);
+    const Shape ns(s.end() - k, s.end());
+    const int64_t cols = numel(ns);
+    if (cols < 1) fail(NK_ERR_INVALID_ARG, "%s: normalized_shape %s has no elements", who, shape_str(ns).c_str());
+    norm_param(weight, x, ns, who, "weight", false);
+    norm_param(bias, x, ns, who, "bias", false);
+    const Shape rs{x->data->n() / cols};
+    auto sm = std::make_shared<Tensor>(x->ctx, rs, NK_F32), sr = std::make_shared<Tensor>(x->ctx, rs, NK_F32);
+    sm->wptr();
+    sr->wptr();
+    TensorP w = weight ? weight->data : nullptr, b = bias ? bias->data : nullptr;
+    std::vector<nkg_var*> operands{x};
+    if (weight) operands.push_back(weight);
+    if (bias) operands.push_back(bias);
+    *out = record(
+        operands, s, x->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<LayerNorm>(x->ctx, x->data, w, b, d, sm, sr, cols, eps); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<LayerNormBackward>(x->ctx, g, x->grad, weight ? weight->grad : nullptr,
+                                                     bias ? bias->grad : nullptr, x->data, w, sm, sr, cols);
+        });
+  });
 }
 
 static int matvec_impl(nkg_var* mat, nkg_var* vec, bool vm, nkg_var** out) {

@@ -1,6 +1,6 @@
 """Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell, Conv1d, Conv2d and Conv3d (neuronika-nn/src/lib.rs:
 406-916), the sequence layers LSTM and GRU over them (stacked and bidirectional like torch.nn.LSTM / GRU), and torch's
-max, average and adaptive average pooling layers."""
+max, average and adaptive average pooling layers and its batch and layer normalization layers."""
 from __future__ import annotations
 
 import math
@@ -389,6 +389,83 @@ class AdaptiveAvgPool2d(_AdaptiveAvgPoolNd):
 class AdaptiveAvgPool3d(_AdaptiveAvgPoolNd):
     """torch.nn.AdaptiveAvgPool3d over (N, C, D, H, W)."""
     nsp = 3
+
+
+class _BatchNorm:
+    """torch's BatchNorm over (N, C, ...): weight = 1 and bias = 0 of the input's dtype when affine, f32 running_mean = 0
+    and running_var = 1 when track_running_stats.  Each module owns a Status: `train()` (the initial mode) normalizes
+    with the batch statistics and updates the running ones on every forward() of the graph, `eval()` normalizes with the
+    running statistics (with the batch ones when not tracking).  `forward` is one graph node (Var.batch_norm)."""
+
+    ranks: tuple = ()
+    expected = ""
+
+    def __init__(self, device: Device, num_features: int, eps: float = 1e-5, momentum: float | None = 0.1,
+                 affine: bool = True, track_running_stats: bool = True, dtype=F32, grad_dtype=None):
+        if momentum is None:
+            raise ValueError("momentum=None (a cumulative moving average) is not supported")
+        self.num_features, self.eps, self.momentum = int(num_features), float(eps), float(momentum)
+        self.affine, self.track_running_stats = bool(affine), bool(track_running_stats)
+        c = (self.num_features,)
+        self.weight = self.bias = self.running_mean = self.running_var = None
+        if self.affine:
+            self.weight = V.from_ndarray(device, np.ones(c, np.float32), dtype).requires_grad(grad_dtype)
+            self.bias = V.from_ndarray(device, np.zeros(c, np.float32), dtype).requires_grad(grad_dtype)
+        if self.track_running_stats:
+            self.running_mean = V.zeros(device, c)
+            self.running_var = V.ones(device, c)
+        self.status = V.Status(True)
+
+    def forward(self, input: V.Var) -> V.Var:
+        if len(input.shape) not in self.ranks:
+            raise ValueError(f"expected {self.expected} input (got {len(input.shape)}D input)")
+        return input.batch_norm(self.weight, self.bias, self.running_mean, self.running_var, self.status,
+                                self.momentum, self.eps)
+
+    def train(self) -> None:
+        self.status.train()
+
+    def eval(self) -> None:
+        self.status.eval()
+
+    def parameters(self):
+        return [self.weight, self.bias] if self.affine else []
+
+
+class BatchNorm1d(_BatchNorm):
+    """torch.nn.BatchNorm1d over (N, C) or (N, C, L)."""
+    ranks, expected = (2, 3), "2D or 3D"
+
+
+class BatchNorm2d(_BatchNorm):
+    """torch.nn.BatchNorm2d over (N, C, H, W)."""
+    ranks, expected = (4,), "4D"
+
+
+class BatchNorm3d(_BatchNorm):
+    """torch.nn.BatchNorm3d over (N, C, D, H, W)."""
+    ranks, expected = (5,), "5D"
+
+
+class LayerNorm:
+    """torch.nn.LayerNorm over the trailing dims `normalized_shape`: weight = 1 (when elementwise_affine) and bias = 0
+    (when also `bias`) of that shape and the input's dtype.  `forward` is one graph node (Var.layer_norm)."""
+
+    def __init__(self, device: Device, normalized_shape, eps: float = 1e-5, elementwise_affine: bool = True,
+                 bias: bool = True, dtype=F32, grad_dtype=None):
+        ns = (int(normalized_shape),) if np.isscalar(normalized_shape) else tuple(int(d) for d in normalized_shape)
+        self.normalized_shape, self.eps, self.elementwise_affine = ns, float(eps), bool(elementwise_affine)
+        self.weight = self.bias = None
+        if self.elementwise_affine:
+            self.weight = V.from_ndarray(device, np.ones(ns, np.float32), dtype).requires_grad(grad_dtype)
+            if bias:
+                self.bias = V.from_ndarray(device, np.zeros(ns, np.float32), dtype).requires_grad(grad_dtype)
+
+    def forward(self, input: V.Var) -> V.Var:
+        return input.layer_norm(self.normalized_shape, self.weight, self.bias, self.eps)
+
+    def parameters(self):
+        return [p for p in (self.weight, self.bias) if p is not None]
 
 
 class GRUCell:

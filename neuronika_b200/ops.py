@@ -422,6 +422,71 @@ def adaptive_avg_pool_nd_bwd(dx: CuArray, g: CuArray, beta=1.0, nsp=None) -> CuA
     return dx
 
 
+# ---------------------------------------------------------------- batch norm / layer norm (csrc/nk_norm.cu)
+def _bn_dims(shape):
+    return int(shape[0]), int(shape[1]), int(np.prod(shape[2:], dtype=np.int64))
+
+
+def batch_norm(x: CuArray, weight: CuArray | None = None, bias: CuArray | None = None,
+               running_mean: CuArray | None = None, running_var: CuArray | None = None, training=True, momentum=0.1,
+               eps=1e-5, out=None, save_mean: CuArray | None = None, save_rstd: CuArray | None = None):
+    """y = batch norm of x (N, C, ...) over N and the sample dims (nk_batch_norm_fwd).  Returns (y, save_mean,
+    save_rstd), the f32 (C,) statistics the backward takes; running_mean / running_var (f32) are updated in place when
+    training."""
+    n, c, s = _bn_dims(x.shape)
+    out = out or CuArray(x.device, x.shape, x.dtype)
+    save_mean = save_mean or CuArray(x.device, (c,), F32)
+    save_rstd = save_rstd or CuArray(x.device, (c,), F32)
+    _ck(lib.nk_batch_norm_fwd(x.device.ctx, out.ptr, x.ptr, x.dtype, n, c, s, _ptr(weight), _ptr(bias),
+                              _ptr(running_mean), _ptr(running_var), save_mean.ptr, save_rstd.ptr, int(bool(training)),
+                              float(momentum), float(eps)), x.device)
+    return out, save_mean, save_rstd
+
+
+def _grads(*pairs):
+    """(ptr, dtype, beta) for each (array or None, beta)"""
+    out = []
+    for a, beta in pairs:
+        out += [_ptr(a), a.dtype if a is not None else F32, float(beta)]
+    return out
+
+
+def batch_norm_bwd(g: CuArray, x: CuArray, save_mean: CuArray, save_rstd: CuArray, weight: CuArray | None = None,
+                   dx: CuArray | None = None, dw: CuArray | None = None, db: CuArray | None = None, batch_stats=True,
+                   beta=0.0, dw_beta=None, db_beta=None):
+    """dx / dw / db = beta*d + the batch norm's gradients (nk_batch_norm_bwd); any of them may be None."""
+    n, c, s = _bn_dims(x.shape)
+    betas = (beta, beta if dw_beta is None else dw_beta, beta if db_beta is None else db_beta)
+    _ck(lib.nk_batch_norm_bwd(x.device.ctx, *_grads((dx, betas[0]), (dw, betas[1]), (db, betas[2])), g.ptr, g.dtype,
+                              x.ptr, x.dtype, n, c, s, _ptr(weight), save_mean.ptr, save_rstd.ptr,
+                              int(bool(batch_stats))), x.device)
+    return dx, dw, db
+
+
+def layer_norm(x: CuArray, cols: int, weight: CuArray | None = None, bias: CuArray | None = None, eps=1e-5, out=None,
+               save_mean: CuArray | None = None, save_rstd: CuArray | None = None):
+    """y = layer norm of x's rows of `cols` elements (nk_layer_norm_fwd).  Returns (y, save_mean, save_rstd), the f32
+    (rows,) statistics the backward takes."""
+    rows = int(np.prod(x.shape, dtype=np.int64)) // cols
+    out = out or CuArray(x.device, x.shape, x.dtype)
+    save_mean = save_mean or CuArray(x.device, (rows,), F32)
+    save_rstd = save_rstd or CuArray(x.device, (rows,), F32)
+    _ck(lib.nk_layer_norm_fwd(x.device.ctx, out.ptr, x.ptr, x.dtype, rows, cols, _ptr(weight), _ptr(bias),
+                              save_mean.ptr, save_rstd.ptr, float(eps)), x.device)
+    return out, save_mean, save_rstd
+
+
+def layer_norm_bwd(g: CuArray, x: CuArray, cols: int, save_mean: CuArray, save_rstd: CuArray,
+                   weight: CuArray | None = None, dx: CuArray | None = None, dw: CuArray | None = None,
+                   db: CuArray | None = None, beta=0.0, dw_beta=None, db_beta=None):
+    """dx / dw / db = beta*d + the layer norm's gradients (nk_layer_norm_bwd); any of them may be None."""
+    rows = int(np.prod(x.shape, dtype=np.int64)) // cols
+    betas = (beta, beta if dw_beta is None else dw_beta, beta if db_beta is None else db_beta)
+    _ck(lib.nk_layer_norm_bwd(x.device.ctx, *_grads((dx, betas[0]), (dw, betas[1]), (db, betas[2])), g.ptr, g.dtype,
+                              x.ptr, x.dtype, rows, cols, _ptr(weight), save_mean.ptr, save_rstd.ptr), x.device)
+    return dx, dw, db
+
+
 # ---------------------------------------------------------------- 8-f: mv / vm / vv
 def gemv(a: CuArray, x: CuArray, y: CuArray | None = None, trans=False, beta=0.0) -> CuArray:
     rows, cols = a.shape

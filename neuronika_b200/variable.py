@@ -105,6 +105,8 @@ _G = {
     "nkg_max_pool": (i32, [vp, i32, pi64, pi64, pi64, pi64, i32, pvp]),
     "nkg_avg_pool": (i32, [vp, i32, pi64, pi64, pi64, i32, i32, pvp]),
     "nkg_adaptive_avg_pool": (i32, [vp, i32, pi64, pvp]),
+    "nkg_batch_norm": (i32, [vp, vp, vp, vp, vp, vp, f32, f32, pvp]),
+    "nkg_layer_norm": (i32, [vp, i32, vp, vp, f32, pvp]),
 }
 for _n, (_r, _a) in _G.items():
     _f = getattr(lib, _n)
@@ -322,6 +324,27 @@ class Var:
         axis is [floor(i*L/O), ceil((i+1)*L/O))."""
         o = self._nsp_tuple(output_size, "output_size")
         return self._unary(lib.nkg_adaptive_avg_pool, len(o), L.shape_arr(o))
+
+    def batch_norm(self, weight=None, bias=None, running_mean=None, running_var=None, status: Status | None = None,
+                   momentum: float = 0.1, eps: float = 1e-5):
+        """torch's batch_norm over N and the sample dims of an (N, C, ...) operand, as one node.  weight / bias: (C,)
+        of the operand's dtype or None; running_mean / running_var: f32 (C,) Vars (not differentiable) updated in place
+        by every training forward, or both None.  `status` (a Status; training when None) is read on each forward():
+        batch statistics in training mode or without running statistics, the running ones otherwise."""
+        h = lambda v: v._h if v is not None else None
+        return self._unary(lib.nkg_batch_norm, h(weight), h(bias), h(running_mean), h(running_var),
+                           (status or Status())._h, float(momentum), float(eps))
+
+    def layer_norm(self, normalized_shape, weight=None, bias=None, eps: float = 1e-5):
+        """torch's layer_norm over the trailing dims `normalized_shape`, as one node; weight / bias have that shape and
+        the operand's dtype, or are None."""
+        ns = (int(normalized_shape),) if np.isscalar(normalized_shape) else tuple(int(d) for d in normalized_shape)
+        shape = self.shape
+        if not ns or len(ns) > len(shape) or shape[len(shape) - len(ns):] != ns:
+            raise L.NkError(-1, f"Given normalized_shape={list(ns)}, expected input with shape [*, "
+                                f"{', '.join(str(d) for d in ns)}], but got input of size{list(shape)}")
+        h = lambda v: v._h if v is not None else None
+        return self._unary(lib.nkg_layer_norm, len(ns), h(weight), h(bias), float(eps))
 
     def pad(self, padding, value: float = 0.0, mode: str = "constant"):
         """`pad(padding, mode)` (var.rs:726-737): Zero / Constant(value) / Reflective / Replicative over the 1..3
