@@ -501,57 +501,36 @@ int nk_cat_fwd(nk_ctx* ctx, void* y, const void* const* xs, const int64_t* lens,
 int nk_cat_bwd(nk_ctx* ctx, void* const* dxs, const int* dx_dtypes, const float* betas, const void* g, int g_dtype,
                const int64_t* lens, int count, int64_t outer, int64_t inner);
 
-/* ---- SGD (neuronika-optim/src/sgd/mod.rs:191-231, penalty.rs:63-67) ----
- *   g' = grad_scale*g + 2*l2*w ; no momentum: w -= lr*g' ;
- *   momentum: buf = mu*buf + (1-damp)*g' ; w -= lr*(nesterov ? g' + mu*buf : buf).
- *   `buf` (f32, n elements) may be NULL when momentum <= FLT_EPSILON.
- *   `master` (f32, optional) keeps an f32 copy of bf16 weights: the update is applied to
- *   master and w receives its rounding.  grad_scale = 1/world_size for data parallel. */
-int nk_sgd_step(nk_ctx* ctx, void* w, int w_dtype, void* g, int g_dtype, float* buf, float* master,
-                size_t n, float lr, float l2, float momentum, float dampening, int nesterov,
-                float grad_scale, int write_back_grad);
-
-/* ---- Adam / AMSGrad / RMSProp / Adagrad as single fused passes (8-f rank 2; csrc/nk_optim.cu) ----
- * Common to all: g' = grad_scale*g + l1*signum(w) + 2*l2*w (penalty.rs:63-79: L1, L2, ElasticNet), written
- * back into g when write_back_grad (the reference adds the penalty into the gradient); state arrays are
- * f32, n elements, zero before the first step; `master` as in nk_sgd_step.
- *   adam     m = b1*m + (1-b1)g'; v = b2*v + (1-b2)g'^2; w -= m / (sqrt(v)/sqrt(1-b2^t) + eps) * lr/(1-b1^t)
- *            (adam/mod.rs:131-169); max_exp_avg_sq != NULL -> AMSGrad: v^ = max(v^, v) replaces v in the
- *            denominator (amsgrad/mod.rs:159-204).  `step` = t, counted from 1.
- *   rmsprop  s = a*s + (1-a)g'^2; centered (grad_avg != NULL): ga = a*ga + (1-a)g', denom = sqrt(s - ga^2)+eps
- *            else sqrt(s)+eps; momentum (> f32::EPSILON, buffer != NULL): b = mu*b + g'/denom, w -= lr*b;
- *            else w -= g'/denom*lr (rmsprop/mod.rs:193-300).
- *   adagrad  s += g'^2; w -= g' / (sqrt(s) + eps) * lr / (1 + (t-1)*lr_decay)   (adagrad/mod.rs:113-140). */
-int nk_adam_step(nk_ctx* ctx, void* w, int w_dtype, void* g, int g_dtype, float* exp_avg,
-                 float* exp_avg_sq, float* max_exp_avg_sq, float* master, size_t n, int64_t step, float lr,
-                 float beta1, float beta2, float eps, float l1, float l2, float grad_scale,
-                 int write_back_grad);
-int nk_rmsprop_step(nk_ctx* ctx, void* w, int w_dtype, void* g, int g_dtype, float* square_avg,
-                    float* grad_avg, float* momentum_buf, float* master, size_t n, float lr, float alpha,
-                    float eps, float momentum, float l1, float l2, float grad_scale, int write_back_grad);
-int nk_adagrad_step(nk_ctx* ctx, void* w, int w_dtype, void* g, int g_dtype, float* grad_sq, float* master,
-                    size_t n, int64_t step, float lr, float lr_decay, float eps, float l1, float l2,
-                    float grad_scale, int write_back_grad);
-
-/* ---- capturable optimizers and learning-rate schedulers (csrc/nk_optim_multi.cu) ----
- * The per-parameter entry points above take lr and the step count as kernel arguments, so a captured step replays the
- * lr and the bias correction (or lr decay) of the step it was captured at.  Here both live in device memory, in a
- * caller-allocated nk_optim_hyper block that the kernels read (and the prologue and the scheduler write), so a captured
- * step advances them on every replay.
+/* ---- optimizers and learning-rate schedulers (csrc/nk_optim_multi.cu) ----
+ * lr and the step count live in device memory, in a caller-allocated nk_optim_hyper block that the kernels read (and
+ * the prologue and the scheduler write), so a captured step advances them on every replay.
  *   nk_optim_hyper_set / _get copy the whole block to / from the device and synchronise; NK_ERR_UNSUPPORTED while
  *   capturing (a replay would not repeat them).
  *   nk_optim_prologue (one thread): step += 1, then, for NK_OPTIM_ADAM (Adam and AMSGrad), step_size = lr/(1-b1^t) and
  *   sqrt_bc2 = sqrt(1-b2^t), b^t by repeated squaring; for NK_OPTIM_ADAGRAD clr = lr/(1+(t-1)*lr_decay).  Every
- *   operation is rounded on its own in the order nk_adam_step / nk_adagrad_step use on the host, so the scalars are
- *   bit-identical to theirs.  SGD and RMSProp need no prologue: their kernels read lr.
- *   nk_multi_*_step: the update of nk_sgd_step / nk_adam_step / nk_rmsprop_step / nk_adagrad_step, with the same
- *   per-element arithmetic (bit-identical results, written-back gradient included), over `count` <=
- *   NK_OPTIM_TENSORS_PER_LAUNCH tensors of one (w_dtype, g_dtype) pair in ONE launch.  w, g and n are arrays of `count`
- *   entries; each state / master argument is an array of `count` device pointers or NULL (= every entry NULL); a NULL
- *   master entry means that tensor has none.  The tensor table travels in the kernel parameters: no allocation, no
- *   host-to-device copy, so the call can be captured.  A tensor takes 4-element (16-byte f32) accesses when all its
- *   pointers allow them, element accesses otherwise.  nk_multi_sgd_step skips the gradient write-back when l2 = 0 and
- *   grad_scale = 1, as nk_sgd_step does.
+ *   operation is rounded on its own in f32, in the order written.  SGD and RMSProp need no prologue: their kernels read
+ *   lr.
+ *   nk_multi_*_step: one optimizer step over `count` <= NK_OPTIM_TENSORS_PER_LAUNCH tensors of one (w_dtype, g_dtype)
+ *   pair in ONE launch.  w, g and n are arrays of `count` entries; each state / master argument is an array of `count`
+ *   device pointers or NULL (= every entry NULL).  State arrays are f32, n elements, zero before the first step.
+ *   `master` (f32, optional; a NULL entry means that tensor has none) keeps an f32 copy of bf16 weights: the update is
+ *   applied to master and w receives its rounding.  The tensor table travels in the kernel parameters: no allocation,
+ *   no host-to-device copy, so the call can be captured.  A tensor takes 4-element (16-byte f32) accesses when all its
+ *   pointers allow them, element accesses otherwise.  grad_scale = 1/world_size for data parallel.  Per element, with t
+ *   the step count and lr, step_size, sqrt_bc2, clr read from `hyper`:
+ *   sgd      (sgd/mod.rs:191-231, penalty.rs:63-67) g' = grad_scale*g + 2*l2*w ; no momentum: w -= lr*g' ;
+ *            momentum: buf = mu*buf + (1-damp)*g' ; w -= lr*(nesterov ? g' + mu*buf : buf).  `momentum_buf` may be
+ *            NULL when momentum <= FLT_EPSILON.  g' is written back into g when write_back_grad, except when l2 = 0 and
+ *            grad_scale = 1 (then g' = g).
+ *   The Adam family: g' = grad_scale*g + l1*signum(w) + 2*l2*w (penalty.rs:63-79: L1, L2, ElasticNet), written back into
+ *   g when write_back_grad (the reference adds the penalty into the gradient).
+ *   adam     m = b1*m + (1-b1)g'; v = b2*v + (1-b2)g'^2; w -= m / (sqrt(v)/sqrt_bc2 + eps) * step_size
+ *            (adam/mod.rs:131-169); max_exp_avg_sq != NULL -> AMSGrad: v^ = max(v^, v) replaces v in the
+ *            denominator (amsgrad/mod.rs:159-204).
+ *   rmsprop  s = a*s + (1-a)g'^2; centered (grad_avg != NULL): ga = a*ga + (1-a)g', denom = sqrt(s - ga^2)+eps
+ *            else sqrt(s)+eps; momentum (> f32::EPSILON, momentum_buf != NULL): b = mu*b + g'/denom, w -= lr*b;
+ *            else w -= g'/denom*lr (rmsprop/mod.rs:193-300).
+ *   adagrad  s += g'^2; w -= g' / (sqrt(s) + eps) * clr   (adagrad/mod.rs:113-140).
  * Learning-rate schedulers (lr_scheduler/{step_lr,multi_step_lr,exponential_lr,multiplicative_lr,lambda_lr}/mod.rs):
  * nk_lr_sched_step (one thread) advances epoch to t = epoch + 1 and applies the rule to the optimizer block's lr in f32:
  *   STEP           lr *= gamma when t % step_size == 0        MULTI_STEP  lr *= gamma when t is one of the milestones
@@ -609,7 +588,7 @@ int nk_lr_sched_step(nk_ctx* ctx, nk_lr_sched* sched, nk_optim_hyper* hyper);
  * without it.  Rank 0 creates the 128-byte id and ships it to the others by any means; every rank then
  * calls nk_comm_init_rank (collective).  nk_allreduce_sum sums `n` elements in place over the replicas,
  * enqueued on the context stream (ordered with the kernels that produced the gradients and with the
- * nk_sgd_step that follows).  Errors: NK_ERR_NCCL. */
+ * nk_multi_sgd_step that follows).  Errors: NK_ERR_NCCL. */
 int nk_comm_unique_id(nk_ctx* ctx, void* id128);
 int nk_comm_init_rank(nk_ctx* ctx, int world, int rank, const void* id128);
 int nk_comm_destroy(nk_ctx* ctx);

@@ -233,25 +233,14 @@ int nkg_set_grad_hook(nkg_var* leaf, nkg_grad_hook cb, void* user, int row_chunk
 typedef void (*nkg_grad_rs_hook)(void* user, int pushed);
 int nkg_set_grad_rs(nkg_var* leaf, int world, int rank, void* const* slots, nkg_grad_rs_hook cb, void* user);
 
-/* ---- SGD on a leaf (neuronika-optim/src/sgd/mod.rs:191-231) ---- */
-int nkg_sgd_step(nkg_var* param, float* momentum_buf, float* master, float lr, float l2, float momentum,
-                 float dampening, int nesterov, float grad_scale);
-
-/* ---- Adam / AMSGrad / RMSProp / Adagrad on a leaf (neuronika-optim/src/{adam,amsgrad,rmsprop,adagrad}/mod.rs);
- * state arrays are caller-owned f32 device buffers of the parameter's size (see nk_b200.h nk_adam_step ...) */
-int nkg_adam_step(nkg_var* param, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, float* master,
-                  int64_t step, float lr, float beta1, float beta2, float eps, float l1, float l2, float grad_scale);
-int nkg_rmsprop_step(nkg_var* param, float* square_avg, float* grad_avg, float* momentum_buf, float* master, float lr,
-                     float alpha, float eps, float momentum, float l1, float l2, float grad_scale);
-int nkg_adagrad_step(nkg_var* param, float* grad_sq, float* master, int64_t step, float lr, float lr_decay, float eps,
-                     float l1, float l2, float grad_scale);
-
-/* ---- capturable optimizers over many leaves (nk_b200.h nk_multi_*_step): one optimizer step over `count` parameters,
- * lr and the step count in the device block `hyper`.  State and master arguments are arrays of `count` device pointers
- * in parameter order (or NULL: none).  Each parameter is checked and its gradient handled as by nkg_*_step; Adam and
- * Adagrad then launch nk_optim_prologue once; the parameters are grouped by (data, gradient) element types and each
- * group is updated by one nk_multi_*_step call per NK_OPTIM_TENSORS_PER_LAUNCH tensors, in parameter order.  A
- * parameter that is not differentiable fails the call before anything is launched. */
+/* ---- optimizers over many leaves (neuronika-optim/src/{sgd,adam,amsgrad,rmsprop,adagrad}/mod.rs; nk_b200.h
+ * nk_multi_*_step): one optimizer step over `count` parameters, lr and the step count in the device block `hyper`.
+ * State and master arguments are arrays of `count` caller-owned f32 device buffers of the parameters' sizes, in
+ * parameter order (or NULL: none).  Each parameter's gradient is taken as the backward pass left it (zeros after
+ * nkg_zero_grad) and receives the penalised gradient; Adam and Adagrad then launch nk_optim_prologue once; the
+ * parameters are grouped by (data, gradient) element types and each group is updated by one nk_multi_*_step call per
+ * NK_OPTIM_TENSORS_PER_LAUNCH tensors, in parameter order.  A parameter that is not differentiable fails the call
+ * before anything is launched. */
 int nkg_multi_sgd_step(nkg_var* const* params, int count, void* const* momentum_buf, void* const* master,
                        nk_optim_hyper* hyper, float l2, float momentum, float dampening, int nesterov, float grad_scale);
 int nkg_multi_adam_step(nkg_var* const* params, int count, void* const* exp_avg, void* const* exp_avg_sq,

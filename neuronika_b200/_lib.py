@@ -37,7 +37,7 @@ class NkError(RuntimeError):
 
 
 class OptimHyper(C.Structure):
-    """nk_optim_hyper: the device-resident lr and step count of a capturable optimizer"""
+    """nk_optim_hyper: the device-resident lr and step count of an optimizer"""
     _fields_ = [("lr", C.c_float), ("step_size", C.c_float), ("sqrt_bc2", C.c_float), ("clr", C.c_float),
                 ("step", C.c_int64)]
 
@@ -160,9 +160,6 @@ _PROTOS = {
     "nk_conv_layer_nd_bwd_input": (i32, [vp, vp, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, pi64, i32, i32, f32]),
     "nk_conv_layer_nd_bwd_kernel": (i32, [vp, vp, i32, vp, vp, vp, i32, i64, i64, pi64, i64, pi64, pi64, pi64, pi64, i32,
                                           f32, i32, f32]),
-    "nk_adam_step": (i32, [vp, vp, i32, vp, i32, vp, vp, vp, vp, sz, i64, f32, f32, f32, f32, f32, f32, f32, i32]),
-    "nk_rmsprop_step": (i32, [vp, vp, i32, vp, i32, vp, vp, vp, vp, sz, f32, f32, f32, f32, f32, f32, f32, i32]),
-    "nk_adagrad_step": (i32, [vp, vp, i32, vp, i32, vp, vp, sz, i64, f32, f32, f32, f32, f32, f32, i32]),
     "nk_optim_hyper_set": (i32, [vp, vp, vp]),
     "nk_optim_hyper_get": (i32, [vp, vp, vp]),
     "nk_optim_prologue": (i32, [vp, vp, i32, f32, f32, f32]),
@@ -181,7 +178,6 @@ _PROTOS = {
     "nk_comm_world": (i32, [vp]),
     "nk_comm_rank": (i32, [vp]),
     "nk_allreduce_sum": (i32, [vp, vp, sz, i32]),
-    "nk_sgd_step": (i32, [vp, vp, i32, vp, i32, vp, vp, sz, f32, f32, f32, f32, i32, f32, i32]),
     "nk_lstm_cell_fwd": (i32, [vp, vp, vp, vp, vp, i64, i64, i32]),
     "nk_lstm_cell_bwd": (i32, [vp, vp, i32, vp, f32, vp, vp, vp, vp, i64, i64, i32]),
     "nk_gru_cell_fwd": (i32, [vp, vp, vp, vp, vp, i64, i64, i32]),

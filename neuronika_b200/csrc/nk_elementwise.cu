@@ -1,14 +1,10 @@
 // HBM-bound elementwise / broadcast / reduction kernels of the hot path:
 //   fill, cast, broadcast add + un-broadcast (addition/mod.rs:39-135, utils.rs:97-192),
 //   ReLU (relu/mod.rs:29-79), MSE / NLL / sum / mean (squared_error/mod.rs:46-122,
-//   nll/mod.rs:42-133, sum/mod.rs, mean/mod.rs), constant pad (pad/mod.rs:97-182),
-//   SGD (neuronika-optim/src/sgd/mod.rs:191-231).
+//   nll/mod.rs:42-133, sum/mod.rs, mean/mod.rs), constant pad (pad/mod.rs:97-182).
 // All kernels: 128-bit vector loads/stores when pointers are 16-byte aligned, grid sized to a
 // multiple of the SM count, warp-shuffle reductions, f32 arithmetic whatever the storage type.
-#include <float.h>
-
 #include "nk_internal.cuh"
-#include "nk_optim_math.cuh"
 
 namespace {
 
@@ -476,59 +472,6 @@ __global__ void __launch_bounds__(kThreads) pad2d_bwd_kernel(T* __restrict__ dx,
   }
 }
 
-// ---------------------------------------------------------------- SGD
-template <typename TW, typename TG>
-__global__ void __launch_bounds__(kThreads) sgd_kernel(TW* __restrict__ w, TG* __restrict__ g, float* __restrict__ buf,
-                                                      float* __restrict__ master, size_t n, float lr, float l2x2,
-                                                      float mu, float one_minus_damp, int use_momentum, int nesterov,
-                                                      float grad_scale, int write_back_grad) {
-  const size_t stride = size_t(gridDim.x) * blockDim.x;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
-    float wv = master ? master[i] : nk_to_f32<TW>(w[i]);
-    const float gv = nk_sgd_grad(nk_to_f32<TG>(g[i]), wv, grad_scale, l2x2);
-    if (write_back_grad) g[i] = nk_from_f32<TG>(gv);
-    float b = use_momentum ? buf[i] : 0.f;
-    wv = nk_sgd_update(wv, gv, b, lr, mu, one_minus_damp, use_momentum, nesterov);
-    if (use_momentum) buf[i] = b;
-    if (master) master[i] = wv;
-    w[i] = nk_from_f32<TW>(wv);
-  }
-}
-
-// Four elements per thread with 8-/16-byte accesses (the scalar kernel above moved config 4's 16.8 M-element weight at
-// 3.6 TB/s); same arithmetic, element by element, so the results are bit-identical to the scalar kernel.
-template <typename T>
-struct alignas(sizeof(T) * 4) Quad {
-  T v[4];
-};
-template <typename TW, typename TG>
-__global__ void __launch_bounds__(kThreads) sgd_kernel_vec4(TW* __restrict__ w, TG* __restrict__ g, float* __restrict__ buf,
-                                                           float* __restrict__ master, size_t n4, float lr, float l2x2,
-                                                           float mu, float one_minus_damp, int use_momentum, int nesterov,
-                                                           float grad_scale, int write_back_grad) {
-  const size_t stride = size_t(gridDim.x) * blockDim.x;
-  for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    Quad<TW> wq = reinterpret_cast<Quad<TW>*>(w)[i];
-    Quad<TG> gq = reinterpret_cast<Quad<TG>*>(g)[i];
-    Quad<float> mq, bq;
-    if (master) mq = reinterpret_cast<Quad<float>*>(master)[i];
-    if (use_momentum) bq = reinterpret_cast<Quad<float>*>(buf)[i];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      float wv = master ? mq.v[e] : nk_to_f32<TW>(wq.v[e]);
-      const float gv = nk_sgd_grad(nk_to_f32<TG>(gq.v[e]), wv, grad_scale, l2x2);
-      gq.v[e] = nk_from_f32<TG>(gv);
-      wv = nk_sgd_update(wv, gv, bq.v[e], lr, mu, one_minus_damp, use_momentum, nesterov);
-      mq.v[e] = wv;
-      wq.v[e] = nk_from_f32<TW>(wv);
-    }
-    if (write_back_grad) reinterpret_cast<Quad<TG>*>(g)[i] = gq;
-    if (use_momentum) reinterpret_cast<Quad<float>*>(buf)[i] = bq;
-    if (master) reinterpret_cast<Quad<float>*>(master)[i] = mq;
-    reinterpret_cast<Quad<TW>*>(w)[i] = wq;
-  }
-}
-
 }  // namespace
 
 int nk_reduce_finish(nk_ctx* ctx, float* out, const double* partials, int nparts, double scale) {
@@ -965,48 +908,6 @@ int nk_pad2d_bwd(nk_ctx* ctx, void* dx, const void* g, int64_t planes, int64_t h
 #undef NK_PAD_B2
 #undef NK_PAD_B
   NK_LAUNCHED(ctx, "pad2d_bwd");
-  return NK_OK;
-}
-
-int nk_sgd_step(nk_ctx* ctx, void* w, int w_dtype, void* g, int g_dtype, float* buf, float* master, size_t n,
-                float lr, float l2, float momentum, float dampening, int nesterov, float grad_scale,
-                int write_back_grad) {
-  if (!ctx) return NK_ERR_INVALID_ARG;
-  NK_REQUIRE(ctx, nk_dtype_ok(w_dtype) && nk_dtype_ok(g_dtype), "nk_sgd_step: bad dtype");
-  if (n == 0) return NK_OK;
-  NK_REQUIRE(ctx, w && g, "nk_sgd_step: NULL pointer");
-  const int use_mom = momentum > FLT_EPSILON;  // `.filter(|val| *val > f32::EPSILON)`, sgd/mod.rs:202
-  NK_REQUIRE(ctx, !use_mom || buf, "nk_sgd_step: momentum requires a buffer");
-  int blocks = ew_blocks(ctx, n);
-  const float l2x2 = 2.f * l2, omd = 1.f - dampening;
-  if (l2x2 == 0.f && grad_scale == 1.f) write_back_grad = 0;  // g' == g: storing it back would only move bytes
-  // body: four elements per thread where every pointer takes the wide access; tail (n % 4 elements): scalar kernel
-  const bool vec = n >= 4 && (reinterpret_cast<uintptr_t>(w) % (4 * nk_dtype_size(w_dtype)) == 0) &&
-                   (reinterpret_cast<uintptr_t>(g) % (4 * nk_dtype_size(g_dtype)) == 0) &&
-                   (!buf || reinterpret_cast<uintptr_t>(buf) % 16 == 0) && (!master || reinterpret_cast<uintptr_t>(master) % 16 == 0);
-  const size_t n4 = vec ? n / 4 : 0, done = n4 * 4, rest = n - done;
-  const int vblocks = ew_blocks(ctx, n4 ? n4 : 1);
-  blocks = ew_blocks(ctx, rest ? rest : 1);
-#define NK_SGD(TW, TG)                                                                                                    \
-  do {                                                                                                                    \
-    if (n4)                                                                                                               \
-      sgd_kernel_vec4<TW, TG><<<vblocks, kThreads, 0, ctx->stream>>>((TW*)w, (TG*)g, buf, master, n4, lr, l2x2, momentum,   \
-                                                                     omd, use_mom, nesterov, grad_scale, write_back_grad); \
-    if (rest)                                                                                                             \
-      sgd_kernel<TW, TG><<<blocks, kThreads, 0, ctx->stream>>>((TW*)w + done, (TG*)g + done, buf ? buf + done : nullptr,    \
-                                                                master ? master + done : nullptr, rest, lr, l2x2, momentum, \
-                                                                omd, use_mom, nesterov, grad_scale, write_back_grad);      \
-  } while (0)
-  if (w_dtype == NK_F32 && g_dtype == NK_F32)
-    NK_SGD(float, float);
-  else if (w_dtype == NK_BF16 && g_dtype == NK_BF16)
-    NK_SGD(__nv_bfloat16, __nv_bfloat16);
-  else if (w_dtype == NK_BF16 && g_dtype == NK_F32)
-    NK_SGD(__nv_bfloat16, float);
-  else
-    NK_SGD(float, __nv_bfloat16);
-#undef NK_SGD
-  NK_LAUNCHED(ctx, "sgd");
   return NK_OK;
 }
 

@@ -3051,42 +3051,11 @@ int nkg_gru_layer(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* 
   });
 }
 
-// ---------------------------------------------------------------- optimizers on a leaf (neuronika-optim)
-int nkg_adam_step(nkg_var* p, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, float* master, int64_t step,
-                  float lr, float beta1, float beta2, float eps, float l1, float l2, float grad_scale) {
-  return guard([&] {
-    if (!p || !p->diff()) fail(NK_ERR_INVALID_ARG, "adam: parameter is not differentiable");
-    Gradient* g = p->grad->root();
-    ck(p->ctx, nk_adam_step(p->ctx, p->data->rptr(), p->data->dtype, p->grad->get(), g->dtype, exp_avg, exp_avg_sq,
-                            max_exp_avg_sq, master, size_t(p->data->n()), step, lr, beta1, beta2, eps, l1, l2, grad_scale, 1));
-    g->is_zero = false;
-  });
-}
-int nkg_rmsprop_step(nkg_var* p, float* square_avg, float* grad_avg, float* momentum_buf, float* master, float lr,
-                     float alpha, float eps, float momentum, float l1, float l2, float grad_scale) {
-  return guard([&] {
-    if (!p || !p->diff()) fail(NK_ERR_INVALID_ARG, "rmsprop: parameter is not differentiable");
-    Gradient* g = p->grad->root();
-    ck(p->ctx, nk_rmsprop_step(p->ctx, p->data->rptr(), p->data->dtype, p->grad->get(), g->dtype, square_avg, grad_avg,
-                               momentum_buf, master, size_t(p->data->n()), lr, alpha, eps, momentum, l1, l2, grad_scale, 1));
-    g->is_zero = false;
-  });
-}
-int nkg_adagrad_step(nkg_var* p, float* grad_sq, float* master, int64_t step, float lr, float lr_decay, float eps,
-                     float l1, float l2, float grad_scale) {
-  return guard([&] {
-    if (!p || !p->diff()) fail(NK_ERR_INVALID_ARG, "adagrad: parameter is not differentiable");
-    Gradient* g = p->grad->root();
-    ck(p->ctx, nk_adagrad_step(p->ctx, p->data->rptr(), p->data->dtype, p->grad->get(), g->dtype, grad_sq, master,
-                               size_t(p->data->n()), step, lr, lr_decay, eps, l1, l2, grad_scale, 1));
-    g->is_zero = false;
-  });
-}
-
-// ---------------------------------------------------------------- capturable optimizers over many leaves
-// Every parameter gets nkg_*_step's checks and gradient handling in parameter order (the differentiable check first, for
-// all of them, so that an error launches nothing); the tensors are then grouped by (data dtype, gradient dtype) in the
-// order each pair first appears, and each group is updated NK_OPTIM_TENSORS_PER_LAUNCH tensors per call.
+// ---------------------------------------------------------------- optimizers over many leaves (neuronika-optim)
+// Every parameter is checked to be differentiable before anything launches, so that an error launches nothing; then, in
+// parameter order, each gradient is materialised (Gradient::get) and marked nonzero after the update, since the kernels
+// write the penalised gradient back.  The tensors are grouped by (data dtype, gradient dtype) in the order each pair
+// first appears, and each group is updated NK_OPTIM_TENSORS_PER_LAUNCH tensors per call.
 extern "C++" {
 namespace {
 struct MultiGroup {
@@ -3229,17 +3198,6 @@ int nkg_set_grad_hook(nkg_var* leaf, nkg_grad_hook cb, void* user, int row_chunk
     r->hook = cb;
     r->hook_user = user;
     r->hook_chunks = row_chunks > 1 ? row_chunks : 1;
-  });
-}
-
-int nkg_sgd_step(nkg_var* p, float* momentum_buf, float* master, float lr, float l2, float momentum, float dampening,
-                 int nesterov, float grad_scale) {
-  return guard([&] {
-    if (!p || !p->diff()) fail(NK_ERR_INVALID_ARG, "sgd: parameter is not differentiable");
-    Gradient* g = p->grad->root();
-    ck(p->ctx, nk_sgd_step(p->ctx, p->data->rptr(), p->data->dtype, p->grad->get(), g->dtype, momentum_buf, master,
-                           size_t(p->data->n()), lr, l2, momentum, dampening, nesterov, grad_scale, 1));
-    g->is_zero = false;
   });
 }
 

@@ -1,19 +1,105 @@
-// Capturable optimizers: the update of every parameter tensor of one (w dtype, g dtype) pair in one launch per
+// Optimizers: the update of every parameter tensor of one (w dtype, g dtype) pair in one launch per
 // NK_OPTIM_TENSORS_PER_LAUNCH tensors, with lr and the step count in device memory (nk_optim_hyper), plus the
 // learning-rate scheduler step as a one-thread kernel on the same block.
+//
+// The reference walks the parameter three to five times per step (one Zip per state array:
+// neuronika-optim/src/adam/mod.rs:131-169, amsgrad/mod.rs:159-204, rmsprop/mod.rs:193-300, adagrad/mod.rs:113-140);
+// here every element is read and written once.  Per-element arithmetic keeps the reference's operation order (f32), so
+// the f32 path matches it to rounding.
 //
 // The tensor table travels in the kernel parameters (__grid_constant__), as nk_cat.cu's operand table does: the grid
 // is the concatenation of every tensor's CTAs, the host computes the CTA prefix and each CTA finds its tensor with a
 // binary search.  A CTA covers kChunk consecutive elements of its tensor.  Each thread takes 4 consecutive elements
 // (16-byte f32 / 8-byte bf16 accesses) when all of the tensor's pointers are aligned for it, and walks the chunk with
-// element accesses otherwise.  The per-element arithmetic is nk_optim_math.cuh's, the same code the per-parameter
-// kernels inline, so both paths give the same bits.
-// HBM bound: algorithmic bytes per element as nk_optim.cu (24..28 B in f32 for two states).
+// element accesses otherwise.
+// HBM bound: algorithmic bytes per element = w (r+w) + g (r[+w]) + 2 states (r+w) = 24..28 B in f32.
 #include <float.h>
 #include <limits.h>
 
 #include "nk_internal.cuh"
-#include "nk_optim_math.cuh"
+
+// Per-element arithmetic of the five optimizers.  `wv` is the f32 weight (the master copy when there is one), `gv` the
+// penalised gradient.
+//
+// SGD penalty (sgd/mod.rs:191-231, penalty.rs:63-67): g' = grad_scale*g + 2*l2*w.  The SGD update spells out its
+// fused multiply-adds, so that its rounding does not depend on how nvcc contracts `a*b + c*d` where it is inlined.
+__device__ __forceinline__ float nk_sgd_grad(float g, float wv, float grad_scale, float l2x2) {
+  return __fmaf_rn(l2x2, wv, __fmul_rn(g, grad_scale));  // grad += penalty.penalize(w) = 2*lambda*w
+}
+
+__device__ __forceinline__ float nk_sgd_update(float wv, float gv, float& buf, float lr, float mu, float one_minus_damp,
+                                               int use_momentum, int nesterov) {
+  if (!use_momentum) return __fmaf_rn(-gv, lr, wv);
+  const float b = __fmaf_rn(gv, one_minus_damp, __fmul_rn(buf, mu));
+  buf = b;
+  return __fmaf_rn(-(nesterov ? __fmaf_rn(b, mu, gv) : b), lr, wv);
+}
+
+// Adam-family penalties (penalty.rs:63-79): g' = grad_scale*g + l1*signum(w) + 2*l2*w
+struct NkOptPenalty {
+  float l1, l2x2, grad_scale;
+  int write_back_grad;
+};
+
+__device__ __forceinline__ float nk_signum_f32(float w) {  // f32::signum: 1.0 for +0.0, -1.0 for -0.0, NaN for NaN
+  return w != w ? w : copysignf(1.f, w);
+}
+
+__device__ __forceinline__ float nk_opt_grad(const NkOptPenalty& c, float g, float wv) {
+  float gv = g * c.grad_scale;
+  if (c.l1 != 0.f) gv += c.l1 * nk_signum_f32(wv);
+  gv += c.l2x2 * wv;
+  return gv;
+}
+
+// adam/mod.rs:150-166, amsgrad/mod.rs:177-200; `max_sq` is read and written only when `ams`
+__device__ __forceinline__ float nk_adam_update(float wv, float gv, float& exp_avg, float& exp_avg_sq, bool ams,
+                                                float& max_sq, float beta1, float beta2, float sqrt_bc2,
+                                                float step_size, float eps) {
+  const float m = exp_avg * beta1 + gv * (1.f - beta1);
+  const float v = exp_avg_sq * beta2 + gv * gv * (1.f - beta2);
+  exp_avg = m;
+  exp_avg_sq = v;
+  float vv = v;
+  if (ams) {  // AMSGrad: running maximum of the second moment
+    vv = fmaxf(max_sq, v);
+    max_sq = vv;
+  }
+  wv -= m / ((sqrtf(vv) / sqrt_bc2) + eps) * step_size;
+  return wv;
+}
+
+// rmsprop/mod.rs:193-300: the four (centered, momentum) variants
+__device__ __forceinline__ float nk_rmsprop_update(float wv, float gv, float& square_avg, bool centered,
+                                                   float& grad_avg, bool momentum_on, float& buf, float lr,
+                                                   float alpha, float eps, float momentum) {
+  const float sq = square_avg * alpha + gv * gv * (1.f - alpha);
+  square_avg = sq;
+  float denom;
+  if (centered) {
+    const float ga = grad_avg * alpha + gv * (1.f - alpha);
+    grad_avg = ga;
+    denom = sqrtf(sq + (-ga * ga)) + eps;
+  } else {
+    denom = sqrtf(sq) + eps;
+  }
+  if (momentum_on) {
+    const float b = buf * momentum + gv / denom;
+    buf = b;
+    wv -= b * lr;
+  } else {
+    wv -= gv / denom * lr;
+  }
+  return wv;
+}
+
+// adagrad/mod.rs:113-140
+__device__ __forceinline__ float nk_adagrad_update(float wv, float gv, float& grad_sq, float clr, float eps) {
+  const float s = grad_sq + gv * gv;
+  grad_sq = s;
+  wv -= gv / (sqrtf(s) + eps) * clr;
+  return wv;
+}
 
 // a named namespace: kernel symbol names stay the same from build to build (torch.profiler traces)
 namespace nk_optim_multi {
@@ -164,7 +250,7 @@ __global__ void __launch_bounds__(kThreads) nk_optim_multi_kernel(const __grid_c
   }
 }
 
-// step += 1 and the per-step scalars, each operation rounded on its own in the host's order (nk_optim.cu)
+// step += 1 and the per-step scalars, each operation rounded on its own in f32
 __global__ void nk_optim_prologue_kernel(nk_optim_hyper* h, int kind, float beta1, float beta2, float lr_decay) {
   const int64_t step = h->step + 1;
   h->step = step;
@@ -314,7 +400,7 @@ int nk_multi_sgd_step(nk_ctx* ctx, int count, void* const* w, void* const* g, in
   a.nesterov = nesterov;
   a.has[0] = momentum > FLT_EPSILON;  // `.filter(|val| *val > f32::EPSILON)`, sgd/mod.rs:202
   a.pen.grad_scale = grad_scale;
-  a.pen.write_back_grad = (a.sgd_l2x2 == 0.f && grad_scale == 1.f) ? 0 : write_back_grad;  // as nk_sgd_step
+  a.pen.write_back_grad = (a.sgd_l2x2 == 0.f && grad_scale == 1.f) ? 0 : write_back_grad;  // g' = g: nothing to write
   void* const* st[3] = {momentum_buf, nullptr, nullptr};
   return multi_step<SGD>(ctx, "nk_multi_sgd_step", count, w, g, w_dtype, g_dtype, st, master, n, hyper, a);
 }
@@ -345,7 +431,7 @@ int nk_multi_rmsprop_step(nk_ctx* ctx, int count, void* const* w, void* const* g
   a.pen = NkOptPenalty{l1, 2.f * l2, grad_scale, write_back_grad};
   a.has[0] = 1;
   a.has[1] = grad_avg != nullptr;
-  a.has[2] = momentum_buf != nullptr && momentum > FLT_EPSILON;  // rmsprop/mod.rs:213-216, as nk_rmsprop_step
+  a.has[2] = momentum_buf != nullptr && momentum > FLT_EPSILON;  // rmsprop/mod.rs:213-216
   void* const* st[3] = {square_avg, grad_avg, momentum_buf};
   return multi_step<RMSPROP>(ctx, "nk_multi_rmsprop_step", count, w, g, w_dtype, g_dtype, st, master, n, hyper, a);
 }

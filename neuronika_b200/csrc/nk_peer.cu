@@ -13,7 +13,7 @@
 //      nk_reduce_bcast, nk_peer_barrier -- is kept);
 //   3. nk_peer_allreduce_small: biases and other small tensors, one single-CTA kernel through peer memory, issued the
 //      moment the gradient is final;
-//   4. then the ordinary nk_sgd_step on every replica.
+//   4. then the ordinary optimizer step (nk_multi_sgd_step) on every replica.
 // Memory that peers touch comes from nk_ipc_alloc (plain cudaMalloc: CUDA IPC cannot export pool memory) and is
 // mapped into the other processes with nk_ipc_export / nk_ipc_open.
 #include "nk_internal.cuh"

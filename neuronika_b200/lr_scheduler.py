@@ -16,12 +16,13 @@ lr_scheduler/mod.rs:16-17; its code scales each scheduler's private copy instead
 wins -- SURVEY.md 8-c defect 10).  With one scheduler both give the same values.  get_last_lr() is the lr before the
 last step and get_current_lr() the lr after it.
 
-On a default optimizer the scheduler runs on the host in np.float32 and calls set_lr.  On a capturable optimizer
-(`capturable=True`) its state lives on the device (nk_lr_sched) and step() launches a one-thread kernel that rewrites
-the optimizer's device lr, so a captured step advances the schedule on every replay; the other methods read and write
-the device state synchronously and raise NkError while capturing.  The device cannot call a Python closure, so
-MultiplicativeLR and LambdaLR take `horizon`: lr_fn(1..horizon) is evaluated into a device table at construction, and a
-step past the horizon leaves lr unchanged and makes the next read of the scheduler raise NkError."""
+On an optim.Optimizer the scheduler's state lives on the device (nk_lr_sched) and step() launches a one-thread kernel
+that rewrites the optimizer's device lr, so a captured step advances the schedule on every replay; the other methods
+read and write the device state synchronously and raise NkError while capturing.  The device cannot call a Python
+closure, so MultiplicativeLR and LambdaLR run there only when given `horizon`: lr_fn(1..horizon) is evaluated into a
+device table at construction, and a step past the horizon leaves lr unchanged and makes the next read of the scheduler
+raise NkError.  Without `horizon`, or on any other object with get_lr / set_lr, the scheduler runs on the host in
+np.float32 and calls set_lr; inside a capture that call raises NkError."""
 from __future__ import annotations
 
 import ctypes as C
@@ -40,27 +41,27 @@ class _Scheduler:
     kind = None
 
     def __init__(self, optimizer, gamma=1.0, step_size=1, milestones=(), lr_fn=None, horizon=None):
-        from .optim import CapturableOptimizer
+        from .optim import Optimizer
         self.optimizer = optimizer
         self._lr_fn = lr_fn
-        self._device = isinstance(optimizer, CapturableOptimizer)
+        closure = self.kind in (L.NK_LR_MULTIPLICATIVE, L.NK_LR_LAMBDA)
+        self._device = isinstance(optimizer, Optimizer) and (horizon is not None or not closure)
         lr = _f32(optimizer.get_lr())
-        # host state (the device copy is the truth on a capturable optimizer)
+        # host state (the device copy is the truth in device mode)
         self._epoch, self._gamma, self._step_size = 0, _f32(gamma), int(step_size)
         self._milestones = [int(m) for m in milestones]
         self._last, self._current, self._initial = _f32(0.0), lr, lr
         if not self._device:
             return
         if optimizer.hyper_ptr is None:
-            raise L.NkError(-1, "a capturable optimizer's scheduler needs the optimizer's device block: register the "
-                                "parameters first")
+            raise L.NkError(-1, "a scheduler needs the optimizer's device block: register the parameters first")
         self._dev = optimizer._hyper.device
         self._block = CuArray(self._dev, (C.sizeof(L.LrSched) // 4,), F32)
         self._table = None
-        if self.kind in (L.NK_LR_MULTIPLICATIVE, L.NK_LR_LAMBDA):
-            if horizon is None or int(horizon) < 1:
-                raise ValueError("a closure-based scheduler on a capturable optimizer needs horizon >= 1: lr_fn(1..horizon) "
-                                 "is tabulated on the device")
+        if closure:
+            if int(horizon) < 1:
+                raise ValueError("a closure-based scheduler's horizon must be >= 1: lr_fn(1..horizon) is tabulated on "
+                                 "the device")
             self._table = CuArray(self._dev, (int(horizon),), F32)
             self._table.copy_from(np.array([_f32(lr_fn(t)) for t in range(1, int(horizon) + 1)], dtype=np.float32))
         elif self.kind == L.NK_LR_MULTI_STEP:

@@ -262,16 +262,6 @@ def conv2d_bwd_kernel(dw: CuArray, g: CuArray, x: CuArray, stride=(1, 1), dilati
     return dw
 
 
-# ---------------------------------------------------------------- sgd
-def sgd_step(w: CuArray, g: CuArray, lr, l2=0.0, momentum=0.0, dampening=0.0, nesterov=False,
-             buf: CuArray | None = None, master: CuArray | None = None, grad_scale=1.0, write_back_grad=True):
-    dev = w.device
-    _ck(lib.nk_sgd_step(dev.ctx, w.ptr, w.dtype, g.ptr, g.dtype, buf.ptr if buf is not None else None,
-                        master.ptr if master is not None else None, w.size, float(lr), float(l2), float(momentum),
-                        float(dampening), int(nesterov), float(grad_scale), int(write_back_grad)), dev)
-    return w
-
-
 # ---------------------------------------------------------------- 8-f: elementwise family
 BIN = {"add": L.NK_BIN_ADD, "sub": L.NK_BIN_SUB, "mul": L.NK_BIN_MUL, "div": L.NK_BIN_DIV}
 UN = {"neg": L.NK_UN_NEG, "exp": L.NK_UN_EXP, "ln": L.NK_UN_LN, "sqrt": L.NK_UN_SQRT, "sigmoid": L.NK_UN_SIGMOID,

@@ -1,11 +1,8 @@
 """Optimizer registry and optimizers: the mirror of neuronika-optim (optimizer.rs:4-104, sgd/mod.rs:11-236,
-adam/mod.rs, amsgrad/mod.rs, rmsprop/mod.rs, adagrad/mod.rs, penalty.rs:2-79).  Every `optimize()` is ONE fused kernel
-over the parameter (nk_sgd_step / nk_adam_step / nk_rmsprop_step / nk_adagrad_step); optimizer state lives on the
-device in f32.
-
-`capturable=True` on any optimizer's `.new(...)` keeps lr and the step count in device memory instead (nk_optim_hyper)
-and updates every registered parameter with one multi-tensor launch per 64 tensors of one (data, gradient) dtype pair
-(nkg_multi_*_step), so a captured step advances the step count, and sees lr changes, on every replay."""
+adam/mod.rs, amsgrad/mod.rs, rmsprop/mod.rs, adagrad/mod.rs, penalty.rs:2-79).  Optimizer state lives on the device
+in f32, and so do lr and the step count (nk_optim_hyper).  step() updates every registered parameter with one fused
+multi-tensor launch per 64 tensors of one (data, gradient) dtype pair (nkg_multi_*_step), so a captured step advances
+the step count, and sees lr changes, on every replay."""
 from __future__ import annotations
 
 import ctypes as C
@@ -53,40 +50,16 @@ def _l1_l2(penalty):
 
 
 class Optimizer:
-    """`Optimizer<T>`: register / step / zero_grad / get_lr / set_lr (optimizer.rs:33-95)."""
+    """`Optimizer<T>`: register / step / zero_grad / get_lr / set_lr (optimizer.rs:33-95).  lr and the step count live
+    in a device block that the first register() allocates; step() launches (Adam, AMSGrad, Adagrad) the one-thread
+    prologue that advances the step count, then one update launch per 64 tensors per (data, gradient) dtype pair.  Every
+    other hyperparameter is a kernel argument: a captured step keeps the values it was captured with.  get_lr / set_lr
+    read and write the device block (synchronously; NkError while capturing).  All parameters must be registered before
+    the first step, since the step count is shared."""
 
     def __init__(self, status):
         self.status = status
         self.params = []
-
-    def get_lr(self) -> float:
-        return self.status.lr
-
-    def set_lr(self, lr: float) -> None:
-        self.status.lr = float(lr)
-
-    def register(self, variable: V.VarDiff) -> None:
-        self.params.append(self.status.into_param(variable))
-
-    def step(self) -> None:
-        for p in self.params:
-            p.optimize()
-
-    def zero_grad(self) -> None:
-        for p in self.params:
-            p.zero_grad()
-
-
-class CapturableOptimizer(Optimizer):
-    """An optimizer built with `capturable=True`.  lr and the step count live in a device block that the first
-    register() allocates; step() launches (Adam, AMSGrad, Adagrad) the one-thread prologue that advances the step count,
-    then one update launch per 64 tensors per (data, gradient) dtype pair.  Every other hyperparameter is a kernel
-    argument: a captured step keeps the values it was captured with.  get_lr / set_lr read and write the device block
-    (synchronously; NkError while capturing).  All parameters must be registered before the first step, since the step
-    count is shared."""
-
-    def __init__(self, status):
-        super().__init__(status)
         self._hyper = None
         self._stepped = False
 
@@ -127,10 +100,10 @@ class CapturableOptimizer(Optimizer):
                 raise
         else:
             if variable.device is not self._hyper.device:
-                raise L.NkError(-1, "register: a capturable optimizer's parameters share one device")
+                raise L.NkError(-1, "register: an optimizer's parameters share one device")
             self._read()                                  # refused while capturing, like every host access
             if self._stepped:
-                raise L.NkError(-1, "register: a capturable optimizer counts steps for all its parameters together; "
+                raise L.NkError(-1, "register: an optimizer counts steps for all its parameters together; "
                                 "register every parameter before the first step()")
         self.params.append(self.status.into_param(variable))
 
@@ -139,9 +112,9 @@ class CapturableOptimizer(Optimizer):
             self.status.multi_step(self.params, self._hyper.ptr)
             self._stepped = True
 
-
-def _optimizer(status) -> Optimizer:
-    return CapturableOptimizer(status) if status.capturable else Optimizer(status)
+    def zero_grad(self) -> None:
+        for p in self.params:
+            p.zero_grad()
 
 
 def _ptrs(arrays):
@@ -171,14 +144,6 @@ class _SGDParam:
         if not use_mom:
             self.buffer = None
 
-    def optimize(self) -> None:
-        s = self.status
-        self.prepare()
-        V._ck(V.lib.nkg_sgd_step(self.variable._h, self.buffer.ptr if self.buffer is not None else None,
-                                 self.master.ptr if self.master is not None else None, float(s.lr),
-                                 float(s.penalty.lambda_), float(s.momentum or 0.0), float(s.dampening or 0.0),
-                                 int(bool(s.nesterov)), float(s.grad_scale)))
-
     def zero_grad(self) -> None:
         self.variable.zero_grad()
 
@@ -188,8 +153,7 @@ class StochasticGD:
     same argument validation.  `grad_scale` (1/world_size under data parallel) and `master_weights`
     (f32 master copy of bf16 parameters, kept as optimizer state) are additions."""
 
-    def __init__(self, lr, penalty, momentum, dampening, nesterov, grad_scale=1.0, master_weights=False,
-                 capturable=False):
+    def __init__(self, lr, penalty, momentum, dampening, nesterov, grad_scale=1.0, master_weights=False):
         if momentum is None:
             assert dampening is None and not nesterov, \
                 "Dampening and Nesterov momentum flag should be enabled together with momentum."
@@ -197,11 +161,10 @@ class StochasticGD:
             assert 0.0 <= dampening <= 1.0, f"Dampening value should be between 0.0 and 1.0, got: {dampening}"
         self.lr, self.penalty, self.momentum, self.dampening, self.nesterov = float(lr), penalty, momentum, dampening, nesterov
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
-        self.capturable = bool(capturable)
 
     @staticmethod
     def new(lr, penalty=None, momentum=None, dampening=None, nesterov=False, **kw) -> Optimizer:
-        return _optimizer(StochasticGD(lr, penalty or NoPenalty(), momentum, dampening, nesterov, **kw))
+        return Optimizer(StochasticGD(lr, penalty or NoPenalty(), momentum, dampening, nesterov, **kw))
 
     def into_param(self, variable: V.VarDiff) -> _SGDParam:
         return _SGDParam(variable, self)
@@ -220,10 +183,6 @@ def _state(variable: V.VarDiff) -> CuArray:
     return CuArray(variable.device, variable.shape, F32)          # zero-filled, like Array::zeros(raw_dim)
 
 
-def _ptr(a):
-    return a.ptr if a is not None else None
-
-
 class _MasterMixin:
     def _init_master(self, variable, status):
         self.master = None
@@ -235,18 +194,10 @@ class _AdamParam(_MasterMixin):
     """AdamParam / AMSGradParam (adam/mod.rs:113-175, amsgrad/mod.rs:136-210)."""
 
     def __init__(self, variable, status):
-        self.variable, self.status, self.step = variable, status, 0
+        self.variable = variable
         self.exp_avg, self.exp_avg_sq = _state(variable), _state(variable)
         self.max_exp_avg_sq = _state(variable) if status.amsgrad else None
         self._init_master(variable, status)
-
-    def optimize(self) -> None:
-        s = self.status
-        self.step += 1
-        l1, l2 = _l1_l2(s.penalty)
-        V._ck(V.lib.nkg_adam_step(self.variable._h, self.exp_avg.ptr, self.exp_avg_sq.ptr, _ptr(self.max_exp_avg_sq),
-                                  _ptr(self.master), self.step, float(s.lr), float(s.beta1), float(s.beta2),
-                                  float(s.eps), l1, l2, float(s.grad_scale)))
 
     def zero_grad(self) -> None:
         self.variable.zero_grad()
@@ -256,14 +207,13 @@ class Adam:
     """`Adam::new(lr, beta1, beta2, penalty, eps)` (adam/mod.rs:43-60)."""
     amsgrad = False
 
-    def __init__(self, lr, beta1, beta2, penalty, eps, grad_scale=1.0, master_weights=False, capturable=False):
+    def __init__(self, lr, beta1, beta2, penalty, eps, grad_scale=1.0, master_weights=False):
         self.lr, self.beta1, self.beta2, self.penalty, self.eps = float(lr), float(beta1), float(beta2), penalty, float(eps)
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
-        self.capturable = bool(capturable)
 
     @classmethod
     def new(cls, lr, beta1=0.9, beta2=0.999, penalty=None, eps=1e-8, **kw) -> Optimizer:
-        return _optimizer(cls(lr, beta1, beta2, penalty or NoPenalty(), eps, **kw))
+        return Optimizer(cls(lr, beta1, beta2, penalty or NoPenalty(), eps, **kw))
 
     def into_param(self, variable):
         return _AdamParam(variable, self)
@@ -304,14 +254,6 @@ class _RMSPropParam(_MasterMixin):
         if not s.centered:
             self.grad_avg = None
 
-    def optimize(self) -> None:
-        s = self.status
-        self.prepare()
-        l1, l2 = _l1_l2(s.penalty)
-        V._ck(V.lib.nkg_rmsprop_step(self.variable._h, self.square_avg.ptr, _ptr(self.grad_avg), _ptr(self.buffer),
-                                     _ptr(self.master), float(s.lr), float(s.alpha if s.alpha is not None else 0.0),
-                                     float(s.eps), float(s.momentum or 0.0), l1, l2, float(s.grad_scale)))
-
     def zero_grad(self) -> None:
         self.variable.zero_grad()
 
@@ -319,18 +261,16 @@ class _RMSPropParam(_MasterMixin):
 class RMSProp:
     """`RMSProp::new(lr, penalty, alpha, momentum, centered, eps)` (rmsprop/mod.rs:67-100), same validation."""
 
-    def __init__(self, lr, penalty, alpha, momentum, centered, eps, grad_scale=1.0, master_weights=False,
-                 capturable=False):
+    def __init__(self, lr, penalty, alpha, momentum, centered, eps, grad_scale=1.0, master_weights=False):
         if alpha is not None:
             assert 0.0 <= alpha <= 1.0, f"Dampening value should be between 0.0 and 1.0, got: {alpha}"
         self.lr, self.penalty, self.alpha, self.momentum = float(lr), penalty, alpha, momentum
         self.centered, self.eps = bool(centered), float(eps)
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
-        self.capturable = bool(capturable)
 
     @staticmethod
     def new(lr, penalty=None, alpha=0.99, momentum=None, centered=False, eps=1e-8, **kw) -> Optimizer:
-        return _optimizer(RMSProp(lr, penalty or NoPenalty(), alpha, momentum, centered, eps, **kw))
+        return Optimizer(RMSProp(lr, penalty or NoPenalty(), alpha, momentum, centered, eps, **kw))
 
     def into_param(self, variable):
         return _RMSPropParam(variable, self)
@@ -350,16 +290,9 @@ class _AdagradParam(_MasterMixin):
     """AdagradParam (adagrad/mod.rs:96-145)."""
 
     def __init__(self, variable, status):
-        self.variable, self.status, self.step = variable, status, 0
+        self.variable = variable
         self.grad_sq = _state(variable)
         self._init_master(variable, status)
-
-    def optimize(self) -> None:
-        s = self.status
-        self.step += 1
-        l1, l2 = _l1_l2(s.penalty)
-        V._ck(V.lib.nkg_adagrad_step(self.variable._h, self.grad_sq.ptr, _ptr(self.master), self.step, float(s.lr),
-                                     float(s.lr_decay), float(s.eps), l1, l2, float(s.grad_scale)))
 
     def zero_grad(self) -> None:
         self.variable.zero_grad()
@@ -368,14 +301,13 @@ class _AdagradParam(_MasterMixin):
 class Adagrad:
     """`Adagrad::new(lr, lr_decay, penalty, eps)` (adagrad/mod.rs:50-63)."""
 
-    def __init__(self, lr, lr_decay, penalty, eps, grad_scale=1.0, master_weights=False, capturable=False):
+    def __init__(self, lr, lr_decay, penalty, eps, grad_scale=1.0, master_weights=False):
         self.lr, self.lr_decay, self.penalty, self.eps = float(lr), float(lr_decay), penalty, float(eps)
         self.grad_scale, self.master_weights = float(grad_scale), bool(master_weights)
-        self.capturable = bool(capturable)
 
     @staticmethod
     def new(lr, lr_decay=0.0, penalty=None, eps=1e-10, **kw) -> Optimizer:
-        return _optimizer(Adagrad(lr, lr_decay, penalty or NoPenalty(), eps, **kw))
+        return Optimizer(Adagrad(lr, lr_decay, penalty or NoPenalty(), eps, **kw))
 
     def into_param(self, variable):
         return _AdagradParam(variable, self)

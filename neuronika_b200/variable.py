@@ -53,7 +53,6 @@ _G = {
     "nkg_pad": (i32, [vp, i64, i64, f32, pvp]),
     "nkg_convolution": (i32, [vp, vp, i64, i64, i64, i64, i64, pvp]),
     "nkg_flatten": (i32, [vp, pvp]),
-    "nkg_sgd_step": (i32, [vp, vp, vp, f32, f32, f32, f32, i32, f32]),
     "nkg_sub": (i32, [vp, vp, pvp]),
     "nkg_mul": (i32, [vp, vp, pvp]),
     "nkg_div": (i32, [vp, vp, pvp]),
@@ -74,9 +73,6 @@ _G = {
     "nkg_vv": (i32, [vp, vp, pvp]),
     "nkg_convolution_nd": (i32, [vp, vp, i32, pi64, pi64, i64, pvp]),
     "nkg_conv_layer": (i32, [vp, vp, vp, i32, pi64, i32, f32, pi64, pi64, pvp]),
-    "nkg_adam_step": (i32, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, f32]),
-    "nkg_rmsprop_step": (i32, [vp, vp, vp, vp, vp, f32, f32, f32, f32, f32, f32, f32]),
-    "nkg_adagrad_step": (i32, [vp, vp, vp, i64, f32, f32, f32, f32, f32, f32]),
     "nkg_multi_sgd_step": (i32, [pvp, i32, pvp, pvp, vp, f32, f32, f32, i32, f32]),
     "nkg_multi_adam_step": (i32, [pvp, i32, pvp, pvp, pvp, pvp, vp, f32, f32, f32, f32, f32, f32]),
     "nkg_multi_rmsprop_step": (i32, [pvp, i32, pvp, pvp, pvp, pvp, vp, f32, f32, f32, f32, f32, f32]),

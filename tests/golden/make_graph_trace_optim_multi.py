@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Write graph_trace_optim_multi.json: the kernel-ABI call traces of the capturable optimizers' graph entry points
+"""Write graph_trace_optim_multi.json: the kernel-ABI call traces of the optimizers' graph entry points
 (the scenarios of tests/test_graph_trace_optim_multi.py), recorded as make_graph_trace.py records the graph's.
 
     python tests/golden/make_graph_trace_optim_multi.py"""

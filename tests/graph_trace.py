@@ -52,6 +52,10 @@ HOST_ARRAYS = {
     ("nk_cat_bwd", "dxs"): "count", ("nk_cat_bwd", "dx_dtypes"): "count", ("nk_cat_bwd", "betas"): "count",
     ("nk_cat_bwd", "lens"): "count",
     ("nk_gemm_rs", "slots"): "world",
+    **{(f, p): "count" for f in ("nk_multi_sgd_step", "nk_multi_adam_step", "nk_multi_rmsprop_step",
+                                 "nk_multi_adagrad_step")
+       for p in ("w", "g", "n", "master", "momentum_buf", "exp_avg", "exp_avg_sq", "max_exp_avg_sq", "square_avg",
+                 "grad_avg", "grad_sq")},
 }
 
 
@@ -461,27 +465,17 @@ class Var:
     def cat(self, others, axis): return self.g.join("nkg_cat", [self, *others], axis)
     def stack(self, others, axis): return self.g.join("nkg_stack", [self, *others], axis)
 
-    # ---- optimizers (state buffers are scenario-owned memory)
+    # ---- SGD through the multi-tensor entry point (state buffers and the nk_optim_hyper block are scenario-owned
+    # memory; lr lives in the block)
     def sgd(self, momentum=0.9, master=False):
         n = self.numel()
+
+        def one(p):
+            return (C.c_void_p * 1)(p) if p else None
         buf = self.g.ext(n * 4) if momentum else None
-        self.g.ck(self.g.lib.nkg_sgd_step(self.h, buf, self.g.ext(n * 4) if master else None, 0.1, 0.01, momentum,
-                                          0.0, 1 if momentum else 0, 0.5))
-
-    def adam(self, amsgrad=False, master=False):
-        n, e = self.numel(), self.g.ext
-        self.g.ck(self.g.lib.nkg_adam_step(self.h, e(n * 4), e(n * 4), e(n * 4) if amsgrad else None,
-                                           e(n * 4) if master else None, 3, 1e-3, 0.9, 0.999, 1e-8, 0.0, 0.01, 1.0))
-
-    def rmsprop(self, centered=True, momentum=0.5):
-        n, e = self.numel(), self.g.ext
-        self.g.ck(self.g.lib.nkg_rmsprop_step(self.h, e(n * 4), e(n * 4) if centered else None,
-                                              e(n * 4) if momentum else None, None, 1e-2, 0.99, 1e-8, momentum,
-                                              0.001, 0.0, 1.0))
-
-    def adagrad(self):
-        n, e = self.numel(), self.g.ext
-        self.g.ck(self.g.lib.nkg_adagrad_step(self.h, e(n * 4), None, 2, 1e-2, 0.1, 1e-10, 0.0, 0.0, 0.25))
+        mst = self.g.ext(n * 4) if master else None
+        self.g.ck(self.g.lib.nkg_multi_sgd_step((C.c_void_p * 1)(self.h.value), 1, one(buf), one(mst), self.g.ext(24),
+                                                0.01, momentum, 0.0, 1 if momentum else 0, 0.5))
 
     def numel(self):
         n = self.g.lib.nkg_ndim(self.h)
@@ -672,12 +666,12 @@ def _mlp(g, level, steps=1, keep_pre=False, hooks=None, rs=None, zero=True, fail
 
 for _level in range(4):
     SCENARIOS["mlp/level%d" % _level] = lambda g, _l=_level: _mlp(g, _l)
-SCENARIOS["mlp/level1_two_steps"] = lambda g: _mlp(g, 1, steps=2)
+SCENARIOS["mlp/level1_two_multi_sgd_steps"] = lambda g: _mlp(g, 1, steps=2)
 SCENARIOS["mlp/level2_pre_activation_held"] = lambda g: _mlp(g, 2, keep_pre=True)
 SCENARIOS["mlp/level3_colsum_unsupported"] = lambda g: _mlp(g, 3, fail="nk_gemm_relu_bwd_colsum")
 SCENARIOS["mlp/level2_hooks_row_chunks"] = lambda g: _mlp(g, 2, hooks=2)
 SCENARIOS["mlp/level2_rs_push"] = lambda g: _mlp(g, 2, rs=1)
-SCENARIOS["mlp/level2_rs_accumulating"] = lambda g: _mlp(g, 2, steps=2, rs=2, zero=False)
+SCENARIOS["mlp/level2_rs_accumulating_multi_sgd"] = lambda g: _mlp(g, 2, steps=2, rs=2, zero=False)
 SCENARIOS["mlp/level1_rs_and_hooks"] = lambda g: _mlp(g, 1, rs=2, hooks=2)
 
 
@@ -898,28 +892,6 @@ def _lstm_both(g):
                                                                                              (4 * H,), (4 * H,))])
     c2.describe("var c")
     h2.forward()
-
-
-@scenario("optimizers")
-def _optimizers(g):
-    x = g.leaf((3, 6), BF16)
-    w = g.param((4, 6), BF16, F32)
-    s = x.mm_t(w).sum()
-    s.forward()
-    s.backward(1.0)
-    w.sgd(momentum=0.9, master=True)
-    w.sgd(momentum=0.0)
-    w.adam(amsgrad=True, master=True)
-    w.adam()
-    w.rmsprop()
-    w.rmsprop(centered=False, momentum=0.0)
-    w.adagrad()
-    w.zero_grad()
-    w.sgd(momentum=0.0)
-    g.expect_error(x.sgd)
-    g.expect_error(x.adam)
-    g.expect_error(x.rmsprop)
-    g.expect_error(x.adagrad)
 
 
 @scenario("errors")

@@ -390,16 +390,27 @@ def test_pad_bit_exact(nk, dev, O):
         assert np.array_equal(dx.as_ndarray(), r(want))
 
 
-def test_sgd(nk, dev, O):
-    from neuronika_b200 import ops
+def test_multi_sgd_step(nk, dev, O):
+    """nk_multi_sgd_step on one tensor, lr from an nk_optim_hyper block"""
+    import ctypes as C
+    from neuronika_b200 import _lib as L
+    from neuronika_b200.device import CuArray
     rng = np.random.default_rng(8)
+    hyper = CuArray(dev, (C.sizeof(L.OptimHyper) // 4,), nk.F32)
+    L.check(L.lib.nk_optim_hyper_set(dev.ctx, hyper.ptr, C.byref(L.OptimHyper(lr=0.01))), dev.ctx)
+
+    def one(a):
+        return None if a is None else (C.c_void_p * 1)(a.ptr.value)
     for kw in ({}, {"l2": 0.01}, {"momentum": 0.9}, {"momentum": 0.9, "dampening": 0.1, "nesterov": True, "l2": 0.001}):
         w, g = rnd(rng, (1000,)), rnd(rng, (1000,))
         dw_, dg_ = dev.from_ndarray(w), dev.from_ndarray(g)
         buf = dev.zeros((1000,)) if "momentum" in kw else None
         ww, gg, bb = w.copy(), g.copy(), None
         for _ in range(3):
-            ops.sgd_step(dw_, dg_, 0.01, buf=buf, **kw)
+            L.check(L.lib.nk_multi_sgd_step(dev.ctx, 1, one(dw_), one(dg_), dw_.dtype, dg_.dtype, one(buf), None,
+                                            (C.c_int64 * 1)(1000), hyper.ptr, kw.get("l2", 0.0),
+                                            kw.get("momentum", 0.0), kw.get("dampening", 0.0),
+                                            int(kw.get("nesterov", False)), 1.0, 1), dev.ctx)
             bb = O.sgd_step(ww, gg, 0.01, buf=bb, **kw)
         assert np.allclose(dw_.as_ndarray(), ww, rtol=1e-6, atol=1e-7), kw
         assert np.allclose(dg_.as_ndarray(), gg, rtol=1e-6, atol=1e-7), kw   # reference mutates grad (+= penalty)

@@ -1,8 +1,8 @@
-"""The kernel-ABI calls of the capturable optimizers' graph entry points (nkg_multi_*_step), over the recording stub of
+"""The kernel-ABI calls of the optimizers' graph entry points (nkg_multi_*_step), over the recording stub of
 tests/graph_trace.py, so their structure is checked without a GPU: every parameter's gradient is materialised in
-parameter order, Adam and Adagrad launch their prologue once, and each (data, gradient) dtype group is updated by one
-nk_multi_*_step call per 64 tensors, in parameter order; a parameter that is not differentiable fails the call before
-anything is launched.  The traces are pinned in tests/golden/graph_trace_optim_multi.json
+parameter order (a zeroed one is cleared first), Adam and Adagrad launch their prologue once, and each (data, gradient)
+dtype group is updated by one nk_multi_*_step call per 64 tensors, in parameter order; a parameter that is not
+differentiable fails the call before anything is launched.  Every variant runs once on a single parameter too.  The traces are pinned in tests/golden/graph_trace_optim_multi.json
 (tests/golden/make_graph_trace_optim_multi.py)."""
 import ctypes as C
 import json
@@ -15,12 +15,7 @@ import graph_trace as T
 
 BF16, F32 = T.BF16, T.F32
 PER_LAUNCH = 64
-MULTI = ("nk_multi_sgd_step", "nk_multi_adam_step", "nk_multi_rmsprop_step", "nk_multi_adagrad_step")
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "graph_trace_optim_multi.json")
-# the tensor tables are host arrays of `count` entries
-T.HOST_ARRAYS.update({(f, p): "count" for f in MULTI
-                      for p in ("w", "g", "n", "master", "momentum_buf", "exp_avg", "exp_avg_sq", "max_exp_avg_sq",
-                                "square_avg", "grad_avg", "grad_sq")})
 
 
 def _arr(ptrs):
@@ -87,8 +82,34 @@ def not_differentiable(g):
         g.expect_error(lambda: g.ck(getattr(g.lib, name)(hs, 3, *args)))
 
 
+def one_parameter_variants(g):
+    """each optimizer variant on one parameter after a backward pass, then a step after zero_grad(), whose deferred
+    zero fill the step materialises"""
+    x = g.leaf((3, 6), BF16)
+    w = g.param((4, 6), BF16, F32)
+    s = x.mm_t(w).sum()
+    s.forward()
+    s.backward(1.0)
+    spec = [(24, BF16, F32)]
+    hs, hyper = _arr([w.h.value]), g.ext(24)
+    g.ck(g.lib.nkg_multi_sgd_step(hs, 1, _states(g, spec), _masters(g, spec), hyper, 0.01, 0.9, 0.0, 1, 0.5))
+    g.ck(g.lib.nkg_multi_sgd_step(hs, 1, None, None, hyper, 0.01, 0.0, 0.0, 0, 0.5))
+    g.ck(g.lib.nkg_multi_adam_step(hs, 1, _states(g, spec), _states(g, spec), _states(g, spec), _masters(g, spec), hyper,
+                                   0.9, 0.999, 1e-8, 0.0, 0.01, 1.0))
+    g.ck(g.lib.nkg_multi_adam_step(hs, 1, _states(g, spec), _states(g, spec), None, None, hyper, 0.9, 0.999, 1e-8, 0.0,
+                                   0.01, 1.0))
+    g.ck(g.lib.nkg_multi_rmsprop_step(hs, 1, _states(g, spec), _states(g, spec), _states(g, spec), None, hyper, 0.99,
+                                      1e-8, 0.5, 0.001, 0.0, 1.0))
+    g.ck(g.lib.nkg_multi_rmsprop_step(hs, 1, _states(g, spec), None, None, None, hyper, 0.99, 1e-8, 0.0, 0.001, 0.0,
+                                      1.0))
+    g.ck(g.lib.nkg_multi_adagrad_step(hs, 1, _states(g, spec), None, hyper, 0.1, 1e-10, 0.0, 0.0, 0.25))
+    w.zero_grad()
+    g.ck(g.lib.nkg_multi_sgd_step(hs, 1, None, None, hyper, 0.01, 0.0, 0.0, 0, 0.5))
+
+
 SCENARIOS = {"adam_mixed": adam_mixed, "sgd_pairs": sgd_pairs, "rmsprop_pairs": rmsprop_pairs,
-             "adagrad_twice": adagrad_twice, "not_differentiable": not_differentiable}
+             "adagrad_twice": adagrad_twice, "not_differentiable": not_differentiable,
+             "one_parameter_variants": one_parameter_variants}
 
 
 @pytest.fixture(scope="module")

@@ -1,7 +1,7 @@
 """The learning-rate scheduler oracle (oracle/lr_scheduler.py) against the reference's five scheduler tests
 (tests/golden/lr_scheduler.json, transcribed from neuronika-optim/src/lr_scheduler/*/test.rs), chaining against the
-composed product, and the package's host-side schedulers (the ones a default optimizer uses) against the oracle on a
-stub optimizer.  No GPU needed."""
+composed product, and the package's host-side schedulers (the mode a closure scheduler without `horizon` runs in)
+against the oracle on a stub optimizer.  No GPU needed."""
 import json
 import os
 import re
@@ -107,7 +107,7 @@ def test_set_current_epoch_moves_the_schedule():
 
 # ------------------------------------------------------------------------- the package's host-side schedulers
 class StubOptimizer:
-    """what a scheduler needs of a default optimizer: get_lr / set_lr of a Python float"""
+    """what a host-side scheduler needs of an optimizer: get_lr / set_lr of a Python float"""
 
     def __init__(self, lr):
         self.lr = float(lr)
