@@ -344,6 +344,30 @@ int nk_layer_norm_bwd(nk_ctx* ctx, void* dx, int dx_dtype, float dx_beta, void* 
                       void* db, int db_dtype, float db_beta, const void* g, int g_dtype, const void* x, int dtype,
                       int64_t rows, int64_t cols, const void* w, const float* save_mean, const float* save_rstd);
 
+/* ---- embedding: a gather of weight rows and its deterministic gradient, torch's semantics (csrc/nk_embedding.cu) ----
+ * w / dw are (v, e) row-major, y / g are (n, e).  `ids` holds n ids stored as floats, like nll's class ids: ids_dtype
+ * NK_F32, or NK_BF16 when v <= 256 (otherwise NK_ERR_INVALID_ARG); v <= 2^24, where every integer is exact in f32.  A
+ * value x is a valid id when 0 <= x < v (tested on the float: NaN, negative and x >= v are invalid) and its id is
+ * trunc(x).  An INVALID ID gives a zero output row and adds nothing to any gradient row, as nll ignores an out-of-range
+ * target.
+ * nk_embedding_fwd: y[p, :] = w[id(p), :], a bit-exact copy in `dtype`, 16-byte accesses when e * esize and both bases
+ *   allow them.  One launch; n = 0 or e = 0 launches nothing.
+ * nk_embedding_bwd: dw[r, :] = beta*dw[r, :] + sum of g[p, :] over the positions p with id(p) == r, r != padding_idx
+ *   (-1: none).  dw and g are each f32 or bf16.  No float atomics: the positions are grouped by id with a stable LSD
+ *   radix sort (ceil(bits(v + 1) / 8) passes of 8 bits), so each row's positions ascend; the sorted sequence is cut into
+ *   slots of 32 entries, each row's run inside a slot is summed sequentially in f32, and a row spanning several slots
+ *   adds its runs' partials in slot order.  The sum is rounded once into dw's type, the product beta*dw and the add
+ *   rounded separately (beta = 0 never reads dw).  Rows without a valid position: untouched when beta == 1, else
+ *   beta*dw (zeros for beta = 0), so a beta = 0 call writes every row.  The order depends on the ids alone: repeated
+ *   calls give identical bits.  Nothing syncs with the host (launch sizes depend on n, v and e only).
+ *   Launches: 3 per sort pass, then 1 (slots), then 1 more when beta != 1 or n > 32; with n = 0 only the last, and
+ *   none at all when beta == 1.  Workspace (nk_alloc_uninit, freed stream-ordered): 16n + 1024*ceil(n/4096) bytes for
+ *   the sort, plus 8*ceil(n/32)*e bytes of f32 partials when n > 32.  n >= 2^31 is NK_ERR_UNSUPPORTED. */
+int nk_embedding_fwd(nk_ctx* ctx, void* y, const void* w, const void* ids, int ids_dtype, int64_t n, int64_t v, int64_t e,
+                     int dtype);
+int nk_embedding_bwd(nk_ctx* ctx, void* dw, int dw_dtype, const void* ids, int ids_dtype, const void* g, int g_dtype,
+                     int64_t n, int64_t v, int64_t e, int64_t padding_idx, float beta);
+
 /* ---- matrix-vector / vector-matrix / vector-vector products (8-f rank 3; csrc/nk_gemv.cu) ----
  * A is (rows, cols) row-major.  trans = 0: y[rows] = beta*y + A.x[cols] (MatrixVectorMul::forward,
  * matrix_vector_mul/mod.rs:32-40; vm dv, vector_matrix_mul/mod.rs:64-72); trans = 1: y[cols] = beta*y +

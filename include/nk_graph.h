@@ -184,6 +184,15 @@ int nkg_gru_layer(nkg_var* input, nkg_var* hidden, nkg_var* weight_ih, nkg_var* 
 int nkg_cat(nkg_var* const* vars, int count, int axis, nkg_var** out);
 int nkg_stack(nkg_var* const* vars, int count, int axis, nkg_var** out);
 int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out);
+/* nkg_reshape: the operand under `shape` (ndim <= NK_MAX_DIMS entries, same element count).  A view like nkg_flatten
+ * and nkg_unsqueeze: no kernel, no node, and the gradient is the operand's. */
+int nkg_reshape(nkg_var* a, int ndim, const int64_t* shape, nkg_var** out);
+/* nkg_embedding: out = weight[ids], torch's embedding (nk_b200.h nk_embedding_*): weight (v, e) f32 or bf16; ids of
+ * any shape holding float ids (f32, or bf16 when v <= 256), never differentiable; out has shape ids.shape + (e,) and
+ * the weight's dtype, and is differentiable iff the weight is.  An invalid id gives a zero row and no gradient;
+ * padding_idx (-1: none, else 0 <= padding_idx < v) gets no gradient either.  ONE forward and ONE backward node; the
+ * backward writes the weight's gradient. */
+int nkg_embedding(nkg_var* ids, nkg_var* weight, int64_t padding_idx, nkg_var** out);
 
 /* ---- the other criteria and dropout (var.rs:375-521, vardiff.rs:418-583) ----
  * nkg_mae / nkg_bce / nkg_bce_with_logits / nkg_kldiv take (input, target, reduction) like nkg_mse_loss: same shape and

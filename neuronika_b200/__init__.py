@@ -10,9 +10,10 @@ from . import ops
 from . import variable, nn, optim
 from .variable import (Reduction, Status, Var, VarDiff, cat, from_ndarray, full, ones, rand, set_fusion, stack, zeros)
 from .nn import (AdaptiveAvgPool1d, AdaptiveAvgPool2d, AdaptiveAvgPool3d, AvgPool1d, AvgPool2d, AvgPool3d, BatchNorm1d,
-                 BatchNorm2d, BatchNorm3d, LayerNorm, MaxPool1d, MaxPool2d, MaxPool3d)
+                 BatchNorm2d, BatchNorm3d, Embedding, LayerNorm, MaxPool1d, MaxPool2d, MaxPool3d)
 
 __all__ = ["Device", "CuArray", "F32", "BF16", "NkError", "ops", "variable", "nn", "optim", "Var", "VarDiff",
            "Reduction", "Status", "zeros", "ones", "full", "rand", "from_ndarray", "set_fusion", "cat", "stack",
            "MaxPool1d", "MaxPool2d", "MaxPool3d", "AvgPool1d", "AvgPool2d", "AvgPool3d", "AdaptiveAvgPool1d",
-           "AdaptiveAvgPool2d", "AdaptiveAvgPool3d", "BatchNorm1d", "BatchNorm2d", "BatchNorm3d", "LayerNorm"]
+           "AdaptiveAvgPool2d", "AdaptiveAvgPool3d", "BatchNorm1d", "BatchNorm2d", "BatchNorm3d", "LayerNorm",
+           "Embedding"]

@@ -990,6 +990,39 @@ struct PoolBackward : Backward {
   }
 };
 
+// ------------------------------------------------------------------------------- embedding (nk_embedding.cu)
+// out = weight[ids]: ids of any shape (float ids, never differentiable), weight (v, e); the backward writes only the
+// weight's gradient.
+struct Embedding : Forward {
+  TensorP ids, weight, data;
+  Embedding(nk_ctx* c, TensorP i, TensorP w, TensorP d)
+      : Forward(c), ids(std::move(i)), weight(std::move(w)), data(std::move(d)) {}
+  const char* name() const override { return "Embedding"; }
+  void forward() override {
+    const Shape& ws = weight->shape;
+    ck(ctx, nk_embedding_fwd(ctx, data->wptr(), weight->rptr(), ids->rptr(), ids->dtype, ids->n(), ws[0], ws[1],
+                             weight->dtype));
+  }
+};
+struct EmbeddingBackward : Backward {
+  TensorP ids;
+  GradientP weight_grad;
+  int64_t padding_idx;
+  EmbeddingBackward(nk_ctx* c, GradientP g, TensorP i, GradientP wg, int64_t pad)
+      : Backward(c, std::move(g)), ids(std::move(i)), weight_grad(std::move(wg)), padding_idx(pad) {}
+  const char* name() const override { return "EmbeddingBackward"; }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&weight_grad}); }
+  void backward() override {
+    const Shape& ws = weight_grad->shape;
+    const void* g = gradient->get();
+    accumulate(ctx, weight_grad, [&](void* d, float beta) {  // one call for every (dw, g) dtype pair
+      ck(ctx, nk_embedding_bwd(ctx, d, weight_grad->dtype, ids->rptr(), ids->dtype, g, gradient->dtype, ids->n(), ws[0],
+                               ws[1], padding_idx, beta));
+    });
+    grad_written(weight_grad);
+  }
+};
+
 // ------------------------------------------------------------------------------- batch norm / layer norm (nk_norm.cu)
 // Which statistics the last BatchNorm forward normalized with; its backward applies exactly that, whatever the status
 // says by then (as DropoutState).
@@ -2881,6 +2914,48 @@ int nkg_unsqueeze(nkg_var* a, int axis, nkg_var** out) {
     if (s.size() + 1 > NK_MAX_DIMS) fail(NK_ERR_INVALID_ARG, "unsqueeze: the result would have more than %d dimensions", NK_MAX_DIMS);
     s.insert(s.begin() + axis, 1);
     *out = view_of(a, s);
+  });
+}
+
+int nkg_reshape(nkg_var* a, int ndim, const int64_t* shape, nkg_var** out) {
+  return guard([&] {
+    not_null({a, out}, "reshape");
+    if (ndim < 0 || ndim > NK_MAX_DIMS || (ndim > 0 && !shape))
+      fail(NK_ERR_INVALID_ARG, "reshape: 0 to %d dimensions (got %d)", NK_MAX_DIMS, ndim);
+    const Shape s(shape, shape + ndim);
+    for (int64_t d : s)
+      if (d < 0) fail(NK_ERR_INVALID_ARG, "reshape: negative dimension %lld", (long long)d);
+    if (numel(s) != a->data->n())
+      fail(NK_ERR_INVALID_ARG, "shape '%s' is invalid for input of size %lld", shape_str(s).c_str(),
+           (long long)a->data->n());
+    *out = view_of(a, s);
+  });
+}
+
+int nkg_embedding(nkg_var* ids, nkg_var* weight, int64_t padding_idx, nkg_var** out) {
+  return guard([&] {
+    static const char* who = "embedding";
+    not_null({ids, weight, out}, who);
+    if (ids->ctx != weight->ctx) fail(NK_ERR_INVALID_ARG, "%s: operands live on different devices", who);
+    const Shape& ws = weight->data->shape;
+    if (ws.size() != 2) fail(NK_ERR_INVALID_ARG, "%s: weight must be 2-D (v, e), got %s", who, shape_str(ws).c_str());
+    if (ids->diff()) fail(NK_ERR_INVALID_ARG, "%s: ids must not be differentiable", who);
+    const int64_t v = ws[0];
+    if (v > (int64_t(1) << 24)) fail(NK_ERR_INVALID_ARG, "%s: %lld rows exceed 2^24, where f32 ids are exact", who, (long long)v);
+    if (ids->data->dtype == NK_BF16 && v > 256)
+      fail(NK_ERR_INVALID_ARG, "%s: bf16 ids cannot hold ids above 256 (v = %lld); pass the ids as f32", who, (long long)v);
+    if (padding_idx < -1 || padding_idx >= v)
+      fail(NK_ERR_INVALID_ARG, "%s: padding_idx %lld outside [-1, %lld)", who, (long long)padding_idx, (long long)v);
+    Shape os = ids->data->shape;
+    if (os.size() + 1 > NK_MAX_DIMS)
+      fail(NK_ERR_INVALID_ARG, "%s: the result would have more than %d dimensions", who, NK_MAX_DIMS);
+    os.push_back(ws[1]);
+    *out = record(
+        {ids, weight}, os, weight->data->dtype,
+        [&](const TensorP& d) { return std::make_shared<Embedding>(weight->ctx, ids->data, weight->data, d); },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<EmbeddingBackward>(weight->ctx, g, ids->data, weight->grad, padding_idx);
+        });
   });
 }
 

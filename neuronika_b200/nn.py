@@ -1,6 +1,6 @@
 """Layers: the mirror of neuronika-nn's Linear, LSTMCell, GRUCell, Conv1d, Conv2d and Conv3d (neuronika-nn/src/lib.rs:
 406-916), the sequence layers LSTM and GRU over them (stacked and bidirectional like torch.nn.LSTM / GRU), and torch's
-max, average and adaptive average pooling layers and its batch and layer normalization layers."""
+max, average and adaptive average pooling layers, its batch and layer normalization layers and its embedding."""
 from __future__ import annotations
 
 import math
@@ -57,6 +57,31 @@ class Linear:
 
     def parameters(self):
         return [self.weight, self.bias]
+
+
+class Embedding:
+    """torch.nn.Embedding: weight (num_embeddings, embedding_dim) ~ N(0, 1) (`init::normal`, neuronika-nn/src/init.rs:195),
+    its padding_idx row zeroed; forward(ids) = weight[ids] with ids a non-differentiable Var of float ids (f32, or bf16
+    for num_embeddings <= 256).  A negative padding_idx counts from num_embeddings; that row gets no gradient."""
+
+    def __init__(self, device: Device, num_embeddings: int, embedding_dim: int, padding_idx=None, dtype=F32,
+                 grad_dtype=None, rng: np.random.Generator | None = None):
+        rng = rng or np.random.default_rng()
+        if padding_idx is not None:
+            if not -num_embeddings <= padding_idx < num_embeddings:
+                raise ValueError("Padding_idx must be within num_embeddings")
+            padding_idx = padding_idx % num_embeddings
+        self.padding_idx = padding_idx
+        w = rng.standard_normal((num_embeddings, embedding_dim)).astype(np.float32)
+        if padding_idx is not None:
+            w[padding_idx] = 0.0
+        self.weight = V.from_ndarray(device, w, dtype).requires_grad(grad_dtype)
+
+    def forward(self, ids: V.Var) -> V.VarDiff:
+        return V.embedding(ids, self.weight, self.padding_idx)
+
+    def parameters(self):
+        return [self.weight]
 
 
 class Conv2d:

@@ -477,6 +477,23 @@ def layer_norm_bwd(g: CuArray, x: CuArray, cols: int, save_mean: CuArray, save_r
     return dx, dw, db
 
 
+def embedding(w: CuArray, ids: CuArray, out=None) -> CuArray:
+    """y = w[ids] (nk_embedding_fwd): w (v, e); ids of any shape, f32 (or bf16 for v <= 256) ids; y ids.shape + (e,).
+    Invalid ids give zero rows."""
+    v, e = w.shape
+    out = out or CuArray(w.device, tuple(ids.shape) + (e,), w.dtype)
+    _ck(lib.nk_embedding_fwd(w.device.ctx, out.ptr, w.ptr, ids.ptr, ids.dtype, ids.size, v, e, w.dtype), w.device)
+    return out
+
+
+def embedding_bwd(dw: CuArray, ids: CuArray, g: CuArray, padding_idx=None, beta=1.0) -> CuArray:
+    """dw = beta*dw + the embedding's weight gradient (nk_embedding_bwd); padding_idx None = -1 (none)."""
+    v, e = dw.shape
+    _ck(lib.nk_embedding_bwd(dw.device.ctx, dw.ptr, dw.dtype, ids.ptr, ids.dtype, g.ptr, g.dtype, ids.size, v, e,
+                             -1 if padding_idx is None else int(padding_idx), float(beta)), dw.device)
+    return dw
+
+
 # ---------------------------------------------------------------- 8-f: mv / vm / vv
 def gemv(a: CuArray, x: CuArray, y: CuArray | None = None, trans=False, beta=0.0) -> CuArray:
     rows, cols = a.shape

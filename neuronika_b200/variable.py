@@ -89,6 +89,8 @@ _G = {
     "nkg_cat": (i32, [pvp, i32, i32, pvp]),
     "nkg_stack": (i32, [pvp, i32, i32, pvp]),
     "nkg_unsqueeze": (i32, [vp, i32, pvp]),
+    "nkg_reshape": (i32, [vp, i32, pi64, pvp]),
+    "nkg_embedding": (i32, [vp, vp, i64, pvp]),
     "nkg_mae": (i32, [vp, vp, i32, pvp]),
     "nkg_bce": (i32, [vp, vp, i32, pvp]),
     "nkg_bce_with_logits": (i32, [vp, vp, i32, pvp]),
@@ -389,6 +391,26 @@ class Var:
         (the reference records one)."""
         return self._unary(lib.nkg_unsqueeze, int(axis))
 
+    def reshape(self, *shape):
+        """torch's reshape of a contiguous tensor: the same elements under `shape` (ints or one tuple), at most one -1
+        (inferred).  A view like flatten(): no kernel and no node, and the gradient is the operand's."""
+        if len(shape) == 1 and isinstance(shape[0], (tuple, list)):
+            shape = tuple(shape[0])
+        shape = [int(s) for s in shape]
+        size = int(np.prod(self.shape, dtype=np.int64))
+        if shape.count(-1) > 1:
+            raise RuntimeError("only one dimension can be inferred")
+        if any(s < -1 for s in shape):
+            raise RuntimeError(f"invalid shape dimension {min(shape)}")
+        known = int(np.prod([s for s in shape if s != -1], dtype=np.int64))
+        if -1 in shape:
+            if known == 0 or size % known:
+                raise RuntimeError(f"shape '{shape}' is invalid for input of size {size}")
+            shape[shape.index(-1)] = size // known
+        elif known != size:
+            raise RuntimeError(f"shape '{shape}' is invalid for input of size {size}")
+        return self._unary(lib.nkg_reshape, len(shape), L.shape_arr(shape))
+
     def item(self) -> float:
         return float(self.data().reshape(()))
 
@@ -486,6 +508,24 @@ def conv_layer(input: Var, weight: Var, bias: Var | None, padding, mode: str = "
     _ck(lib.nkg_conv_layer(input._h, weight._h, bias._h if bias is not None else None, nsp, L.shape_arr(padding),
                            _pad_mode(mode), float(value), L.shape_arr(stride), L.shape_arr(dilation), C.byref(out)))
     return input._wrap(out)
+
+
+# ---- embedding (one node; see include/nk_graph.h nkg_embedding)
+def embedding(ids: Var, weight: Var, padding_idx: int | None = None):
+    """torch's F.embedding(ids, weight, padding_idx): weight (v, e), ids a non-differentiable Var of float ids (f32,
+    or bf16 for v <= 256) of any shape; the result has shape ids.shape + (e,).  Invalid ids (NaN, < 0, >= v) give zero
+    rows and no gradient; a negative padding_idx counts from v."""
+    v = weight.shape[0] if len(weight.shape) == 2 else 0
+    pad = -1
+    if padding_idx is not None:
+        pad = int(padding_idx)
+        if pad < 0:
+            pad += v
+        if not 0 <= pad < v:
+            raise ValueError("Padding_idx must be within num_embeddings")
+    out = vp()
+    _ck(lib.nkg_embedding(ids._h, weight._h, pad, C.byref(out)))
+    return weight._wrap(out)
 
 
 # ---- concatenation (neuronika-variable/src/lib.rs:258, 281)
