@@ -368,6 +368,41 @@ int nk_embedding_fwd(nk_ctx* ctx, void* y, const void* w, const void* ids, int i
 int nk_embedding_bwd(nk_ctx* ctx, void* dw, int dw_dtype, const void* ids, int ids_dtype, const void* g, int g_dtype,
                      int64_t n, int64_t v, int64_t e, int64_t padding_idx, float beta);
 
+/* ---- cross-entropy with class-index targets, torch's F.cross_entropy (csrc/nk_cross_entropy.cu) ----
+ * x is (n, c, s) row-major in `dtype` (f32 or bf16): the class axis is the middle one, s = prod(d1..dk) for an
+ * (N, C, d1, ..., dk) input and 1 for (N, C).  `target` holds n*s class ids stored as floats, like nll's: target_dtype
+ * NK_F32, or NK_BF16 when c <= 256 (otherwise NK_ERR_INVALID_ARG); 1 <= c <= 2^24.  A position is IGNORED when its id
+ * is invalid (NaN, < 0, >= c; torch raises instead) or trunc(id) == ignore_index; otherwise its class is t = trunc(id).
+ * `weight` is NULL (every weight 1) or c f32 class weights w, W = sum w.  With lse = ln sum_k exp(x_k), eps =
+ * label_smoothing in [0, 1] (otherwise NK_ERR_INVALID_ARG), a non-ignored position's loss is
+ *   l = (1 - eps)*w_t*(lse - x_t) + eps/c * sum_k w_k*(lse - x_k),
+ * and an ignored one's 0.  Sum: loss = sum l; mean (torch's): loss = sum l / sum of w_t over non-ignored positions,
+ * NaN (0/0) when every position is ignored or n = 0.
+ * nk_cross_entropy_fwd writes the device f32 scalars *loss and *denom (that denominator, whatever `mean`) and lse
+ *   (n*s f32, 0 for ignored positions), which the backward reads.  One read of x.
+ * nk_cross_entropy_bwd: with p = softmax(x) of the position and gs = *g (Sum) or *g / *denom (mean),
+ *   dx_k = beta*dx_k + gs*((1 - eps)*w_t*(p_k - [k == t]) + eps/c*(W*p_k - w_k))
+ *   in dx_dtype (f32 or bf16, independently of x), the product and the add rounded separately; beta = 0 never reads
+ *   dx; an ignored position gets beta*dx (untouched when beta == 1).  One read of x and lse, one write of dx.
+ * Layouts, chosen from the shape: s == 1 rows of <= 4096 bytes, or 4096 rows and more, a warp per row; fewer longer
+ * rows a CTA per row, or a CTA per (row, chunk) when there are fewer than 2*SMs rows of at least 65536 classes (the
+ * chunks' partial (max, sum) pairs merged in ascending chunk order); s > 1 a thread per position walking the classes
+ * with stride s.  16-byte loads of rows whenever x (and dx) are 16-byte aligned, with a scalar head and tail per row.
+ * A -inf logit (a masked class) adds nothing to the sum, wherever it falls; a NaN logit makes the position's loss NaN.  Fixed reduction orders, no float
+ * atomics: repeated calls give identical bits; nothing is synchronised with the host, so a captured step replays with
+ * new targets (and a new ignored count).
+ * Launches: forward 1 (finish only, n = 0), 2, or 3 for split rows, plus 1 for W when both weight and eps > 0;
+ * backward 1 (none for n = 0), plus the same W launch.  Workspace (nk_alloc_uninit, freed stream-ordered): forward
+ * 16 bytes per block of the main kernel (at most 8 per SM), 16 bytes per (row, chunk) for split rows, 16 for W;
+ * backward 16 bytes for W. */
+int nk_cross_entropy_fwd(nk_ctx* ctx, float* loss, float* lse, float* denom, const void* x, int dtype,
+                         const void* target, int target_dtype, const float* weight, int64_t n, int64_t c, int64_t s,
+                         int64_t ignore_index, float label_smoothing, int mean);
+int nk_cross_entropy_bwd(nk_ctx* ctx, void* dx, int dx_dtype, const void* x, int dtype, const void* target,
+                         int target_dtype, const float* weight, const float* lse, const float* denom, const float* g,
+                         int64_t n, int64_t c, int64_t s, int64_t ignore_index, float label_smoothing, int mean,
+                         float beta);
+
 /* ---- matrix-vector / vector-matrix / vector-vector products (8-f rank 3; csrc/nk_gemv.cu) ----
  * A is (rows, cols) row-major.  trans = 0: y[rows] = beta*y + A.x[cols] (MatrixVectorMul::forward,
  * matrix_vector_mul/mod.rs:32-40; vm dv, vector_matrix_mul/mod.rs:64-72); trans = 1: y[cols] = beta*y +

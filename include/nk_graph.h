@@ -193,6 +193,16 @@ int nkg_reshape(nkg_var* a, int ndim, const int64_t* shape, nkg_var** out);
  * padding_idx (-1: none, else 0 <= padding_idx < v) gets no gradient either.  ONE forward and ONE backward node; the
  * backward writes the weight's gradient. */
 int nkg_embedding(nkg_var* ids, nkg_var* weight, int64_t padding_idx, nkg_var** out);
+/* nkg_cross_entropy: torch's F.cross_entropy with class-index targets (nk_b200.h nk_cross_entropy_*): input (N, C) or
+ * (N, C, d1, ..., dk), f32 or bf16; target (N) or (N, d1, ..., dk) holding float class ids (f32, or bf16 when C <= 256),
+ * never differentiable; weight NULL or an f32 (C) tensor, never differentiable; reduction NKG_MEAN (torch's: divided by
+ * the summed weights of the non-ignored positions, NaN when there are none) or NKG_SUM; label_smoothing in [0, 1].
+ * Positions whose id equals ignore_index or is invalid (NaN, < 0, >= C) are ignored.  The result is a 0-d f32 scalar.
+ * ONE forward node, which owns the saved per-position lse and the denominator, and, for a differentiable input, ONE
+ * backward node into the input's gradient.  Invalid arguments (shapes, weight, label_smoothing, bf16 target with
+ * C > 256, devices) are NK_ERR_INVALID_ARG and record nothing. */
+int nkg_cross_entropy(nkg_var* input, nkg_var* target, nkg_var* weight, int reduction, int64_t ignore_index,
+                      float label_smoothing, nkg_var** out);
 
 /* ---- the other criteria and dropout (var.rs:375-521, vardiff.rs:418-583) ----
  * nkg_mae / nkg_bce / nkg_bce_with_logits / nkg_kldiv take (input, target, reduction) like nkg_mse_loss: same shape and

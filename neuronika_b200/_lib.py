@@ -151,6 +151,8 @@ _PROTOS = {
     "nk_layer_norm_bwd": (i32, [vp, vp, i32, f32, vp, i32, f32, vp, i32, f32, vp, i32, vp, i32, i64, i64, vp, vp, vp]),
     "nk_embedding_fwd": (i32, [vp, vp, vp, vp, i32, i64, i64, i64, i32]),
     "nk_embedding_bwd": (i32, [vp, vp, i32, vp, i32, vp, i32, i64, i64, i64, i64, f32]),
+    "nk_cross_entropy_fwd": (i32, [vp, vp, vp, vp, vp, i32, vp, i32, vp, i64, i64, i64, i64, f32, i32]),
+    "nk_cross_entropy_bwd": (i32, [vp, vp, i32, vp, i32, vp, i32, vp, vp, vp, vp, i64, i64, i64, i64, f32, i32, f32]),
     "nk_gemv": (i32, [vp, i32, i64, i64, vp, vp, f32, vp, i32, i32]),
     "nk_outer_acc": (i32, [vp, vp, i32, vp, vp, i64, i64, i32, f32]),
     "nk_dot": (i32, [vp, vp, vp, vp, sz, i32]),

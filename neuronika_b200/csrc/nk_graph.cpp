@@ -1142,6 +1142,59 @@ struct LayerNormBackward : Backward {
   }
 };
 
+// ------------------------------------------------------------------------------- cross-entropy (nk_cross_entropy.cu)
+// input (N, C, d1..dk), target (N, d1..dk) of float class ids, weight (C) f32 or NULL; neither target nor weight is
+// differentiable.  The forward node owns lse (N*S floats) and the denominator, allocated when the node is built; the
+// backward reads both.
+struct CeDims {
+  int64_t n, c, s;
+};
+static CeDims ce_dims(const Shape& xs) {
+  int64_t s = 1;
+  for (size_t i = 2; i < xs.size(); ++i) s *= xs[i];
+  return {xs[0], xs[1], s};
+}
+struct CrossEntropy : Forward {
+  TensorP input, target, weight, data, lse, denom;
+  bool mean;
+  int64_t ignore_index;
+  float label_smoothing;
+  CrossEntropy(nk_ctx* c, TensorP x, TensorP t, TensorP w, TensorP d, TensorP l, TensorP dn, bool m, int64_t ig,
+               float eps)
+      : Forward(c), input(std::move(x)), target(std::move(t)), weight(std::move(w)), data(std::move(d)),
+        lse(std::move(l)), denom(std::move(dn)), mean(m), ignore_index(ig), label_smoothing(eps) {}
+  const char* name() const override { return "CrossEntropy"; }
+  void forward() override {
+    const CeDims d = ce_dims(input->shape);
+    ck(ctx, nk_cross_entropy_fwd(ctx, (float*)data->wptr(), (float*)lse->wptr(), (float*)denom->wptr(), input->rptr(),
+                                 input->dtype, target->rptr(), target->dtype, (const float*)opt_r(weight), d.n, d.c, d.s,
+                                 ignore_index, label_smoothing, mean));
+  }
+};
+struct CrossEntropyBackward : Backward {
+  TensorP input, target, weight, lse, denom;
+  GradientP input_grad;
+  bool mean;
+  int64_t ignore_index;
+  float label_smoothing;
+  CrossEntropyBackward(nk_ctx* c, GradientP g, TensorP x, TensorP t, TensorP w, TensorP l, TensorP dn, GradientP xg,
+                       bool m, int64_t ig, float eps)
+      : Backward(c, std::move(g)), input(std::move(x)), target(std::move(t)), weight(std::move(w)), lse(std::move(l)),
+        denom(std::move(dn)), input_grad(std::move(xg)), mean(m), ignore_index(ig), label_smoothing(eps) {}
+  const char* name() const override { return "CrossEntropyBackward"; }
+  void targets(std::vector<Gradient*>& out) override { add_targets(out, {&input_grad}); }
+  void backward() override {
+    const CeDims d = ce_dims(input->shape);
+    accumulate(ctx, input_grad, [&](void* dx, float beta) {  // one call for every (dx, x) dtype pair
+      ck(ctx, nk_cross_entropy_bwd(ctx, dx, input_grad->dtype, input->rptr(), input->dtype, target->rptr(),
+                                   target->dtype, (const float*)opt_r(weight), (const float*)lse->rptr(),
+                                   (const float*)denom->rptr(), (const float*)gradient->get(), d.n, d.c, d.s,
+                                   ignore_index, label_smoothing, mean, beta));
+    });
+    grad_written(input_grad);
+  }
+};
+
 // ------------------------------------------------------------------------------- mv / vm / vv
 // matrix_vector_mul/mod.rs:11-129, vector_matrix_mul/mod.rs:11-129, vector_vector_mul/mod.rs:11-91
 struct MatVec : Forward {
@@ -2955,6 +3008,56 @@ int nkg_embedding(nkg_var* ids, nkg_var* weight, int64_t padding_idx, nkg_var** 
         [&](const TensorP& d) { return std::make_shared<Embedding>(weight->ctx, ids->data, weight->data, d); },
         [&](const TensorP&, const GradientP& g) {
           return std::make_shared<EmbeddingBackward>(weight->ctx, g, ids->data, weight->grad, padding_idx);
+        });
+  });
+}
+
+int nkg_cross_entropy(nkg_var* input, nkg_var* target, nkg_var* weight, int reduction, int64_t ignore_index,
+                      float label_smoothing, nkg_var** out) {
+  return guard([&] {
+    static const char* who = "cross_entropy";
+    not_null({input, target, out}, who);
+    if (input->ctx != target->ctx || (weight && weight->ctx != input->ctx))
+      fail(NK_ERR_INVALID_ARG, "%s: operands live on different devices", who);
+    if (reduction != NKG_MEAN && reduction != NKG_SUM) fail(NK_ERR_INVALID_ARG, "%s: unknown reduction %d", who, reduction);
+    const Shape &xs = input->data->shape, &ts = target->data->shape;
+    if (xs.size() < 2 || ts.size() + 1 != xs.size() || ts[0] != xs[0] || !std::equal(ts.begin() + 1, ts.end(), xs.begin() + 2))
+      fail(NK_ERR_INVALID_ARG, "%s: input must be (N, C, d1, ..., dk) and target (N, d1, ..., dk), got %s and %s", who,
+           shape_str(xs).c_str(), shape_str(ts).c_str());
+    const int64_t c = xs[1];
+    if (c < 1) fail(NK_ERR_INVALID_ARG, "%s: the input has no classes", who);
+    if (c > (int64_t(1) << 24))
+      fail(NK_ERR_INVALID_ARG, "%s: %lld classes exceed 2^24, where f32 class ids are exact", who, (long long)c);
+    if (target->data->dtype == NK_BF16 && c > 256)
+      fail(NK_ERR_INVALID_ARG, "%s: a bf16 target cannot hold class ids above 256 (C = %lld); pass the target as f32", who,
+           (long long)c);
+    if (target->diff()) fail(NK_ERR_INVALID_ARG, "%s: the target must not be differentiable", who);
+    if (weight) {
+      if (weight->data->dtype != NK_F32 || weight->data->shape != Shape{c})
+        fail(NK_ERR_INVALID_ARG, "%s: weight must be an f32 tensor of shape (%lld,), got %s", who, (long long)c,
+             shape_str(weight->data->shape).c_str());
+      if (weight->diff()) fail(NK_ERR_INVALID_ARG, "%s: the weight must not be differentiable", who);
+    }
+    if (!(label_smoothing >= 0.f && label_smoothing <= 1.f))
+      fail(NK_ERR_INVALID_ARG, "%s: label_smoothing must be between 0.0 and 1.0, got %g", who, double(label_smoothing));
+    const CeDims d = ce_dims(xs);
+    auto lse = std::make_shared<Tensor>(input->ctx, Shape{d.n * d.s}, NK_F32);
+    auto denom = std::make_shared<Tensor>(input->ctx, Shape{}, NK_F32);
+    lse->wptr();
+    denom->wptr();
+    TensorP w = weight ? weight->data : nullptr;
+    std::vector<nkg_var*> operands{input, target};
+    if (weight) operands.push_back(weight);
+    const bool mean = reduction == NKG_MEAN;
+    *out = record(
+        operands, Shape{}, NK_F32,
+        [&](const TensorP& dt) {
+          return std::make_shared<CrossEntropy>(input->ctx, input->data, target->data, w, dt, lse, denom, mean,
+                                                ignore_index, label_smoothing);
+        },
+        [&](const TensorP&, const GradientP& g) {
+          return std::make_shared<CrossEntropyBackward>(input->ctx, g, input->data, target->data, w, lse, denom,
+                                                        input->grad, mean, ignore_index, label_smoothing);
         });
   });
 }

@@ -152,6 +152,39 @@ def nll_bwd(dlogp, target, g, mean=True, beta=1.0):
     return dlogp
 
 
+def _ce_dims(x: CuArray):
+    s = 1
+    for d in x.shape[2:]:
+        s *= int(d)
+    return x.shape[0], x.shape[1], s
+
+
+def cross_entropy(x: CuArray, target: CuArray, weight: CuArray | None = None, mean=True, ignore_index=-100,
+                  label_smoothing=0.0, out=None, lse=None, denom=None):
+    """torch's F.cross_entropy with class-index targets (nk_cross_entropy_fwd): x (N, C, d1, ...), target (N, d1, ...)
+    float class ids, weight f32 (C,) or None.  Returns (loss, lse, denom): the 0-d f32 loss, the per-position f32 lse
+    (N*S) and the 0-d f32 denominator that cross_entropy_bwd reads."""
+    n, c, s = _ce_dims(x)
+    out = out or CuArray(x.device, (), F32)
+    lse = lse or CuArray(x.device, (n * s,), F32)
+    denom = denom or CuArray(x.device, (), F32)
+    _ck(lib.nk_cross_entropy_fwd(x.device.ctx, out.ptr, lse.ptr, denom.ptr, x.ptr, x.dtype, target.ptr, target.dtype,
+                                 weight.ptr if weight is not None else None, n, c, s, int(ignore_index),
+                                 float(label_smoothing), int(mean)), x.device)
+    return out, lse, denom
+
+
+def cross_entropy_bwd(dx: CuArray, x: CuArray, target: CuArray, lse: CuArray, denom: CuArray, g: CuArray,
+                      weight: CuArray | None = None, mean=True, ignore_index=-100, label_smoothing=0.0,
+                      beta=1.0) -> CuArray:
+    """dx = beta*dx + the cross-entropy gradient times the seed g (nk_cross_entropy_bwd), dx in its own element type"""
+    n, c, s = _ce_dims(x)
+    _ck(lib.nk_cross_entropy_bwd(x.device.ctx, dx.ptr, dx.dtype, x.ptr, x.dtype, target.ptr, target.dtype,
+                                 weight.ptr if weight is not None else None, lse.ptr, denom.ptr, g.ptr, n, c, s,
+                                 int(ignore_index), float(label_smoothing), int(mean), float(beta)), x.device)
+    return dx
+
+
 _CRITERIA = {"mae": (lib.nk_mae_fwd, lib.nk_mae_bwd), "bce": (lib.nk_bce_fwd, lib.nk_bce_bwd),
              "bce_with_logits": (lib.nk_bce_with_logits_fwd, lib.nk_bce_with_logits_bwd),
              "kldiv": (lib.nk_kldiv_fwd, lib.nk_kldiv_bwd)}

@@ -91,6 +91,7 @@ _G = {
     "nkg_unsqueeze": (i32, [vp, i32, pvp]),
     "nkg_reshape": (i32, [vp, i32, pi64, pvp]),
     "nkg_embedding": (i32, [vp, vp, i64, pvp]),
+    "nkg_cross_entropy": (i32, [vp, vp, vp, i32, i64, f32, pvp]),
     "nkg_mae": (i32, [vp, vp, i32, pvp]),
     "nkg_bce": (i32, [vp, vp, i32, pvp]),
     "nkg_bce_with_logits": (i32, [vp, vp, i32, pvp]),
@@ -274,6 +275,18 @@ class Var:
     def mean(self): return self._unary(lib.nkg_mean)
     def mse_loss(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_mse_loss, target, int(reduction))
     def nll_loss(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_nll_loss, target, int(reduction))
+
+    def cross_entropy(self, target, reduction=Reduction.Mean, weight=None, ignore_index: int = -100,
+                      label_smoothing: float = 0.0):
+        """torch's F.cross_entropy with class-index targets, as ONE node: the receiver holds the logits, (N, C) or
+        (N, C, d1, ..., dk); `target` (N) or (N, d1, ..., dk) holds float class ids (f32, or bf16 for C <= 256) and is
+        not differentiable; `weight` is None or an f32 (C,) Var.  Positions whose id equals `ignore_index`, or is not a
+        class (NaN, < 0, >= C: torch raises there), are left out.  Mean divides by the summed weights of the other
+        positions, as torch does (nll_loss's Mean divides by N); it is NaN when every position is ignored."""
+        out = vp()
+        _ck(lib.nkg_cross_entropy(self._h, target._h, weight._h if weight is not None else None, int(reduction),
+                                  int(ignore_index), float(label_smoothing), C.byref(out)))
+        return self._wrap(out)
     def mae(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_mae, target, int(reduction))
     def bce(self, target, reduction=Reduction.Mean): return self._binary(lib.nkg_bce, target, int(reduction))
 
