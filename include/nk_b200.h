@@ -642,6 +642,33 @@ int nk_lr_sched_set(nk_ctx* ctx, nk_lr_sched* sched, const nk_lr_sched* host);
 int nk_lr_sched_get(nk_ctx* ctx, const nk_lr_sched* sched, nk_lr_sched* host);
 int nk_lr_sched_step(nk_ctx* ctx, nk_lr_sched* sched, nk_optim_hyper* hyper);
 
+/* ---- gradient clipping, torch.nn.utils' get_total_norm / clip_grads_with_norm_ / clip_grad_value_ (csrc/nk_optim_multi.cu)
+ * Each call takes `count` gradients of any dtypes (g_dtype[i]: NK_F32 or NK_BF16) with n[i] elements each.  Inside a
+ * call the tensors are grouped by dtype in order of first appearance, and each group takes one launch per
+ * NK_OPTIM_TENSORS_PER_LAUNCH tensors (a group of empty tensors takes none); the table travels in the kernel parameters.
+ * A tensor takes 4-element (16-byte f32, 8-byte bf16) accesses when its base allows them, element accesses otherwise.
+ * Nothing is read back to the host, so every call can be captured.  Invalid arguments (a bad dtype, a negative n, a
+ * NULL pointer where elements are, a bad norm_type) fail with NK_ERR_INVALID_ARG before anything is launched.
+ *   nk_grad_norm: with k = grad_scale and v = f32(k*g) (one f32 multiply) over every element of every tensor,
+ *     p = 2: sqrt(sum v^2)   p = 1: sum |v|   p = +inf: max |v|   other p > 0: (sum |v|^p)^(1/p)  (powf only here),
+ *     written to *total (device, one f32).  A NaN element makes the total NaN (for p = +inf too), an infinite one
+ *     makes it +inf; count = 0 gives 0.  norm_type <= 0, -inf and NaN are rejected.  Launches: one per group, each
+ *     CTA writing one f32 partial (its elements folded in a fixed tree) to a workspace from nk_alloc_uninit that is
+ *     freed stream-ordered, then one CTA that merges every partial in a fixed order in double, takes the root in
+ *     double and rounds once to f32.  No float atomics: repeated calls give identical bits.
+ *   nk_grad_scale_by_norm: torch's coefficient, each operation rounded on its own in f32,
+ *     c = (1 / (*total + 1e-6)) * max_norm (torch evaluates max_norm / x as x.reciprocal() * max_norm), c = 1 when
+ *     c > 1 (a compare: a NaN total gives c = NaN); then g = dtype(f32(g) * c), one rounding.  When c == 1 nothing is
+ *     written (g * 1 == g).  One launch per group.
+ *   nk_grad_clamp: b = clip_value / grad_scale in f32; g = min(max(g, -b), b), clamp_min first as torch applies them, a
+ *     NaN element stays NaN; clip_value < 0 makes every other element b.  One launch per group. */
+int nk_grad_norm(nk_ctx* ctx, int count, const void* const* g, const int* g_dtype, const int64_t* n, float norm_type,
+                 float grad_scale, float* total);
+int nk_grad_scale_by_norm(nk_ctx* ctx, int count, void* const* g, const int* g_dtype, const int64_t* n,
+                          const float* total, float max_norm);
+int nk_grad_clamp(nk_ctx* ctx, int count, void* const* g, const int* g_dtype, const int64_t* n, float clip_value,
+                  float grad_scale);
+
 /* ---- NCCL all-reduce behind the ABI (SURVEY.md 8-b, 8-e; csrc/nk_comm.cu) ----
  * The context owns the communicator; libnccl.so.2 is bound at run time (dlopen), so the library loads
  * without it.  Rank 0 creates the 128-byte id and ships it to the others by any means; every rank then

@@ -271,6 +271,18 @@ int nkg_multi_rmsprop_step(nkg_var* const* params, int count, void* const* squar
 int nkg_multi_adagrad_step(nkg_var* const* params, int count, void* const* grad_sq, void* const* master,
                            nk_optim_hyper* hyper, float lr_decay, float eps, float l1, float l2, float grad_scale);
 
+/* ---- gradient clipping over many leaves (torch.nn.utils; nk_b200.h nk_grad_norm / nk_grad_scale_by_norm /
+ * nk_grad_clamp).  Every parameter must be differentiable and on one context, or the call fails before anything is
+ * materialised or launched.  Then each gradient is materialised in parameter order (a pending zero_grad() gets its
+ * zero fill) and ONE ABI call takes the tables in parameter order.  nkg_grad_norm writes the total norm of the
+ * gradients times grad_scale to `total` (device, one f32) and needs at least one parameter (the total's device);
+ * nkg_clip_grads_with_norm scales them by torch's coefficient from max_norm and that total; nkg_clip_grad_value clamps
+ * them to +-clip_value / grad_scale.  The two writing calls mark the gradients nonzero; with count = 0 they do
+ * nothing. */
+int nkg_grad_norm(nkg_var* const* params, int count, float norm_type, float grad_scale, float* total);
+int nkg_clip_grads_with_norm(nkg_var* const* params, int count, float max_norm, const float* total);
+int nkg_clip_grad_value(nkg_var* const* params, int count, float clip_value, float grad_scale);
+
 #ifdef __cplusplus
 }
 #endif

@@ -176,6 +176,9 @@ _PROTOS = {
     "nk_lr_sched_set": (i32, [vp, vp, vp]),
     "nk_lr_sched_get": (i32, [vp, vp, vp]),
     "nk_lr_sched_step": (i32, [vp, vp, vp]),
+    "nk_grad_norm": (i32, [vp, i32, pvp, C.POINTER(i32), pi64, f32, f32, vp]),
+    "nk_grad_scale_by_norm": (i32, [vp, i32, pvp, C.POINTER(i32), pi64, vp, f32]),
+    "nk_grad_clamp": (i32, [vp, i32, pvp, C.POINTER(i32), pi64, f32, f32]),
     "nk_comm_unique_id": (i32, [vp, vp]),
     "nk_comm_init_rank": (i32, [vp, i32, i32, vp]),
     "nk_comm_destroy": (i32, [vp]),

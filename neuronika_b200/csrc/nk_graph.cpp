@@ -3241,17 +3241,24 @@ struct MultiGroup {
   std::vector<int> idx;
 };
 
-template <typename Launch>
-void multi_step(const char* who, nkg_var* const* params, int count, void* const* const* states, int nstates,
-                void* const* master, Launch launch) {
+// the context of `count` differentiable parameters on one device (nullptr for none); fails before anything else runs
+nk_ctx* params_ctx(const char* who, nkg_var* const* params, int count) {
   if (count < 0 || (count > 0 && !params)) fail(NK_ERR_INVALID_ARG, "%s: bad parameter array", who);
   for (int i = 0; i < count; ++i)
     if (!params[i] || !params[i]->diff())
       fail(NK_ERR_INVALID_ARG, "%s: parameter %d is not differentiable", who, i);
-  if (count == 0) return;
+  if (count == 0) return nullptr;
   nk_ctx* ctx = params[0]->ctx;
   for (int i = 1; i < count; ++i)
     if (params[i]->ctx != ctx) fail(NK_ERR_INVALID_ARG, "%s: parameters on different devices", who);
+  return ctx;
+}
+
+template <typename Launch>
+void multi_step(const char* who, nkg_var* const* params, int count, void* const* const* states, int nstates,
+                void* const* master, Launch launch) {
+  nk_ctx* ctx = params_ctx(who, params, count);
+  if (count == 0) return;
   std::vector<void*> w(count), g(count);
   std::vector<int64_t> n(count);
   std::vector<Gradient*> roots(count);
@@ -3288,6 +3295,28 @@ void multi_step(const char* who, nkg_var* const* params, int count, void* const*
                      cn.data()));
     }
   for (Gradient* r : roots) r->is_zero = false;
+}
+
+// Gradient clipping: the parameters are checked as multi_step checks them, then each gradient is materialised in
+// parameter order and `launch` makes one ABI call with the tables in parameter order.  The writing calls mark the
+// gradients nonzero afterwards.
+template <typename Launch>
+void grad_call(const char* who, nkg_var* const* params, int count, bool writes, Launch launch) {
+  nk_ctx* ctx = params_ctx(who, params, count);
+  if (count == 0) return;
+  std::vector<void*> g(count);
+  std::vector<int> dt(count);
+  std::vector<int64_t> n(count);
+  std::vector<Gradient*> roots(count);
+  for (int i = 0; i < count; ++i) {
+    roots[i] = params[i]->grad->root();
+    g[i] = params[i]->grad->get();
+    dt[i] = roots[i]->dtype;
+    n[i] = roots[i]->n();
+  }
+  ck(ctx, launch(ctx, g.data(), dt.data(), n.data()));
+  if (writes)
+    for (Gradient* r : roots) r->is_zero = false;
 }
 }  // namespace
 }  // extern "C++"
@@ -3352,6 +3381,33 @@ int nkg_multi_adagrad_step(nkg_var* const* params, int count, void* const* grad_
                  }
                  return nk_multi_adagrad_step(ctx, c, w, g, wd, gd, st[0], m, n, hyper, eps, l1, l2, grad_scale, 1);
                });
+  });
+}
+
+int nkg_grad_norm(nkg_var* const* params, int count, float norm_type, float grad_scale, float* total) {
+  return guard([&] {
+    if (count == 0) fail(NK_ERR_INVALID_ARG, "grad_norm: no parameters, so no device for the total");
+    if (!(norm_type > 0.f)) fail(NK_ERR_INVALID_ARG, "grad_norm: norm_type must be > 0 or +inf (got %g)", norm_type);
+    grad_call("grad_norm", params, count, false, [&](nk_ctx* ctx, void* const* g, const int* dt, const int64_t* n) {
+      return nk_grad_norm(ctx, count, g, dt, n, norm_type, grad_scale, total);
+    });
+  });
+}
+
+int nkg_clip_grads_with_norm(nkg_var* const* params, int count, float max_norm, const float* total) {
+  return guard([&] {
+    grad_call("clip_grads_with_norm", params, count, true,
+              [&](nk_ctx* ctx, void* const* g, const int* dt, const int64_t* n) {
+                return nk_grad_scale_by_norm(ctx, count, g, dt, n, total, max_norm);
+              });
+  });
+}
+
+int nkg_clip_grad_value(nkg_var* const* params, int count, float clip_value, float grad_scale) {
+  return guard([&] {
+    grad_call("clip_grad_value", params, count, true, [&](nk_ctx* ctx, void* const* g, const int* dt, const int64_t* n) {
+      return nk_grad_clamp(ctx, count, g, dt, n, clip_value, grad_scale);
+    });
   });
 }
 

@@ -38,6 +38,7 @@ class Device:
             raise L.NkError(rc, L.last_error(None))
         self.ctx = ctx
         self.index = int(device)
+        self.capturing = False          # inside `with capture()`: host reads of device results are refused
         if stream is not None:
             self.set_stream(stream)
 
@@ -174,9 +175,11 @@ class _Capture:
 
     def __enter__(self):
         L.check(L.lib.nk_capture_begin(self.device.ctx, self.arena_bytes), self.device.ctx)
+        self.device.capturing = True
         return self
 
     def __exit__(self, exc_type, exc, tb):
+        self.device.capturing = False
         h = C.c_void_p()
         rc = L.lib.nk_capture_end(self.device.ctx, C.byref(h))
         if exc_type is None:

@@ -743,3 +743,38 @@ def cat_bwd(dxs, g: CuArray, axis: int, betas, lens=None):
     _ck(lib.nk_cat_bwd(g.device.ctx, ptrs, dts, (L.f32 * n)(*[float(b) for b in betas]), g.ptr, g.dtype,
                        (L.i64 * n)(*lens), n, outer, inner), g.device)
     return dxs
+
+
+# ---------------------------------------------------------------- gradient clipping (csrc/nk_optim_multi.cu)
+def _grad_tables(grads):
+    n = len(grads)
+    return ((L.vp * n)(*[g.ptr.value for g in grads]), (L.i32 * n)(*[g.dtype for g in grads]),
+            (L.i64 * n)(*[g.size for g in grads]))
+
+
+def grad_norm(grads, norm_type=2.0, grad_scale=1.0, out: CuArray | None = None) -> CuArray:
+    """out = the norm_type-norm of grad_scale * (every element of every array), one f32 on the device (0 for no arrays;
+    then `out` gives the device)."""
+    grads = list(grads)
+    dev = out.device if out is not None else grads[0].device
+    out = out if out is not None else CuArray(dev, (), F32)
+    _ck(lib.nk_grad_norm(dev.ctx, len(grads), *_grad_tables(grads), float(norm_type), float(grad_scale), out.ptr), dev)
+    return out
+
+
+def grad_scale_by_norm(grads, total: CuArray, max_norm: float):
+    """every array *= min(max_norm / (total + 1e-6), 1), torch's clip coefficient from the device scalar `total`"""
+    grads = list(grads)
+    _ck(lib.nk_grad_scale_by_norm(total.device.ctx, len(grads), *_grad_tables(grads), total.ptr, float(max_norm)),
+        total.device)
+    return grads
+
+
+def grad_clamp(grads, clip_value: float, grad_scale=1.0):
+    """every array = clamp(array, -b, b), b = clip_value / grad_scale in f32"""
+    grads = list(grads)
+    if not grads:
+        return grads
+    dev = grads[0].device
+    _ck(lib.nk_grad_clamp(dev.ctx, len(grads), *_grad_tables(grads), float(clip_value), float(grad_scale)), dev)
+    return grads

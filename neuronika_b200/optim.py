@@ -319,4 +319,60 @@ class Adagrad:
                                            float(self.eps), l1, l2, float(self.grad_scale)))
 
 
+# ------------------------------------------------------------------------------------------- gradient clipping
+# torch.nn.utils' clipping functions over the gradients of VarDiff parameters, on the device's stream: one multi-tensor
+# launch per 64 gradients of one dtype (nkg_grad_norm / nkg_clip_grads_with_norm / nkg_clip_grad_value), nothing read
+# back to the host unless error_if_nonfinite.  `grad_scale` is the optimizer's (1/world under data parallel): the norm
+# is that of grad_scale * g, and the coefficient multiplies the raw buffers.
+def _grad_params(params):
+    return [params] if isinstance(params, V.VarDiff) else list(params)
+
+
+def _var_handles(ps):
+    return (C.c_void_p * len(ps))(*[p._h.value for p in ps])
+
+
+def get_total_norm(params, norm_type=2.0, error_if_nonfinite=False, grad_scale=1.0) -> CuArray:
+    """The norm of all the gradients together as one vector (a 0-d f32 CuArray on the device; reading it is the
+    caller's sync).  norm_type > 0 or inf.  With error_if_nonfinite the total is read back, which a capture refuses."""
+    ps = _grad_params(params)
+    if not ps:
+        raise ValueError("get_total_norm: no parameters, so no device to hold the total")
+    dev = ps[0].device
+    if error_if_nonfinite and dev.capturing:
+        raise L.NkError(-5, "get_total_norm: error_if_nonfinite reads the total back, which a captured step could not "
+                            "repeat on replay")
+    total = CuArray(dev, (), F32)
+    V._ck(V.lib.nkg_grad_norm(_var_handles(ps), len(ps), float(norm_type), float(grad_scale), total.ptr))
+    if error_if_nonfinite and not np.isfinite(total.as_ndarray()):
+        raise RuntimeError(
+            f"The total norm of order {float(norm_type)} for gradients from `parameters` is non-finite, so it cannot be "
+            "clipped. To disable this error and scale the gradients by the non-finite norm anyway, set "
+            "`error_if_nonfinite=False`")
+    return total
+
+
+def clip_grads_with_norm_(params, max_norm, total_norm: CuArray) -> None:
+    """grad *= min(max_norm / (total_norm + 1e-6), 1), with total_norm a 0-d f32 CuArray on the device."""
+    ps = _grad_params(params)
+    if total_norm.dtype != F32 or total_norm.size != 1:
+        raise ValueError("clip_grads_with_norm_: total_norm must be one f32 element")
+    V._ck(V.lib.nkg_clip_grads_with_norm(_var_handles(ps), len(ps), float(max_norm), total_norm.ptr))
+
+
+def clip_grad_norm_(params, max_norm, norm_type=2.0, error_if_nonfinite=False, grad_scale=1.0) -> CuArray:
+    """get_total_norm, then clip_grads_with_norm_; returns the total.  Inside a capture the total lives in the graph's
+    arena and every replay rewrites it."""
+    ps = _grad_params(params)
+    total = get_total_norm(ps, norm_type, error_if_nonfinite, grad_scale)
+    clip_grads_with_norm_(ps, max_norm, total)
+    return total
+
+
+def clip_grad_value_(params, clip_value, grad_scale=1.0) -> None:
+    """grad = clamp(grad, -b, b) with b = clip_value / grad_scale (in f32)."""
+    ps = _grad_params(params)
+    V._ck(V.lib.nkg_clip_grad_value(_var_handles(ps), len(ps), float(clip_value), float(grad_scale)))
+
+
 from . import lr_scheduler  # noqa: E402  (optim.lr_scheduler, as in the reference)

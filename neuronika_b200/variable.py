@@ -77,6 +77,9 @@ _G = {
     "nkg_multi_adam_step": (i32, [pvp, i32, pvp, pvp, pvp, pvp, vp, f32, f32, f32, f32, f32, f32]),
     "nkg_multi_rmsprop_step": (i32, [pvp, i32, pvp, pvp, pvp, pvp, vp, f32, f32, f32, f32, f32, f32]),
     "nkg_multi_adagrad_step": (i32, [pvp, i32, pvp, pvp, vp, f32, f32, f32, f32, f32]),
+    "nkg_grad_norm": (i32, [pvp, i32, f32, f32, vp]),
+    "nkg_clip_grads_with_norm": (i32, [pvp, i32, f32, vp]),
+    "nkg_clip_grad_value": (i32, [pvp, i32, f32, f32]),
     "nkg_set_grad_hook": (i32, [vp, vp, vp, i32]),
     "nkg_set_grad_rs": (i32, [vp, i32, i32, pvp, vp, vp]),
     "nkg_chunks": (i32, [vp, i32, pi64, i32, pvp, C.POINTER(i32)]),
