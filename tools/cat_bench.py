@@ -24,47 +24,12 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from gemm_sweep import Clock  # noqa: E402
-
-HBM_GBPS = 3350.0
-
-
-def timed(torch, fn, clock, window_ms):
-    """ms per call over one window of back-to-back calls of about `window_ms` (at least 150), and the median SM clock"""
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    iters = int(min(5000, max(3, window_ms / ((time.perf_counter() - t0) * 1e3))))
-    clock.armed.set()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    e1.synchronize()
-    clock.armed.clear()
-    return e0.elapsed_time(e1) / iters, clock.take()
-
-
-def alternate(torch, fns, clock, window_ms, reps):
-    """{name: median ms} over `reps` rounds, one window per function per round; and the median clock"""
-    res, mhz = {k: [] for k in fns}, []
-    for _ in range(reps):
-        for k, fn in fns.items():
-            ms, m = timed(torch, fn, clock, window_ms)
-            res[k].append(ms)
-            mhz.append(m)
-    return {k: float(np.median(v)) for k, v in res.items()}, float(np.median(mhz))
+from measure import DATASHEET, alternate, capture, setup  # noqa: E402
 
 
 def copy_case(nk, dev, torch, name, shapes, axis, dt, gdt, stack):
@@ -147,12 +112,7 @@ def head_step(nk, dev, T, n, hidden, use_cat):
         loss.backward(1.0)
         opt.step()
 
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(4 << 30) as cap:
-        step()
-    return cap.graph
+    return capture(dev, step, 4 << 30)
 
 
 def main():
@@ -165,14 +125,7 @@ def main():
 
     import neuronika_b200 as nk
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "hbm_datasheet_gbps": HBM_GBPS}), flush=True)
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
     cases = [("sequence", [(1024, 2048)] * 32, 0, nk.BF16, nk.F32, False),
              ("channels", [(256, 64, 56, 56)] * 2, 1, nk.BF16, nk.BF16, False),
              ("interleave", [(1 << 24,)] * 3, 1, nk.F32, nk.F32, True)]
@@ -180,13 +133,13 @@ def main():
         fwd, bwd, fb, bb, check = copy_case(nk, dev, torch, name, shapes, axis, dt, gdt, stack)
         check()
         for direction, fns, nbytes in (("forward", fwd, fb), ("backward", bwd, bb)):
-            ms, mhz = alternate(torch, fns, clock, args.window_ms, args.reps)
+            ms, mhz = alternate(fns, args.window_ms, args.reps)
             gbps = {k: round(nbytes / v / 1e6, 1) for k, v in ms.items()}
             print(json.dumps({
                 "case": name, "direction": direction, "op": "stack" if stack else "cat", "operands": len(shapes),
                 "shape": list(shapes[0]), "axis": axis, "bytes": nbytes,
                 "us": {k: round(v * 1e3, 2) for k, v in ms.items()}, "gbps": gbps,
-                "share_of_hbm": {k: round(v / HBM_GBPS, 3) for k, v in gbps.items()},
+                "share_of_hbm": {k: round(v / DATASHEET["hbm_gbps"], 3) for k, v in gbps.items()},
                 "ours_vs_torch": round(ms["torch"] / ms["ours"], 3),
                 "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
         del fwd, bwd
@@ -194,8 +147,7 @@ def main():
     T, n, hidden = 32, 256, 1024
     per_step = head_step(nk, dev, T, n, hidden, use_cat=False)
     catted = head_step(nk, dev, T, n, hidden, use_cat=True)
-    ms, mhz = alternate(torch, {"per_step_heads": per_step.launch, "cat_one_head": catted.launch}, clock,
-                        args.window_ms, args.reps)
+    ms, mhz = alternate({"per_step_heads": per_step.launch, "cat_one_head": catted.launch}, args.window_ms, args.reps)
     print(json.dumps({
         "case": "sequence_head", "T": T, "N": n, "H": hidden, "dtype": "bf16", "grad_dtype": "f32",
         "ms_per_step": {k: round(v, 4) for k, v in ms.items()},
@@ -204,7 +156,6 @@ def main():
         "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
     per_step.close()
     catted.close()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

@@ -28,9 +28,9 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-HBM_GBPS = 3350.0
+from measure import DATASHEET, alternate, capture, setup  # noqa: E402
+
 V_, E_, T_, N_ = 10000, 650, 35, 256
 _MLP = [(4096, 1024), (4096,), (4096, 4096), (4096,), (10, 4096), (10,)]
 _LM = [(V_, E_), (4 * E_, E_), (4 * E_, E_), (4 * E_,), (4 * E_,), (V_, E_), (V_,)]
@@ -74,10 +74,7 @@ def param_set(nk, dev, torch, shapes, dt, gdt, seed):
 
 def captured(nk, dev, torch, ours, theirs, max_norm):
     from neuronika_b200 import optim
-    optim.clip_grad_norm_(ours, max_norm)
-    dev.synchronize()
-    with dev.capture(64 << 20) as cap:
-        optim.clip_grad_norm_(ours, max_norm)
+    ours_graph = capture(dev, lambda: optim.clip_grad_norm_(ours, max_norm), 64 << 20)
     g = torch.cuda.CUDAGraph()
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
@@ -86,7 +83,7 @@ def captured(nk, dev, torch, ours, theirs, max_norm):
     torch.cuda.current_stream().wait_stream(side)
     with torch.cuda.graph(g):
         torch.nn.utils.clip_grad_norm_(theirs, max_norm, foreach=True)
-    return cap.graph, g
+    return ours_graph, g
 
 
 def lm_step(nk, dev, clip, V=V_, E=E_, T=T_, N=N_):
@@ -115,13 +112,9 @@ def lm_step(nk, dev, clip, V=V_, E=E_, T=T_, N=N_):
             keep.append(optim.clip_grad_norm_(params, 0.25))
         opt.step()
 
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(8 << 30) as cap:
-        step()
+    graph = capture(dev, step, 8 << 30)
     total = float(keep[-1].as_ndarray()) if clip else None
-    return cap.graph, total
+    return graph, total
 
 
 def main():
@@ -139,18 +132,9 @@ def main():
     import torch
 
     import neuronika_b200 as nk
-    from cat_bench import alternate
-    from gemm_sweep import Clock
     from neuronika_b200 import optim
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "hbm_datasheet_gbps": HBM_GBPS}), flush=True)
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
     for name, (shapes, dt, gdt) in SETS.items():
         ours, theirs = param_set(nk, dev, torch, shapes, dt, gdt, 0)
         t_ours = float(optim.get_total_norm(ours).as_ndarray())
@@ -162,13 +146,13 @@ def main():
             fns = {"ours_eager": lambda: optim.clip_grad_norm_(ours, max_norm),
                    "torch_eager": lambda: torch.nn.utils.clip_grad_norm_(theirs, max_norm, foreach=True),
                    "ours_captured": g_ours.launch, "torch_captured": g_theirs.replay}
-            ms, mhz = alternate(torch, fns, clock, args.window_ms, args.reps)
+            ms, mhz = alternate(fns, args.window_ms, args.reps)
             nbytes = traffic(shapes, gdt, clip)
             print(json.dumps({
                 "set": name, "tensors": len(shapes), "elements": numel(shapes), "grad_dtype": gdt, "clip": clip,
                 "bytes": nbytes, "us": {k: round(v * 1e3, 1) for k, v in ms.items()},
                 "ours_captured_gbps": round(nbytes / ms["ours_captured"] / 1e6, 1),
-                "ours_captured_share_of_hbm": round(nbytes / ms["ours_captured"] / 1e6 / HBM_GBPS, 3),
+                "ours_captured_share_of_hbm": round(nbytes / ms["ours_captured"] / 1e6 / DATASHEET["hbm_gbps"], 3),
                 "captured_vs_torch": round(ms["torch_captured"] / ms["ours_captured"], 3),
                 "eager_vs_torch": round(ms["torch_eager"] / ms["ours_eager"], 3),
                 "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
@@ -179,7 +163,7 @@ def main():
     graphs = {}
     for clip in (False, True):
         graphs["lm_step_clip" if clip else "lm_step"] = lm_step(nk, dev, clip)
-    ms, mhz = alternate(torch, {k: g.launch for k, (g, _) in graphs.items()}, clock, args.window_ms, args.reps)
+    ms, mhz = alternate({k: g.launch for k, (g, _) in graphs.items()}, args.window_ms, args.reps)
     for k, (g, total) in graphs.items():
         print(json.dumps({"case": k, "V": V_, "E": E_, "T": T_, "N": N_, "dtype": "bf16", "grad_dtype": "f32",
                           "ms_per_step": round(ms[k], 4), "kernels_per_step": g.kernel_count,
@@ -189,7 +173,6 @@ def main():
                       "share": round(ms["lm_step_clip"] / ms["lm_step"] - 1.0, 4)}), flush=True)
     for g, _ in graphs.values():
         g.close()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

@@ -27,12 +27,9 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from cat_bench import alternate  # noqa: E402
-from gemm_sweep import Clock  # noqa: E402
+from measure import DATASHEET, alternate, setup  # noqa: E402
 
-BF16_TFLOPS = 989.0
 # name: (N, Cin, Cout, sample extents, kernel, padding, mode)
 CASES = {
     "conv1d": (64, 256, 256, (4096,), (3,), (1,), "zero"),
@@ -105,20 +102,13 @@ def main():
 
     import neuronika_b200 as nk
 
-    torch.cuda.set_device(0)
     torch.backends.cudnn.benchmark = True
-    stream = torch.cuda.Stream()
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "bf16_datasheet_tflops": BF16_TFLOPS}), flush=True)
+    dev, card = setup(bf16_datasheet_tflops=DATASHEET["bf16_tflops"])
     for name in args.cases.split(","):
         n, cin, cout, sp, k, pad, mode = CASES[name]
         fwd, both, flops, cols, err = case_fns(nk, dev, torch, n, cin, cout, sp, k, pad, mode)
         for direction, fns, fl in (("forward", fwd, flops), ("forward+backward", both, 3 * flops)):
-            ms, mhz = alternate(torch, fns, clock, args.window_ms, args.reps)
+            ms, mhz = alternate(fns, args.window_ms, args.reps)
             tf = {key: round(fl / v / 1e9, 1) for key, v in ms.items()}
             print(json.dumps({
                 "case": name, "direction": direction, "N": n, "cin": cin, "cout": cout, "extent": list(sp),
@@ -130,7 +120,6 @@ def main():
                 "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
         del fwd, both
         torch.cuda.empty_cache()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

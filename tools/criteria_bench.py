@@ -31,9 +31,9 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-HBM_GBPS = 3350.0
+from measure import DATASHEET, alternate, capture, setup  # noqa: E402
+
 OPS = ["mae", "bce", "bce_with_logits", "kldiv", "dropout"]
 
 
@@ -126,12 +126,7 @@ def mlp_step(nk, dev, batch=4096, n_in=1024, hidden=4096):
         opt.step()
 
     dev.manual_seed(0)
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(2 << 30) as cap:
-        step()
-    return cap.graph
+    return capture(dev, step, 2 << 30)
 
 
 def main():
@@ -152,40 +147,30 @@ def main():
     import torch
 
     import neuronika_b200 as nk
-    from cat_bench import alternate
-    from gemm_sweep import Clock
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "hbm_datasheet_gbps": HBM_GBPS}), flush=True)
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
     for op in OPS:
         for dname, dt in (("f32", torch.float32), ("bf16", torch.bfloat16)):
             fwd, bwd = case(nk, dev, torch, op, shape, dt)
             nbytes = traffic(op, n, 2 if dt == torch.bfloat16 else 4)
             for k, (direction, fns) in enumerate((("forward", fwd), ("backward", bwd))):
-                ms, mhz = alternate(torch, fns, clock, args.window_ms, args.reps)
+                ms, mhz = alternate(fns, args.window_ms, args.reps)
                 gbps = {i: round(nbytes[i][k] / v / 1e6, 1) for i, v in ms.items()}
                 print(json.dumps({
                     "op": op, "dtype": dname, "direction": direction, "n": n,
                     "bytes": {i: nbytes[i][k] for i in ms}, "us": {i: round(v * 1e3, 2) for i, v in ms.items()},
-                    "gbps": gbps, "share_of_hbm": {i: round(v / HBM_GBPS, 3) for i, v in gbps.items()},
+                    "gbps": gbps, "share_of_hbm": {i: round(v / DATASHEET["hbm_gbps"], 3) for i, v in gbps.items()},
                     "ours_vs_torch": round(ms["torch"] / ms["ours"], 3),
                     "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
             del fwd, bwd
             torch.cuda.empty_cache()
     g = mlp_step(nk, dev)
-    ms, mhz = alternate(torch, {"step": g.launch}, clock, args.window_ms, args.reps)
+    ms, mhz = alternate({"step": g.launch}, args.window_ms, args.reps)
     print(json.dumps({
         "case": "mlp_dropout_bce_with_logits", "batch": 4096, "layers": [1024, 4096, 1], "p": 0.5,
         "dtype": "bf16", "grad_dtype": "f32", "ms_per_step": round(ms["step"], 4), "kernels_per_step": g.kernel_count,
         "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
     g.close()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

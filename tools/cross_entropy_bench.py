@@ -28,9 +28,9 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-HBM_GBPS = 3350.0
+from measure import DATASHEET, alternate, capture, setup  # noqa: E402
+
 # name: (x shape, dtype)
 CASES = {
     "config4_8192x10_f32": ((8192, 10), "f32"),
@@ -114,12 +114,7 @@ def lm_step(nk, dev, fused, V=10000, E=650, T=35, N=256):
         loss.backward(1.0)
         opt.step()
 
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(8 << 30) as cap:
-        step()
-    return cap.graph
+    return capture(dev, step, 8 << 30)
 
 
 def main():
@@ -138,26 +133,17 @@ def main():
     import torch
 
     import neuronika_b200 as nk
-    from cat_bench import alternate
-    from gemm_sweep import Clock
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "hbm_datasheet_gbps": HBM_GBPS}), flush=True)
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
     for name, (shape, xdt) in CASES.items():
         fwd, fb = case(nk, dev, torch, shape, xdt)
         fbytes, bbytes = traffic(shape, 2 if xdt == "bf16" else 4)
         for direction, fns, nbytes in (("forward", fwd, fbytes), ("fwd+bwd", fb, fbytes + bbytes)):
-            ms, mhz = alternate(torch, fns, clock, args.window_ms, args.reps)
+            ms, mhz = alternate(fns, args.window_ms, args.reps)
             rec = {"case": name, "shape": shape, "dtype": xdt, "direction": direction, "bytes": nbytes,
                    "us": {k: round(v * 1e3, 1) for k, v in ms.items()},
                    "fused_gbps": round(nbytes / ms["fused"] / 1e6, 1),
-                   "fused_share_of_hbm": round(nbytes / ms["fused"] / 1e6 / HBM_GBPS, 3),
+                   "fused_share_of_hbm": round(nbytes / ms["fused"] / 1e6 / DATASHEET["hbm_gbps"], 3),
                    "fused_vs_torch": round(ms["torch"] / ms["fused"], 3)}
             if "composition" in ms:
                 rec["fused_vs_composition"] = round(ms["composition"] / ms["fused"], 3)
@@ -166,13 +152,12 @@ def main():
         del fwd, fb
         torch.cuda.empty_cache()
     graphs = {"lm_step_cross_entropy": lm_step(nk, dev, True), "lm_step_log_softmax_nll": lm_step(nk, dev, False)}
-    ms, mhz = alternate(torch, {k: g.launch for k, g in graphs.items()}, clock, args.window_ms, args.reps)
+    ms, mhz = alternate({k: g.launch for k, g in graphs.items()}, args.window_ms, args.reps)
     for k, g in graphs.items():
         print(json.dumps({"case": k, "V": 10000, "E": 650, "T": 35, "N": 256, "dtype": "bf16", "grad_dtype": "f32",
                           "ms_per_step": round(ms[k], 4), "kernels_per_step": g.kernel_count, "median_sm_mhz": mhz,
                           "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
         g.close()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

@@ -29,9 +29,9 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-HBM_GBPS = 3350.0
+from measure import DATASHEET, alternate, capture, setup  # noqa: E402
+
 # name: (v, e, ids shape, id distribution, weight dtype); gradients are f32
 CASES = {
     "gpt2_v50257_e768_8x1024": (50257, 768, (8, 1024), "uniform", "bf16"),
@@ -121,12 +121,7 @@ def lm_step(nk, dev, onehot, V=10000, E=650, T=35, N=256):
         loss.backward(1.0)
         opt.step()
 
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(8 << 30) as cap:
-        step()
-    return cap.graph
+    return capture(dev, step, 8 << 30)
 
 
 def main():
@@ -144,39 +139,29 @@ def main():
     import torch
 
     import neuronika_b200 as nk
-    from cat_bench import alternate
-    from gemm_sweep import Clock
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "hbm_datasheet_gbps": HBM_GBPS}), flush=True)
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
     for name, (v, e, shape, kind, wdt) in CASES.items():
         fwd, bwd, n = case(nk, dev, torch, v, e, shape, kind, wdt)
         fb, bb = traffic(v, e, n, 2 if wdt == "bf16" else 4)
         for direction, fns, nbytes in (("forward", fwd, fb), ("backward", bwd, bb)):
-            ms, mhz = alternate(torch, fns, clock, args.window_ms, args.reps)
+            ms, mhz = alternate(fns, args.window_ms, args.reps)
             print(json.dumps({
                 "case": name, "dtype": wdt, "grad_dtype": "f32", "direction": direction, "v": v, "e": e, "n": n,
                 "bytes": nbytes, "us": {i: round(t * 1e3, 1) for i, t in ms.items()},
                 "ours_gbps": round(nbytes / ms["ours"] / 1e6, 1),
-                "ours_share_of_hbm": round(nbytes / ms["ours"] / 1e6 / HBM_GBPS, 3),
+                "ours_share_of_hbm": round(nbytes / ms["ours"] / 1e6 / DATASHEET["hbm_gbps"], 3),
                 "ours_vs_torch": round(ms["torch"] / ms["ours"], 3),
                 "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
         del fwd, bwd
         torch.cuda.empty_cache()
     graphs = {"lm_step_embedding": lm_step(nk, dev, False), "lm_step_onehot_gemm": lm_step(nk, dev, True)}
-    ms, mhz = alternate(torch, {k: g.launch for k, g in graphs.items()}, clock, args.window_ms, args.reps)
+    ms, mhz = alternate({k: g.launch for k, g in graphs.items()}, args.window_ms, args.reps)
     for k, g in graphs.items():
         print(json.dumps({"case": k, "V": 10000, "E": 650, "T": 35, "N": 256, "dtype": "bf16", "grad_dtype": "f32",
                           "ms_per_step": round(ms[k], 4), "kernels_per_step": g.kernel_count, "median_sm_mhz": mhz,
                           "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
         g.close()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

@@ -12,7 +12,7 @@ convolution layers (nk_conv_layer_nd_*) with the padding folded into the gather;
 
 Shapes: config 5's two Conv2d layers (3->32 and 32->64, k3, pad 1, 32x32, N 4096), the config 3 stem (3->64 k3 p0,
 224x224, N 64), Conv1d 256->256 (k3, zero pad 1, N 64, L 4096) and Conv3d 64->64 (k3, replicative pad 1, N 8, 32^3).
-The ieee path takes up to seconds per call at these sizes: each window runs at least one call, after one warm-up call.
+The ieee path takes up to seconds per call at these sizes: each window runs at least one call.
 
 A separate torch.profiler pass per shape and tf32 mode splits a forward + backward call into the gathers and packs
 (tf32_im2col_kernel, tf32_pack_kernel), the GEMM (tf32_gemm_kernel) and the rest (col2im, the dW reduction, db).
@@ -32,14 +32,12 @@ import json
 import math
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from gemm_sweep import Clock  # noqa: E402
+from measure import DATASHEET, alternate, capture, kernel_ms, setup, window  # noqa: E402
 
 MODES = ("ieee", "tf32", "tf32x3")
 # name: (x shape, Cout, kernel, padding, padding mode)
@@ -51,25 +49,8 @@ SHAPES = {
     "conv3d 64->64 k3 replicative-pad1 32^3 N8": ((8, 64, 32, 32, 32), 64, (3, 3, 3), (1, 1, 1), "replicative"),
 }
 TORCH_PAD = {"zero": "zeros", "replicative": "replicate"}
-
-
-def timed(torch, fn, clock, window_ms):
-    """ms per call over one window of back-to-back calls (after one warm-up call), and the median SM clock meanwhile"""
-    fn()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    iters = int(min(1000, max(1, window_ms / ((time.perf_counter() - t0) * 1e3))))
-    clock.armed.set()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    e1.synchronize()
-    clock.armed.clear()
-    return e0.elapsed_time(e1) / iters, clock.take()
+# kernel groups of the profiler split ("" takes every other kernel)
+SPLIT = {"gather_pack": ("tf32_im2col", "tf32_pack"), "gemm": ("tf32_gemm",), "other": ("",)}
 
 
 def variants(nk, dev, torch, xs, cout, k, pad, pmode):
@@ -148,33 +129,8 @@ def variants(nk, dev, torch, xs, cout, k, pad, pmode):
     return vf, vb, flop
 
 
-def kernel_split(torch, fn, tag, out_dir):
-    """ms per call of (gathers + packs, GEMM, everything else) from a torch.profiler pass over 5 calls"""
-    from torch.profiler import ProfilerActivity, profile
-    fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(5):
-            fn()
-        torch.cuda.synchronize()
-    split = {"gather_pack": 0.0, "gemm": 0.0, "other": 0.0}
-    for e in prof.key_averages():
-        t = getattr(e, "device_time_total", None)
-        if t is None:
-            t = e.cuda_time_total
-        if "tf32_im2col" in e.key or "tf32_pack" in e.key:
-            split["gather_pack"] += t
-        elif "tf32_gemm" in e.key:
-            split["gemm"] += t
-        elif "Memcpy" not in e.key and "Memset" not in e.key:
-            split["other"] += t
-    if out_dir:
-        prof.export_chrome_trace(os.path.join(out_dir, f"f32_conv_{tag}.trace.json"))
-    return {k: v / 5e3 for k, v in split.items()}   # us over 5 calls -> ms per call
-
-
 def convnet_step(nk, dev, mode, batch=4096):
-    """config 5's ConvNet in f32, its training step captured in `mode` after one eager warm-up step"""
+    """config 5's ConvNet in f32, its training step captured in `mode`"""
     rng = np.random.default_rng(1)
     c1 = nk.nn.Conv2d(dev, 3, 32, (3, 3), padding=(1, 1), rng=rng)
     c2 = nk.nn.Conv2d(dev, 32, 64, (3, 3), padding=(1, 1), rng=rng)
@@ -194,13 +150,10 @@ def convnet_step(nk, dev, mode, batch=4096):
         opt.step()
 
     dev.f32_conv(mode)
-    step()
-    dev.synchronize()
-    with dev.capture(24 << 30) as cap:
-        step()
+    graph = capture(dev, step, 24 << 30)
     kern = dev.last_conv_kernel
     dev.f32_conv("ieee")
-    return cap.graph, kern
+    return graph, kern
 
 
 def main():
@@ -215,34 +168,20 @@ def main():
 
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-    torch.cuda.set_device(0)
     torch.backends.cudnn.benchmark = True
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count}), flush=True)
+    dev, card = setup(tf32_datasheet_tflops=DATASHEET["tf32_tflops"], fp32_datasheet_tflops=DATASHEET["fp32_tflops"])
     for name, (xs, cout, k, pad, pmode) in SHAPES.items():
         vf, vb, flop = variants(nk, dev, torch, xs, cout, k, pad, pmode)
         for what, v, products in (("fwd", vf, 1), ("fwd+bwd", vb, 3)):
-            times = {key: [] for key in v}
-            mhz = []
-            for _ in range(args.reps):
-                for key, fn in v.items():
-                    ms, m = timed(torch, fn, clock, args.window_ms)
-                    times[key].append(ms)
-                    mhz.append(m)
+            times, mhz = alternate(v, args.window_ms, args.reps)
             row = {"shape": name, "pass": what, "card": card["name"], "power_limit_w": card["power_limit_w"],
-                   "sm_mhz_median": float(np.nanmedian(mhz))}
-            for key, ts in times.items():
-                ms = float(np.median(ts))
+                   "sm_mhz_median": mhz}
+            for key, ms in times.items():
                 row[key] = {"ms": round(ms, 4), "tflops": round(products * flop / ms / 1e9, 2)}
             if what == "fwd+bwd":
                 for mode in ("tf32", "tf32x3"):
-                    tag = f"{name.split()[0]}_{mode}"
-                    sp = kernel_split(torch, v[mode], tag, args.out)
+                    trace = f"f32_conv_{name.split()[0]}_{mode}.trace.json"
+                    sp = kernel_ms(v[mode], SPLIT, os.path.join(args.out, trace) if args.out else None)
                     total = sum(sp.values())
                     row[mode].update({k2 + "_ms": round(t, 4) for k2, t in sp.items()})
                     row[mode]["gather_pack_share"] = round(sp["gather_pack"] / total, 3) if total > 0 else None
@@ -259,7 +198,7 @@ def main():
     for _ in range(args.reps):
         for m in MODES:
             g, kern[m] = convnet_step(nk, dev, m)
-            ms, c = timed(torch, g.launch, clock, max(args.window_ms, 300.0))
+            ms, c = window(g.launch, max(args.window_ms, 300.0), 1)
             g.close()
             times[m].append(ms)
             mhz.append(c)
@@ -269,7 +208,6 @@ def main():
         row[m + "_ms"] = round(float(np.median(times[m])), 3)
         row[m + "_conv_kernel"] = kern[m]
     print(json.dumps(row), flush=True)
-    clock.halt.set()
 
 
 if __name__ == "__main__":

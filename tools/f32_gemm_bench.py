@@ -24,39 +24,16 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from gemm_sweep import Clock  # noqa: E402
+from measure import DATASHEET, alternate, capture, kernel_ms, setup  # noqa: E402
 
 SHAPES = [("NT", 4096, 4096, 4096), ("NN", 4096, 4096, 4096), ("TN", 4096, 4096, 4096),
           ("NT", 8192, 4096, 1024), ("NT", 8192, 4096, 4096), ("NT", 8192, 10, 4096)]
 MODES = ("ieee", "tf32", "tf32x3")
-HBM_BYTES_PER_S = 3.35e12
-
-
-def timed(torch, fn, clock, window_ms):
-    """ms per call over one window of back-to-back calls (after a short warm-up), and the median SM clock meanwhile"""
-    for _ in range(2):
-        fn()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    iters = int(min(2000, max(3, window_ms / ((time.perf_counter() - t0) * 1e3))))
-    clock.armed.set()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    e1.synchronize()
-    clock.armed.clear()
-    return e0.elapsed_time(e1) / iters, clock.take()
 
 
 def gemm_variants(nk, dev, torch, form, M, N, K):
@@ -88,36 +65,19 @@ def gemm_variants(nk, dev, torch, form, M, N, K):
     return v
 
 
-def pack_share(torch, fn, M, N, K, mode, out_dir):
-    """(pack ms, gemm ms, pack GB/s) per call from a torch.profiler pass over 10 calls"""
-    from torch.profiler import ProfilerActivity, profile
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(10):
-            fn()
-        torch.cuda.synchronize()
-    pack = gemm = 0.0
-    for e in prof.key_averages():
-        t = getattr(e, "device_time_total", None)
-        if t is None:
-            t = e.cuda_time_total
-        if "tf32_pack" in e.key:
-            pack += t
-        elif "tf32_gemm" in e.key:
-            gemm += t
-    pack, gemm = pack / 10e3, gemm / 10e3    # us total over 10 calls -> ms per call
+def pack_share(fn, M, N, K, mode, out_dir):
+    """(pack ms, gemm ms, pack GB/s) per call from a torch.profiler pass"""
+    trace = os.path.join(out_dir, f"f32_gemm_{M}x{N}x{K}_{mode}.trace.json") if out_dir else None
+    ms = kernel_ms(fn, {"pack": ("tf32_pack",), "gemm": ("tf32_gemm",)}, trace)
+    pack, gemm = ms["pack"], ms["gemm"]
     kp = K * (3 if mode == "tf32x3" else 1)
     ldp = (kp + 3) // 4 * 4
     bytes_ = 4 * (M + N) * (K + ldp)
-    if out_dir:
-        prof.export_chrome_trace(os.path.join(out_dir, f"f32_gemm_{M}x{N}x{K}_{mode}.trace.json"))
     return pack, gemm, (bytes_ / (pack * 1e-3) / 1e9) if pack > 0 else float("nan")
 
 
 def mlp_step(nk, dev, mode, batch=8192, sizes=(1024, 4096, 4096, 10)):
-    """the captured f32 training step of the MLP in `mode` (captured after one eager warm-up step)"""
+    """the captured f32 training step of the MLP in `mode`"""
     rng = np.random.default_rng(1)
     layers = [nk.nn.Linear(dev, a, b, rng=rng) for a, b in zip(sizes[:-1], sizes[1:])]
     opt = nk.optim.StochasticGD.new(0.01)
@@ -139,12 +99,9 @@ def mlp_step(nk, dev, mode, batch=8192, sizes=(1024, 4096, 4096, 10)):
         opt.step()
 
     dev.f32_matmul(mode)
-    step()
-    dev.synchronize()
-    with dev.capture(6 << 30) as cap:
-        step()
+    graph = capture(dev, step, 6 << 30)
     dev.f32_matmul("ieee")
-    return cap.graph, layers
+    return graph, layers
 
 
 def main():
@@ -159,34 +116,21 @@ def main():
 
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count}), flush=True)
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"], tf32_datasheet_tflops=DATASHEET["tf32_tflops"],
+                      fp32_datasheet_tflops=DATASHEET["fp32_tflops"])
     for form, M, N, K in SHAPES:
         v = gemm_variants(nk, dev, torch, form, M, N, K)
-        times = {k: [] for k in v}
-        mhz = []
-        for _ in range(args.reps):
-            for name, fn in v.items():
-                ms, m = timed(torch, fn, clock, args.window_ms)
-                times[name].append(ms)
-                mhz.append(m)
+        times, mhz = alternate(v, args.window_ms, args.reps)
         flop = 2.0 * M * N * K
         row = {"form": form, "M": M, "N": N, "K": K, "card": card["name"], "power_limit_w": card["power_limit_w"],
-               "sm_mhz_median": float(np.nanmedian(mhz))}
-        for name, ts in times.items():
-            ms = float(np.median(ts))
+               "sm_mhz_median": mhz}
+        for name, ms in times.items():
             row[name] = {"ms": round(ms, 4), "tflops": round(flop / ms / 1e9, 1)}
         for mode in ("tf32", "tf32x3"):
-            pack, gemm, gbs = pack_share(torch, v[mode], M, N, K, mode, args.out)
+            pack, gemm, gbs = pack_share(v[mode], M, N, K, mode, args.out)
             row[mode].update({"pack_ms": round(pack, 4), "gemm_kernel_ms": round(gemm, 4),
                               "pack_share": round(pack / (pack + gemm), 3) if pack + gemm > 0 else None,
-                              "pack_gbs": round(gbs, 1), "pack_hbm_fraction": round(gbs * 1e9 / HBM_BYTES_PER_S, 3),
+                              "pack_gbs": round(gbs, 1), "pack_hbm_fraction": round(gbs / DATASHEET["hbm_gbps"], 3),
                               "gemm_kernel_tflops": round(flop / gemm / 1e9, 1) if gemm > 0 else None})
         row["tf32x3_over_simt"] = round(row["ieee"]["ms"] / row["tf32x3"]["ms"], 2)
         print(json.dumps(row), flush=True)
@@ -194,21 +138,14 @@ def main():
         torch.backends.cuda.matmul.allow_tf32 = False
 
     graphs = {m: mlp_step(nk, dev, m) for m in MODES}
-    times = {m: [] for m in MODES}
-    mhz = []
-    for _ in range(args.reps):
-        for m, (g, _) in graphs.items():
-            ms, c = timed(torch, g.launch, clock, max(args.window_ms, 300.0))
-            times[m].append(ms)
-            mhz.append(c)
+    times, mhz = alternate({m: g.launch for m, (g, _) in graphs.items()}, max(args.window_ms, 300.0), args.reps)
     row = {"mlp_step": "1024-4096-4096-10 f32, batch 8192, captured", "card": card["name"],
-           "power_limit_w": card["power_limit_w"], "sm_mhz_median": float(np.nanmedian(mhz))}
+           "power_limit_w": card["power_limit_w"], "sm_mhz_median": mhz}
     for m in MODES:
-        row[m + "_ms"] = round(float(np.median(times[m])), 3)
+        row[m + "_ms"] = round(times[m], 3)
     print(json.dumps(row), flush=True)
     for g, _ in graphs.values():
         g.close()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Where the time of the wgmma GEMM engine goes: a K sweep of the three GEMM forms of the Linear 4096->4096 step.
 
-    python tools/gemm_sweep.py                    # writes one JSON line (and a table on stderr)
+    python tools/gemm_sweep.py                    # writes a header and one JSON line (and a table on stderr)
     python tools/gemm_sweep.py --root OTHER_TREE  # the same sweep against another build of the package
 
 The three forms exactly as the step calls them (nk_gemm_bias_act):
@@ -21,68 +21,15 @@ import argparse
 import json
 import os
 import sys
-import threading
-import time
 
 import numpy as np
+
+from measure import setup, window
 
 KS = (1024, 2048, 4096, 8192)
 MN = 4096
 BLOCK_M, BLOCK_N, BLOCK_K = 128, 256, 64
 CYCLES_PER_KBLOCK = 2 * BLOCK_M * BLOCK_N * BLOCK_K / 4096     # dense bf16: 4096 FLOP per cycle and SM on H100
-
-
-class Clock(threading.Thread):
-    """median SM clock (NVML) while armed"""
-
-    def __init__(self, index):
-        super().__init__(daemon=True)
-        import pynvml
-        pynvml.nvmlInit()
-        self.nv, self.h = pynvml, pynvml.nvmlDeviceGetHandleByIndex(index)
-        self.samples, self.armed, self.halt = [], threading.Event(), threading.Event()
-
-    def run(self):
-        while not self.halt.is_set():
-            if self.armed.is_set():
-                self.samples.append(int(self.nv.nvmlDeviceGetClockInfo(self.h, self.nv.NVML_CLOCK_SM)))
-            time.sleep(0.002)
-
-    def take(self):
-        s, self.samples = self.samples, []
-        return float(np.median(s)) if s else float("nan")
-
-    def card(self):
-        nv, h = self.nv, self.h
-        name = nv.nvmlDeviceGetName(h)
-        return {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0,
-                "sm_max_mhz": int(nv.nvmlDeviceGetMaxClockInfo(h, nv.NVML_CLOCK_SM))}
-
-
-def time_calls(torch, fn, clock, window_ms, reps):
-    """median over `reps` windows of back-to-back calls, each about `window_ms` long (ms per call), and the median SM
-    clock meanwhile"""
-    for _ in range(5):
-        fn()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(5):
-        fn()
-    torch.cuda.synchronize()
-    iters = int(min(5000, max(20, window_ms / ((time.perf_counter() - t0) * 1e3 / 5))))
-    clock.armed.set()
-    per = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        e1.synchronize()
-        per.append(e0.elapsed_time(e1) / iters)
-    clock.armed.clear()
-    return float(np.median(per)), clock.take()
 
 
 def main():
@@ -99,11 +46,7 @@ def main():
     import neuronika_b200 as nk
     from neuronika_b200 import ops
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.current_stream()
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
+    dev, card = setup()
     sm = dev.sm_count
     tiles = (MN // BLOCK_M) * (MN // BLOCK_N)
     waves = -(-tiles // sm)
@@ -137,12 +80,12 @@ def main():
                 own = lambda: ops.gemm(A, B, C32, trans_a=True)
                 ref = lambda: torch.mm(a.t(), b, out_dtype=torch.float32)
             A, B, C16, C32, Bias = wrap(a), wrap(b), wrap(y16), wrap(y32), wrap(bias)
-            ms, mhz = time_calls(torch, own, clock, args.window_ms, args.reps)
+            ms, mhz = window(own, args.window_ms, args.reps)
             row = {"K": K, "ms": round(ms, 5), "sm_mhz": mhz, "kcycles": round(ms * mhz, 1),
                    "tflops": round(2.0 * MN * MN * K / ms / 1e9, 1), "kernel": dev.last_gemm_kernel}
             if not args.no_cublas:
                 try:
-                    cms, cmhz = time_calls(torch, ref, clock, args.window_ms, args.reps)
+                    cms, cmhz = window(ref, args.window_ms, args.reps)
                     row.update(cublas_ms=round(cms, 5), cublas_sm_mhz=cmhz, cublas_kcycles=round(cms * cmhz, 1),
                                cublas_tflops=round(2.0 * MN * MN * K / cms / 1e9, 1))
                 except Exception as e:  # noqa: BLE001 -- an older torch without out_dtype: leave the column out
@@ -150,7 +93,6 @@ def main():
             rows[form].append(row)
             del a, b, A, B
     torch.cuda.synchronize()
-    clock.halt.set()
 
     fits = {}
     for form, rs in rows.items():
@@ -178,7 +120,7 @@ def main():
                 "intercept_kcycles_per_tile": round(bc / tiles_per_cta, 2)}
         fits[form] = fit
     out = {"what": "K sweep of the Linear step's three GEMM forms at M = N = 4096; fit time = a.K + b",
-           "card": clock.card(), "sm_count": sm, "grid": grid, "tiles_per_cta": tiles_per_cta,
+           "card": card, "sm_count": sm, "grid": grid, "tiles_per_cta": tiles_per_cta,
            "window_ms": args.window_ms, "reps": args.reps, "root": os.path.abspath(args.root), "rows": rows, "fits": fits}
     for form, rs in rows.items():
         print(form, file=sys.stderr)

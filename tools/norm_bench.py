@@ -2,7 +2,7 @@
 """Normalization benchmark (development tool; bench.py measures the flagship workload).
 
 For each case, csrc/nk_norm.cu against torch CUDA (cuDNN batch norm, torch's native layer norm) on the same tensors in
-the same process, the two alternating window by window after a warm-up, timed with CUDA events:
+the same process, the two alternating window by window, timed with CUDA events:
   forward           ours: nk_batch_norm_fwd in training mode (running statistics updated) / nk_layer_norm_fwd;
                     torch: F.batch_norm(training=True) / F.layer_norm;
   forward+backward  the forward, then ours: nk_*_norm_bwd writing dx, dw and db (beta 0); torch: torch.autograd.grad
@@ -10,7 +10,8 @@ the same process, the two alternating window by window after a warm-up, timed wi
 Bytes are the least the algorithm moves: the batch-norm forward reads x twice (statistics, then apply: these maps do not
 fit the 50 MB L2) and writes y; its backward reads g and x twice and writes dx; the layer-norm forward reads x once and
 writes y (a row fits on chip); its backward reads g and x once and writes dx.  GB/s are reported beside the 3.35 TB/s
-HBM3 data-sheet bound of the H100 SXM.  Card name and power limit are printed beside the numbers.
+HBM3 data-sheet bound of the H100 SXM.  Card name, power limit and the median SM clock during the timed windows (NVML)
+are printed beside the numbers.
 
     python tools/norm_bench.py [--reps 5] [--window-ms 200] [--only bn2d_cfg5_c32]
     python tools/norm_bench.py --dry-run      # the byte counts only, no device
@@ -20,14 +21,14 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-HBM_GBPS = 3350.0
+from measure import DATASHEET, alternate, setup  # noqa: E402
+
 # name: (kind, shape, dtypes); layer norm normalizes the last dim
 CASES = {
     "bn2d_cfg5_c32": ("bn", (4096, 32, 32, 32), ("bf16", "f32")),
@@ -48,41 +49,13 @@ def traffic(kind, shape, esize):
     return fwd, fwd + bwd
 
 
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
-
-
-def timed(fn, window_ms, torch):
-    """ms per call: calls in a window of about window_ms, timed with CUDA events"""
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    n = max(3, int(window_ms / max(s.elapsed_time(e), 1e-3)))
-    s.record()
-    for _ in range(n):
-        fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e) / n
-
-
-def run_case(name, dtype, reps, window_ms):
+def run_case(dev, card, name, dtype, reps, window_ms):
     import torch
     import torch.nn.functional as F
 
     import neuronika_b200 as nk
     from neuronika_b200 import ops
     kind, shape, _ = CASES[name]
-    stream = torch.cuda.Stream()   # ours and torch's kernels on one stream, so that the events time both
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
     tdt = torch.bfloat16 if dtype == "bf16" else torch.float32
     ndt = nk.BF16 if dtype == "bf16" else nk.F32
     gen = torch.Generator(device="cuda").manual_seed(0)
@@ -133,22 +106,15 @@ def run_case(name, dtype, reps, window_ms):
             torch.autograd.grad(F.layer_norm(xr, (cols,), w, b), (xr, w, b), g)
 
     fns = {"ours_fwd": ours_f, "torch_fwd": torch_f, "ours_fwdbwd": ours_fb, "torch_fwdbwd": torch_fb}
-    for f in fns.values():   # warm-up: module loads, cuDNN picks its algorithms
-        f()
-        f()
-    torch.cuda.synchronize()
-    times = {k: [] for k in fns}
-    for _ in range(reps):
-        for k, f in fns.items():     # alternating ours / torch, window by window
-            times[k].append(timed(f, window_ms, torch))
-    med = {k: float(np.median(v)) for k, v in times.items()}
+    med, mhz = alternate(fns, window_ms, reps)
     fb, fbb = traffic(kind, shape, 2 if dtype == "bf16" else 4)
     return {"case": name, "dtype": dtype, "shape": list(shape),
             "ours_fwd_us": med["ours_fwd"] * 1e3, "torch_fwd_us": med["torch_fwd"] * 1e3,
             "ours_fwd_GBps": fb / med["ours_fwd"] / 1e6, "torch_fwd_GBps": fb / med["torch_fwd"] / 1e6,
             "ours_fwdbwd_us": med["ours_fwdbwd"] * 1e3, "torch_fwdbwd_us": med["torch_fwdbwd"] * 1e3,
             "ours_fwdbwd_GBps": fbb / med["ours_fwdbwd"] / 1e6,
-            "torch_fwdbwd_GBps": fbb / med["torch_fwdbwd"] / 1e6}
+            "torch_fwdbwd_GBps": fbb / med["torch_fwdbwd"] / 1e6,
+            "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}
 
 
 def main():
@@ -165,16 +131,16 @@ def main():
             for d in dts:
                 print(n, d, "bytes fwd / fwd+bwd:", traffic(kind, shape, 2 if d == "bf16" else 4))
         return
-    print("card:", card())
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
     for n in names:
         for d in CASES[n][2]:
-            r = run_case(n, d, a.reps, a.window_ms)
+            r = run_case(dev, card, n, d, a.reps, a.window_ms)
             print(json.dumps(r))
             print("  %-20s %-4s fwd ours %8.1f us %6.0f GB/s (%2.0f %%) | torch %8.1f us | %4.2fx    fwd+bwd ours %8.1f us "
                   "%6.0f GB/s (%2.0f %%) | torch %8.1f us | %4.2fx" % (
-                      n, d, r["ours_fwd_us"], r["ours_fwd_GBps"], 100 * r["ours_fwd_GBps"] / HBM_GBPS, r["torch_fwd_us"],
-                      r["torch_fwd_us"] / r["ours_fwd_us"], r["ours_fwdbwd_us"], r["ours_fwdbwd_GBps"],
-                      100 * r["ours_fwdbwd_GBps"] / HBM_GBPS, r["torch_fwdbwd_us"],
+                      n, d, r["ours_fwd_us"], r["ours_fwd_GBps"], 100 * r["ours_fwd_GBps"] / DATASHEET["hbm_gbps"],
+                      r["torch_fwd_us"], r["torch_fwd_us"] / r["ours_fwd_us"], r["ours_fwdbwd_us"],
+                      r["ours_fwdbwd_GBps"], 100 * r["ours_fwdbwd_GBps"] / DATASHEET["hbm_gbps"], r["torch_fwdbwd_us"],
                       r["torch_fwdbwd_us"] / r["ours_fwdbwd_us"]), flush=True)
 
 

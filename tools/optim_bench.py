@@ -2,9 +2,9 @@
 """Optimizer step benchmark: one optimizer's step over three parameter sets, and a training step with it (development
 tool; bench.py measures the flagship workload).
 
-Each step is captured (Device.capture) and replayed in windows of `--window-ms`, timed with CUDA events
-(Device.timer_start / timer_stop).  Parameters are bf16 with f32 gradients, no master weights.  `--optimizer`: sgd
-(no momentum, as bench.py's configs 4 and 5), adam, rmsprop (centered, momentum 0.9) or adagrad.  Parameter sets:
+Each step is captured (Device.capture) and replayed in windows of `--window-ms`, timed with CUDA events.  Parameters
+are bf16 with f32 gradients, no master weights.  `--optimizer`: sgd (no momentum, as bench.py's configs 4 and 5), adam,
+rmsprop (centered, momentum 0.9) or adagrad.  Parameter sets:
   - mlp:  config 4's MLP 1024-4096-4096-10 (6 tensors);
   - lstm: the README's 2-layer bidirectional LSTM at N = 256, I = H = 1024 (16 tensors: per layer and direction W_ih,
           W_hh, b_ih, b_hh);
@@ -13,8 +13,8 @@ Reported per set, one JSON line each: us per optimizer step (median of the windo
 step (the captured graph's kernel count), and GB/s from the bytes the optimizer must move per element -- w read +
 written (2 x 2 B), g read (4 B) and, except for plain SGD, the penalised gradient written back (4 B), and each f32
 state array read + written (2 x 4 B) -- against the H100 SXM's 3.35 TB/s.  Then one captured training step of the mlp
-set (batch 8192, MSE) with the optimizer and StepLR, in ms per step and kernels per step.  Card name and power limit
-are printed beside the numbers.
+set (batch 8192, MSE) with the optimizer and StepLR, in ms per step and kernels per step.  Card name, power limit and
+the median SM clock during the timed windows (NVML) are printed beside the numbers.
 
     python tools/optim_bench.py [--optimizer adam] [--reps 7] [--window-ms 200]
 """
@@ -23,15 +23,14 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-HBM_TBPS = 3.35
+from measure import DATASHEET, capture, setup, window  # noqa: E402
+
 BYTES_PER_ELEM = {"sgd": 2 * 2 + 4, "adam": 2 * 2 + 2 * 4 + 4 * 4, "rmsprop": 2 * 2 + 2 * 4 + 6 * 4,
                   "adagrad": 2 * 2 + 2 * 4 + 2 * 4}
 
@@ -45,16 +44,6 @@ def make_opt(family, lr, **kw):
     if family == "rmsprop":
         return optim.RMSProp.new(lr, momentum=0.9, centered=True, **kw)
     return optim.Adagrad.new(lr, **kw)
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, limit = [s.strip() for s in out.split(",")]
-        return {"gpu": name, "power_limit": limit}
-    except Exception as e:  # the numbers stand without it, but say so
-        return {"gpu": "unknown (%s)" % e, "power_limit": "unknown"}
 
 
 def shapes(name):
@@ -71,16 +60,10 @@ def shapes(name):
     return [(4096,)] * 256
 
 
-def timed(dev, launch, window_ms):
-    """ms per launch over a window of about window_ms"""
-    dev.timer_start()
-    launch()
-    one = max(dev.timer_stop(), 1e-3)
-    n = max(3, int(window_ms / one))
-    dev.timer_start()
-    for _ in range(n):
-        launch()
-    return dev.timer_stop() / n
+def windows(launch, args):
+    """(ms per launch of each of `args.reps` windows, median SM MHz)"""
+    runs = [window(launch, args.window_ms, 1) for _ in range(args.reps)]
+    return [ms for ms, _ in runs], float(np.nanmedian([mhz for _, mhz in runs]))
 
 
 def optimizer_rows(nk, dev, args):
@@ -94,19 +77,18 @@ def optimizer_rows(nk, dev, args):
         opt = make_opt(args.optimizer, 1e-4)
         for p in ps:
             opt.register(p)
-        opt.step()
-        with dev.capture(1 << 20) as cap:
-            opt.step()
-        times = [timed(dev, cap.graph.launch, args.window_ms) for _ in range(args.reps)]
+        graph = capture(dev, opt.step, 1 << 20)
+        times, mhz = windows(graph.launch, args)
         elems = sum(int(np.prod(s)) for s in shapes(name))
         bpe = BYTES_PER_ELEM[args.optimizer]
         us = 1e3 * float(np.median(times))
         rows.append({"optimizer": args.optimizer, "set": name, "tensors": len(shapes(name)), "elements": elems,
                      "bytes_per_elem": bpe, "us_per_step": round(us, 2),
                      "us_min_max": [round(1e3 * min(times), 2), round(1e3 * max(times), 2)],
-                     "kernels_per_step": cap.graph.kernel_count, "GB_s": round(elems * bpe / (us * 1e-6) / 1e9, 1),
-                     "share_of_3.35_TB_s": round(elems * bpe / (us * 1e-6) / (HBM_TBPS * 1e12), 3)})
-        cap.graph.close()
+                     "kernels_per_step": graph.kernel_count, "GB_s": round(elems * bpe / (us * 1e-6) / 1e9, 1),
+                     "share_of_3.35_TB_s": round(elems * bpe / (us * 1e-6) / 1e9 / DATASHEET["hbm_gbps"], 3),
+                     "median_sm_mhz": mhz})
+        graph.close()
     return rows
 
 
@@ -136,14 +118,12 @@ def training_row(nk, dev, args):
         loss.backward(1.0)
         opt.step()
         sched.step()
-    step()
-    with dev.capture(4 << 30) as cap:
-        step()
-    times = [timed(dev, cap.graph.launch, args.window_ms) for _ in range(args.reps)]
+    graph = capture(dev, step, 4 << 30)
+    times, mhz = windows(graph.launch, args)
     row = {"optimizer": args.optimizer, "set": "mlp training step (batch 8192, MSE, StepLR)",
            "ms_per_step": round(float(np.median(times)), 4), "ms_min_max": [round(min(times), 4), round(max(times), 4)],
-           "kernels_per_step": cap.graph.kernel_count}
-    cap.graph.close()
+           "kernels_per_step": graph.kernel_count, "median_sm_mhz": mhz}
+    graph.close()
     return row
 
 
@@ -154,8 +134,8 @@ def main():
     ap.add_argument("--optimizer", default="adam", choices=sorted(BYTES_PER_ELEM))
     args = ap.parse_args()
     import neuronika_b200 as nk
-    dev = nk.Device(0)
-    info = card()
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
+    info = {"gpu": card["name"], "power_limit": card["power_limit_w"]}
     for row in optimizer_rows(nk, dev, args):
         print(json.dumps({**info, **row}), flush=True)
     print(json.dumps({**info, **training_row(nk, dev, args)}), flush=True)

@@ -29,9 +29,9 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-HBM_GBPS = 3350.0
+from measure import DATASHEET, alternate, capture, setup  # noqa: E402
+
 # name: (kind, input shape, kernel, stride, padding)  (adaptive: kernel = output size)
 CASES = {
     "maxpool2d_k3s2p1_resnet_stem": ("max", (256, 64, 112, 112), (3, 3), (2, 2), (1, 1)),
@@ -135,12 +135,7 @@ def convnet_step(nk, dev, pooled, batch=4096):
         loss.backward(1.0)
         opt.step()
 
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(24 << 30) as cap:
-        step()
-    return cap.graph
+    return capture(dev, step, 24 << 30)
 
 
 def main():
@@ -160,41 +155,31 @@ def main():
     import torch
 
     import neuronika_b200 as nk
-    from cat_bench import alternate
-    from gemm_sweep import Clock
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "hbm_datasheet_gbps": HBM_GBPS}), flush=True)
+    dev, card = setup(hbm_datasheet_gbps=DATASHEET["hbm_gbps"])
     for name, (kind, shape, k, s, p) in CASES.items():
         for dname, dt in (("bf16", torch.bfloat16), ("f32", torch.float32)):
             fwd, fb, oshape = case(nk, dev, torch, kind, shape, k, s, p, dt)
             nbytes = traffic(kind, shape, oshape, 2 if dt == torch.bfloat16 else 4)
             for direction, fns in (("forward", fwd), ("forward+backward", fb)):
-                ms, mhz = alternate(torch, fns, clock, args.window_ms, args.reps)
+                ms, mhz = alternate(fns, args.window_ms, args.reps)
                 b = {i: nbytes[i][0] + (nbytes[i][1] if direction != "forward" else 0) for i in ms}
                 gbps = {i: round(b[i] / v / 1e6, 1) for i, v in ms.items()}
                 print(json.dumps({
                     "case": name, "dtype": dname, "direction": direction, "shape": shape, "out": oshape, "bytes": b,
                     "us": {i: round(v * 1e3, 1) for i, v in ms.items()}, "gbps": gbps,
-                    "share_of_hbm": {i: round(v / HBM_GBPS, 3) for i, v in gbps.items()},
+                    "share_of_hbm": {i: round(v / DATASHEET["hbm_gbps"], 3) for i, v in gbps.items()},
                     "ours_vs_torch": round(ms["torch"] / ms["ours"], 3),
                     "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"]}), flush=True)
             del fwd, fb
             torch.cuda.empty_cache()
     graphs = {"config5_convnet": convnet_step(nk, dev, False), "config5_convnet_maxpool": convnet_step(nk, dev, True)}
-    ms, mhz = alternate(torch, {k: g.launch for k, g in graphs.items()}, clock, args.window_ms, args.reps)
+    ms, mhz = alternate({k: g.launch for k, g in graphs.items()}, args.window_ms, args.reps)
     for k, g in graphs.items():
         print(json.dumps({"case": k, "batch": 4096, "dtype": "bf16", "grad_dtype": "f32", "ms_per_step": round(ms[k], 4),
                           "kernels_per_step": g.kernel_count, "median_sm_mhz": mhz, "card": card["name"],
                           "power_limit_w": card["power_limit_w"]}), flush=True)
         g.close()
-    clock.halt.set()
 
 
 if __name__ == "__main__":

@@ -36,40 +36,15 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from gemm_sweep import Clock  # noqa: E402
+from measure import alternate, capture, setup, window  # noqa: E402
 
 T = 32
 SHAPES = [(256, 1024, 1024), (1024, 2048, 2048)]
-
-
-def timed(torch, fn, clock, window_ms, reps):
-    """median ms per call over `reps` windows of back-to-back calls, and the median SM clock meanwhile"""
-    for _ in range(2):
-        fn()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    iters = int(min(2000, max(3, window_ms / ((time.perf_counter() - t0) * 1e3))))
-    clock.armed.set()
-    per = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            fn()
-        e1.record()
-        e1.synchronize()
-        per.append(e0.elapsed_time(e1) / iters)
-    clock.armed.clear()
-    return float(np.median(per)), clock.take()
 
 
 def composed_cell(kind, cell, state, x, n, hidden):
@@ -124,12 +99,7 @@ def graph_step(nk, dev, kind, n, n_in, hidden, variant):
         loss.backward(1.0)
         opt.step()
 
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(8 << 30) as cap:
-        step()
-    return cap.graph
+    return capture(dev, step, 8 << 30)
 
 
 def torch_step(torch, kind, n, n_in, hidden):
@@ -196,25 +166,16 @@ def stacked_step(nk, dev, kind, n, n_in, hidden, layers, bidirectional):
         loss.backward(1.0)
         opt.step()
 
-    step()
-    step()
-    dev.synchronize()
-    with dev.capture(12 << 30) as cap:   # the GRU's 2 layers x 2 directions at N = 1024, H = 2048 take ~9 GiB
-        step()
-    return cap.graph
+    return capture(dev, step, 12 << 30)   # the GRU's 2 layers x 2 directions at N = 1024, H = 2048 take ~9 GiB
 
 
-def stacked_row(nk, dev, torch, clock, args, card, kind, n, n_in, hidden):
+def stacked_row(nk, dev, torch, args, card, kind, n, n_in, hidden):
     graphs = {name: stacked_step(nk, dev, kind, n, n_in, hidden, layers, bi) for name, layers, bi in STACKED}
     cudnn = {name: torch_cudnn_step(torch, kind, n, n_in, hidden, layers, bi) for name, layers, bi in STACKED}
-    res, mhz = {}, []
-    for _ in range(args.reps):      # alternating, one window each
-        for name, _, _ in STACKED:
-            for key, fn in ((name, graphs[name].launch), (name + "_torch_cudnn_bf16", cudnn[name])):
-                ms, m = timed(torch, fn, clock, args.window_ms, 1)
-                res.setdefault(key, []).append(ms)
-                mhz.append(m)
-    med = {k: float(np.median(v)) for k, v in res.items()}
+    fns = {}
+    for name, _, _ in STACKED:
+        fns[name], fns[name + "_torch_cudnn_bf16"] = graphs[name].launch, cudnn[name]
+    med, mhz = alternate(fns, args.window_ms, args.reps)
     print(json.dumps({
         "cell": kind, "variant": "stacked", "N": n, "I": n_in, "H": hidden, "T": T,
         "ms_per_sequence": {k: round(v, 3) for k, v in med.items()},
@@ -222,7 +183,7 @@ def stacked_row(nk, dev, torch, clock, args, card, kind, n, n_in, hidden):
         "bidirectional_over_2x_unidirectional": round(med["bidirectional"] / (2 * med["unidirectional"]), 3),
         "speedup_vs_torch_cudnn_bf16": {name: round(med[name + "_torch_cudnn_bf16"] / med[name], 2)
                                         for name, _, _ in STACKED},
-        "median_sm_mhz": float(np.median(mhz)), "card": card["name"], "power_limit_w": card["power_limit_w"],
+        "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"],
     }), flush=True)
     for g in graphs.values():
         g.close()
@@ -304,41 +265,27 @@ def main():
 
     import neuronika_b200 as nk
 
-    torch.cuda.set_device(0)
-    stream = torch.cuda.Stream()        # a created stream: the legacy default stream cannot be captured
-    torch.cuda.set_stream(stream)
-    dev = nk.Device(0, stream=stream.cuda_stream)
-    clock = Clock(0)
-    clock.start()
-    card = clock.card()
-    print(json.dumps({"card": card, "sm_count": dev.sm_count, "T": T}), flush=True)
+    dev, card = setup(T=T)
     for kind in ("lstm", "gru"):
         for n, n_in, hidden in SHAPES:
             if args.stacked_only:
-                stacked_row(nk, dev, torch, clock, args, card, kind, n, n_in, hidden)
+                stacked_row(nk, dev, torch, args, card, kind, n, n_in, hidden)
                 continue
             fused = graph_step(nk, dev, kind, n, n_in, hidden, "fused")
             comp = graph_step(nk, dev, kind, n, n_in, hidden, "composed")
             seq = graph_step(nk, dev, kind, n, n_in, hidden, "sequence")
             teager = torch_step(torch, kind, n, n_in, hidden)
             tcudnn = torch_cudnn_step(torch, kind, n, n_in, hidden)
-            res = {"fused": [], "composed": [], "sequence": [], "torch_eager_bf16": [], "torch_cudnn_bf16": []}
-            mhz = []
-            for _ in range(args.reps):      # alternating, one window each
-                for name, fn in (("fused", fused.launch), ("composed", comp.launch), ("sequence", seq.launch),
-                                 ("torch_eager_bf16", teager), ("torch_cudnn_bf16", tcudnn)):
-                    ms, m = timed(torch, fn, clock, args.window_ms, 1)
-                    res[name].append(ms)
-                    mhz.append(m)
+            med, mhz = alternate({"fused": fused.launch, "composed": comp.launch, "sequence": seq.launch,
+                                  "torch_eager_bf16": teager, "torch_cudnn_bf16": tcudnn}, args.window_ms, args.reps)
             gem, flops = gemm_only(nk, dev, torch, kind, n, n_in, hidden)
-            gms, _ = timed(torch, gem, clock, args.window_ms / 4, args.reps)
+            gms, _ = window(gem, args.window_ms / 4, args.reps)
             whole, sequential = sequence_gemms(nk, dev, kind, n, n_in, hidden)
-            wms, _ = timed(torch, whole, clock, args.window_ms / 4, args.reps)
-            sms, _ = timed(torch, sequential, clock, args.window_ms / 4, args.reps)
+            wms, _ = window(whole, args.window_ms / 4, args.reps)
+            sms, _ = window(sequential, args.window_ms / 4, args.reps)
             fwd, fb, bwd, bb = gate_kernels(nk, dev, kind, n, hidden)
-            fms, _ = timed(torch, fwd, clock, args.window_ms / 4, args.reps)
-            bms, _ = timed(torch, bwd, clock, args.window_ms / 4, args.reps)
-            med = {k: float(np.median(v)) for k, v in res.items()}
+            fms, _ = window(fwd, args.window_ms / 4, args.reps)
+            bms, _ = window(bwd, args.window_ms / 4, args.reps)
             print(json.dumps({
                 "cell": kind, "N": n, "I": n_in, "H": hidden, "T": T,
                 "ms_per_sequence": {k: round(v, 3) for k, v in med.items()},
@@ -358,13 +305,12 @@ def main():
                 "gemm_share_of_fused_step": round(gms * T / med["fused"], 3),
                 "gate_fwd_us": round(fms * 1e3, 2), "gate_fwd_gbps": round(fb / fms / 1e6, 1),
                 "gate_bwd_us": round(bms * 1e3, 2), "gate_bwd_gbps": round(bb / bms / 1e6, 1),
-                "median_sm_mhz": float(np.median(mhz)), "card": card["name"], "power_limit_w": card["power_limit_w"],
+                "median_sm_mhz": mhz, "card": card["name"], "power_limit_w": card["power_limit_w"],
             }), flush=True)
             fused.close()
             comp.close()
             seq.close()
-            stacked_row(nk, dev, torch, clock, args, card, kind, n, n_in, hidden)
-    clock.halt.set()
+            stacked_row(nk, dev, torch, args, card, kind, n, n_in, hidden)
 
 
 if __name__ == "__main__":
